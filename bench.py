@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — differentiable world-steps/s (fwd+bwd) of the batched Atlas timestep.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch B]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch B] [--dump-outputs DIR]
   torchrun --nproc-per-node N bench.py --gpus N ...         (one rank per GPU; batch shards, no data-path collective)
 
 Headline workload (BASELINE.json configs[1]): Atlas humanoid (33 DoF, 28 moving bodies), contact-free, batch 4096 per GPU,
@@ -29,6 +29,7 @@ sys.path.insert(0, ROOT)
 
 ATLAS = os.path.join(ROOT, "tests", "golden", "models", "atlas.json")
 METRIC = "differentiable world-steps/sec (fwd+bwd), batched Atlas"
+HBM_PEAK_GBS = 3350.0  # H100 SXM data sheet: the denominator of the roofline fractions, not a measured figure
 UNIT = "world-steps/s"
 
 
@@ -49,8 +50,19 @@ def make_inputs(raw, B, seed):
     return (np.concatenate([q, v], 1).astype(np.float32), a.astype(np.float32), g.astype(np.float32))
 
 
+def gpu_info(gpu_index):
+    """Name, power limit and maximum SM clock of the card: an absolute number is only meaningful next to these."""
+    try:
+        out = subprocess.run(["nvidia-smi", f"--id={gpu_index}", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        name, power, mhz = [x.strip() for x in out.split(",")]
+        return {"name": name, "power_limit_w": float(power), "sm_max_mhz": float(mhz)}
+    except Exception:
+        return None
+
+
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons during the timed region."""
 
     def __init__(self, gpu_index):
         super().__init__(daemon=True)
@@ -78,6 +90,7 @@ class ClockSampler(threading.Thread):
         if self.proc:
             try:
                 self.proc.terminate()
+                self.proc.wait(timeout=10)
             except Exception:
                 pass
         sm, mx, reasons = [], [], set()
@@ -143,7 +156,7 @@ def bind_to_gpu_numa(local_rank):
 
 
 def probe_reference():
-    """BASELINE.md §3 step 1: is the real reference importable (a driver-provided install under baseline/_ref/ or site-packages)?
+    """BASELINE.md §3 step 1: is the real reference importable (an install under baseline/_ref/ or in site-packages)?
     Returns the module or None.  It cannot be built in the authoring container (needs Eigen, ccd, assimp, boost, ...)."""
     ref_dir = os.path.join(ROOT, "baseline", "_ref")
     if os.path.isdir(ref_dir) and ref_dir not in sys.path:
@@ -334,22 +347,15 @@ def contact_leg(nb, torch, name, B, K, W, dev, dist, rank, world_size, peak, cpu
     value = B * world_size * K / (ms * 1e-3)
     alg = ALG_BYTES[name]
     achieved = (value / world_size) * alg / 1e9
-    traffic = None
-    if name == "atlas_ground" and B == 8192:  # the ncu capture behind profiles/dram_traffic.json is this workload at this batch (sum of the 5 kernels of a step)
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "dram_traffic.json")))
-            traffic = float(sum(tj[k] for k in ("k_cbuild", "k_csolve<0>", "k_csolve<1>", "k_capply", "k_cstep_bwd")))
-        except Exception:
-            traffic = None
     n, na = raw.ndof, len(raw.action_map)
     leg = {"workload": f"{name}: fwd+bwd step with the contact / boxed-LCP stage, batch={B}/GPU, fresh states (x_t+1 = step(x_t), LCP cache flowing)",
            "value": value, "unit": UNIT, "n_gpus": world_size, "steps": K, "warmup": W, "ms_per_step": ms / K,
            "sustained": {"value": B * world_size * n_sus / (sus_ms * 1e-3), "steps": n_sus, "timed_region_s": sus_ms * 1e-3},
            "kernel_ms": {"forward (build + solve x2 + apply)": float(np.mean([a_.elapsed_time(b_) for a_, b_ in fwd_ms])),
                          "backward (k_cstep_bwd)": float(np.mean([a_.elapsed_time(b_) for a_, b_ in bwd_ms]))},
-           "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+           "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                         "algorithmic_bytes_per_world_step": alg, "algorithmic_bytes_per_step": alg * B,
-                        "note": "latency / instruction-issue bound fp64 kernels (profiles/r02_*): the HBM fraction is reported as asked"},
+                        "note": "latency / instruction-issue bound fp64 kernels: the HBM fraction is reported as asked"},
            "e2e": {"value": B * world_size * e2e_steps / (e2e_ms * 1e-3), "unit": UNIT, "steps": e2e_steps,
                    "h2d_bytes_per_step": int(4 * B * (2 * n + na + 2 * n)), "d2h_bytes_per_step": int(4 * B * (2 * n + 2 * n + na)),
                    "path": "nimblephysics_b200.timestep() with pinned host tensors (copies inside the timed region)"},
@@ -440,7 +446,11 @@ def main():
     ap.add_argument("--precision", default="fp32", choices=["fp32", "fp64"])
     ap.add_argument("--lanes", type=int, default=0, help="threads cooperating on one world (0 = library picks from the batch size)")
     ap.add_argument("--no-extra", action="store_true", help="skip the cpu_baseline / e2e-independent extra contact legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (next state, state and action gradients) to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
 
     rank = int(os.environ.get("RANK", "0"))
     world_size = int(os.environ.get("WORLD_SIZE", "1"))
@@ -455,7 +465,7 @@ def main():
     config = {"workload": "Atlas (atlas_v3 URDF, 33 DoF, 28 moving bodies) contact-free Featherstone step fwd+bwd, "
                           f"batch={args.batch}/GPU, dt=1e-3, y-up gravity (BASELINE configs[1])",
               "global_batch": args.batch * max(world_size, 1), "parallelism": f"batch-sharded x{max(world_size,1)} (no data-path collective)",
-              "l2_policy": "rotating buffer sets > L2 (126 MB)", "precision_inside_kernels": args.precision}
+              "l2_policy": "rotating buffer sets > L2 (50 MB on H100)", "precision_inside_kernels": args.precision}
 
     # ------------------------------------------------------------------ reference arm (CPU)
     if args.impl == "reference":
@@ -570,6 +580,7 @@ def main():
     for i in range(args.warmup):
         fwd(sets[i % nsets]); bwd(sets[i % nsets])
     barrier()
+    gpu = gpu_info(local_rank)
     sampler = ClockSampler(local_rank)
     sampler.start()
     # keep the GPU busy (untimed) while the clock sampler starts: an idle gap right before a timed region of a few milliseconds would make it
@@ -592,6 +603,13 @@ def main():
     barrier()
     launches = _cabi.lib().nb2_launch_count() - l0
     total_ms = t0.elapsed_time(t1)
+    if args.dump_outputs and rank == 0:  # before the passes below reuse the buffers
+        d = sets[(args.warmup + args.steps - 1) % nsets]
+        keep = min(B, (64 << 20) // (4 * (4 * n + na)))  # all worlds, or a fixed seeded sample of them that fits in 64 MB
+        rows = torch.arange(B, device=dev) if keep == B else torch.tensor(np.sort(np.random.default_rng(0).choice(B, keep, replace=False)), device=dev)
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, key in (("next_state", "nxt"), ("grad_state", "gs"), ("grad_action", "ga")):
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), d[key][rows].cpu().numpy())
     # per-kernel times from a separate instrumented pass (an event after every launch), outside the timed region
     ne = min(args.steps, 50)
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(2 * ne + 1)]
@@ -643,14 +661,9 @@ def main():
     if numa is not None:
         extra["numa_binding"] = numa
     if not args.no_extra:
-        peak_hbm = 6650.0
-        try:
-            peak_hbm = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("hbm_gbs", peak_hbm))
-        except Exception:
-            pass
         for cname, cB, label in (("half_cheetah", 4096, "half_cheetah_ground_fwd_bwd (configs[2])"), ("atlas_ground", 8192, "atlas_ground_fwd_bwd (configs[3])")):
             try:
-                extra["legs"][label] = contact_leg(nb, torch, cname, cB, max(args.steps, 8), max(args.warmup, 3), dev, dist, rank, world_size, peak_hbm,
+                extra["legs"][label] = contact_leg(nb, torch, cname, cB, args.steps, max(args.warmup, 3), dev, dist, rank, world_size, HBM_PEAK_GBS,
                                                    cpu_contact.get(cname))
             except Exception as ex:  # never let a leg break the headline line
                 extra["legs"][label] = {"error": repr(ex)}
@@ -700,34 +713,23 @@ def main():
     e2e_value = B * world_size * e2e_steps / (e2e_ms * 1e-3)
 
     if rank == 0:
-        peaks = {}
-        try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        except Exception:
-            pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
+        peak = HBM_PEAK_GBS
         dom, dom_ms, dom_bytes = ("k_step_bwd", bwd_ms, bytes_bwd) if bwd_ms >= fwd_ms else ("k_step_fwd", fwd_ms, bytes_fwd)
         achieved = dom_bytes * B / (dom_ms * 1e-3) / 1e9
-        traffic = None
-        try:
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "dram_traffic.json"))).get(dom)
-        except Exception:
-            pass
         out = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world_size, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": total_ms / args.steps, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "f32" if prec == FP32 else "f64", "data": "synthetic", "config": config,
             "kernel_ms": {"k_step_fwd": fwd_ms, "k_step_bwd": bwd_ms, "note": "separate instrumented pass with an event after every launch (about +3 us per launch); the timed region has two events"}, "lanes_per_world": lanes_used,
             "roofline": {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": traffic,
-                         "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6650 GB/s",
+                         "frac": achieved / peak, "peak_source": "H100 SXM data sheet (3.35 TB/s), not measured",
                          "algorithmic_bytes_per_world": {"k_step_fwd": bytes_fwd, "k_step_bwd": bytes_bwd, "step": bytes_fwd + bytes_bwd},
                          "note": "path is FP32-latency bound, not HBM bound (DESIGN.md §roofline): the HBM fraction is reported as asked"},
             "e2e": {"value": e2e_value, "unit": UNIT,
                     "h2d_bytes_per_step": int(4 * B * (2 * n + na + 2 * n)), "d2h_bytes_per_step": int(4 * B * (2 * n + 2 * n + na)),
                     "steps": e2e_steps, "path": "nb2_step_forward_host + nb2_step_backward_host (pinned host buffers)"},
             "sustained": {"value": B * world_size * n_sus / (sus_ms * 1e-3), "steps": n_sus, "timed_region_s": sus_ms * 1e-3},
-            "gpu_launches": int(launches), "clocks": clocks, "extra": extra,
+            "gpu_launches": int(launches), "gpu": gpu, "clocks": clocks, "extra": extra,
         }
         if cpu_baseline is not None:
             out["cpu_baseline"] = cpu_baseline

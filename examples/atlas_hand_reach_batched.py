@@ -5,7 +5,7 @@ ground, towards a goal point — B worlds with B different goals at once, everyt
     IKMapping          ikMap.addLinearBodyNode(l_hand) + map_to_pos: the task-space loss and its gradient never leave the device
     torch.optim.Adam   on the open-loop joint torques (the reference hands the same problem to IPOPT through MultiShot)
 
-Run on a B200:  python examples/atlas_hand_reach_batched.py [B] [T] [iterations]"""
+Run on an H100:  python examples/atlas_hand_reach_batched.py [B] [T] [iterations]"""
 import os
 import sys
 

@@ -1,4 +1,4 @@
-"""The reference's python/new_examples/cartpole.py, batched: 4096 cartpoles swing up in parallel on one B200.
+"""The reference's python/new_examples/cartpole.py, batched: 4096 cartpoles swing up in parallel on one H100.
 
 Same builder calls, same `timestep(world, state, action)` — `state` / `action` are [B, 2n] / [B, a] CUDA tensors and the
 whole horizon is differentiated on the device (nimblephysics_b200.rollout_fused: one C-ABI call per direction).

@@ -1,4 +1,4 @@
-/* nb2.h — C ABI of the B200 batched differentiable-timestep engine (libnb2.so).
+/* nb2.h — C ABI of the H100 batched differentiable-timestep engine (libnb2.so).
  *
  * Drop-in boundary for the reference's hot path.  What each entry point replaces:
  *   nb2_step_forward   <- neural::forwardPass(world)            dart/neural/NeuralUtils.cpp:26-66

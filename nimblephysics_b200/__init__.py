@@ -1,4 +1,4 @@
-"""nimblephysics_b200 — B200-native batched differentiable timestep behind the
+"""nimblephysics_b200 — H100-native batched differentiable timestep behind the
 Nimble ``timestep(world, state, action)`` surface.  See DESIGN.md."""
 from . import world as _world
 from .world import (World, Skeleton, BodyNode, Joint, Isometry3, BoxShape, SphereShape, CapsuleShape)

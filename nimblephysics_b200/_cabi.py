@@ -133,7 +133,7 @@ def lib() -> ctypes.CDLL:
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise Nb2Error(f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                           "(nvcc, sm_100a). nimblephysics_b200 has no CPU fallback.")
+                           "(nvcc, sm_90a). nimblephysics_b200 has no CPU fallback.")
         L = ctypes.CDLL(LIB_PATH)
         L.nb2_last_error.restype = ctypes.c_char_p
         L.nb2_version.restype = ctypes.c_char_p

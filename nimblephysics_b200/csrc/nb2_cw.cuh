@@ -94,8 +94,8 @@ namespace cw {
 #define CW_LANE ((int)(threadIdx.x & 31))
 #define CW_SYNC() __syncwarp()
 // NB2_CW_FOR_UNIFORM: the loop over passes gets a warp-uniform trip count and only the body is predicated.  In isolation a divergent loop
-// exit costs ~110 cycles on B200 against ~60 for this form (scripts/dev/ubench/br.cu); inside the real kernels the plain per-lane loop
-// measured 10 % FASTER (the compiler turns the guarded bodies into divergent branches anyway), so it is the default.
+// exit costs more than this form (scripts/dev/ubench/br.cu measures both); inside the real kernels the compiler turns the guarded bodies
+// into divergent branches anyway, so the plain per-lane loop is the default.
 #ifndef NB2_CW_FOR_UNIFORM
 #define CW_FOR(i, n) for (int i = (int)(threadIdx.x & 31); i < (n); i += 32)
 #else

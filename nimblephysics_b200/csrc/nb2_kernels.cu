@@ -1,4 +1,4 @@
-// libnb2.so — kernels + C ABI (include/nb2.h).  sm_100a only.
+// libnb2.so — kernels + C ABI (include/nb2.h).  sm_90a only.
 //
 // Kernel shape (contact-free step): ONE THREAD PER WORLD, 32 worlds per warp.  The model is a __grid_constant__
 // kernel parameter (constant-bank, warp-uniform loads); per-world working storage lives in dynamic shared memory,
@@ -316,8 +316,7 @@ k_cbuild(const __grid_constant__ Nb2ModelDev<double> M, const __grid_constant__ 
   if (live) nb2::fwd_store<double, 1>(M, scr, next + (size_t)w * 2 * M.ndof, 1, lane, 32);  // [q+ ; v*]: the apply kernel replaces v* by v+ where there are contacts
 }
 // Several worlds per block (one warp each): the warps run the phases of the chain in LOCKSTEP (CW_PHASE = __syncthreads), so that the
-// SM fetches each piece of code once for all of them.  Measured on B200 (Atlas + ground, 8192 worlds): 6.6 -> 3.7 ms per forward step
-// going from 1 to 11 worlds per block.  The warp count per block is chosen at launch (shared memory, batch size).
+// SM fetches each piece of code once for all of them.  The warp count per block is chosen at launch (shared memory, batch size).
 #define NB2_CSOLVE_MAXW 12
 // solve kernel A (every world: warm start + short-circuit classification) / B (the worlds A listed in `todo`: the rest of the chain)
 template <int PART>
@@ -959,7 +958,7 @@ template <class Kern> static int cstep_smem_attr(Kern kern, size_t smem, bool* d
 extern "C" {
 
 const char* nb2_last_error(void) { return g_err.c_str(); }
-const char* nb2_version(void) { return "nb2 0.2 (sm_100a; cooperative-lane ABA + adjoint, warp-per-world contact / boxed-LCP stage)"; }
+const char* nb2_version(void) { return "nb2 0.2 (sm_90a; cooperative-lane ABA + adjoint, warp-per-world contact / boxed-LCP stage)"; }
 long long nb2_launch_count(void) { return g_launches.load(); }
 
 int nb2_model_create(const nb2_model_desc* desc, nb2_model** out) {

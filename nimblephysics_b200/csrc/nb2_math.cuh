@@ -36,9 +36,9 @@ NB2_HD void nb2_sincos(float x, float* s, float* c) {
 }
 NB2_HD void nb2_sincos(double x, double* s, double* c) { sincos(x, s, c); }
 NB2_HD float nb2_sqrt(float x) { return sqrtf(x); }
-// fp64 division / square root are ~40-instruction dependent sequences on the GPU (measured on B200: ~375 cycles for a dependent
-// division against 8 for a multiply-add).  The hot paths use a seed from the special-function unit refined by two Newton steps
-// (~1 ulp, ~80 cycles); arguments outside the comfortable exponent range take the IEEE routine.
+// fp64 division / square root are ~40-instruction dependent sequences on the GPU (scripts/dev/ubench/lat.cu measures their latency
+// against a multiply-add).  The hot paths use a seed from the special-function unit refined by two Newton steps (~1 ulp);
+// arguments outside the comfortable exponent range take the IEEE routine.
 NB2_HD double nb2_rcp(double b) {
 #ifdef __CUDA_ARCH__
   const unsigned ex = ((unsigned)__double2hiint(b) >> 20) & 0x7ffu;

@@ -27,7 +27,7 @@ def step_jacobians(world, state: torch.Tensor, action: torch.Tensor) -> Tuple[to
     if state.dim() != 2 or state.shape[1] != n2 or action.shape != (state.shape[0], na):
         raise ValueError(f"step_jacobians(): state {tuple(state.shape)} / action {tuple(action.shape)} do not match [B,{n2}] / [B,{na}]")
     if not state.is_cuda:
-        raise RuntimeError("step_jacobians needs CUDA tensors (B200); there is no CPU fallback")
+        raise RuntimeError("step_jacobians needs CUDA tensors; there is no CPU fallback")
     B = state.shape[0]
     s = state.detach().to(torch.float32).repeat_interleave(n2, dim=0).requires_grad_(True)
     a = action.detach().to(device=state.device, dtype=torch.float32).repeat_interleave(n2, dim=0).requires_grad_(True)

@@ -141,7 +141,7 @@ class _MapLayer(torch.autograd.Function):
         legacy = state.dim() == 1
         s2 = state.detach().reshape(-1, n2)
         if not torch.cuda.is_available():
-            raise RuntimeError("nimblephysics_b200.mapping needs a CUDA device (B200); there is no CPU fallback")
+            raise RuntimeError("nimblephysics_b200.mapping needs a CUDA device; there is no CPU fallback")
         dev = s2.device if s2.is_cuda else torch.device("cuda", torch.cuda.current_device())
         sd = s2.to(device=dev, dtype=torch.float32).contiguous()
         B, dim = sd.shape[0], mapping.getPosDim()

@@ -87,7 +87,7 @@ class _ContactRollout(torch.autograd.Function):
         if state0.shape != (B, n2) or actions.shape[2] != na:
             raise ValueError(f"rollout(): state0 {tuple(state0.shape)} / actions {tuple(actions.shape)} do not match [B,{n2}] / [T,B,{na}]")
         if not state0.is_cuda:
-            raise RuntimeError("rollout_fused needs CUDA tensors (B200); there is no CPU fallback")
+            raise RuntimeError("rollout_fused needs CUDA tensors; there is no CPU fallback")
         dev = state0.device
         states = torch.empty((T + 1, B, n2), dtype=torch.float32, device=dev)
         states[0].copy_(state0.detach())

@@ -55,7 +55,7 @@ class TimestepLayer(torch.autograd.Function):
         if a2.dim() != 2 or a2.shape[1] != na or a2.shape[0] != s2.shape[0]:
             raise ValueError(f"timestep(): action has shape {tuple(action.shape)}, expected [{s2.shape[0]}, {na}] (= getActionSize())")
         if not torch.cuda.is_available():
-            raise RuntimeError("nimblephysics_b200.timestep needs a CUDA device (B200); there is no CPU fallback")
+            raise RuntimeError("nimblephysics_b200.timestep needs a CUDA device; there is no CPU fallback")
         dev = s2.device if s2.is_cuda else torch.device("cuda", torch.cuda.current_device())
         sd = s2.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
         ad = a2.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()

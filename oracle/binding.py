@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE ONLY — ctypes binding of oracle/liboracle.so (fp64 restatement) and, when present,
-oracle/_ref/libodelcp.so (the reference's own ODE LCP solver compiled from /root/reference).
+oracle/_ref/libodelcp.so (the reference's own ODE LCP solver, `make -C oracle REF=<nimblephysics tree>`).
 May be imported only by tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs."""
 import ctypes
 import os
@@ -206,7 +206,7 @@ _REF = None
 
 
 def ref_ode():
-    """The reference's own dSolveLCP (compiled from /root/reference by oracle/Makefile) or None."""
+    """The reference's own dSolveLCP (compiled from a nimblephysics tree by oracle/Makefile) or None."""
     global _REF
     if _REF is None:
         path = os.path.join(_HERE, "_ref", "libodelcp.so")

@@ -2,8 +2,8 @@
 //   dSolveLCP   dart/external/odelcpsolver/lcp.cpp:780-1114   (driver loop, ratio test, cmd 1..6)
 //   dLCP        lcp.cpp:362-775 (index sets C / N kept contiguous by physically permuting the problem, friction rows moved to the
 //               end :491-501, lo/hi of friction rows fixed when the first one is reached :856-873)
-// Pinned against the REAL reference code: tests/test_lcp.py compares it with dSolveLCP compiled from /root/reference
-// (oracle/_ref/libodelcp.so) on random and literal LCP instances.  The product has its OWN, warp-cooperative implementation
+// Pinned against the REAL reference code: tests/test_lcp.py compares it with dSolveLCP (oracle/_ref/libodelcp.so, or
+// its answers recorded in tests/golden/dantzig_seeded.npz) on random and literal LCP instances.  The product has its OWN, warp-cooperative implementation
 // (nimblephysics_b200/csrc/nb2_cw.cuh dantzig_solve) which is compared against this one through the solve chain — the two share
 // no code.  Dense linear algebra: full symmetric A, L D L^T of A[C,C] appended row by row, rebuilt when an index leaves C.
 #pragma once

@@ -6,7 +6,7 @@
 //   ConstrainedGroupGradientMatrices::{constructMatrices, opportunisticallyStandardizeResults}
 //                                             dart/neural/ConstrainedGroupGradientMatrices.cpp:482-872, 218-339
 //   Dantzig: oracle/dantzig_serial.hpp (serial restatement, pinned against the reference's own dSolveLCP, tests/test_lcp.py)
-// Eigen's completeOrthogonalDecomposition().solve (third-party, not under /root/reference) is restated as the
+// Eigen's completeOrthogonalDecomposition().solve (third-party, not part of the reference) is restated as the
 // minimum-norm least-squares solution computed from a one-sided Jacobi SVD with Eigen's default rank threshold
 // (eps * max(rows, cols) relative to the largest singular value / pivot).
 #pragma once

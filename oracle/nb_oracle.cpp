@@ -19,7 +19,7 @@
 // Parity status: the reference cannot be built in this container (Eigen/ccd/assimp absent).  What its test-suite holds as literal
 // vectors for this path IS pinned: the 8 LCP instances of unittests/unit/test_LCPUtils.cpp (tests/test_lcp.py) and the contact sets of
 // unittests/unit/test_DARTCollide.cpp (box-box face-face annotation, sphere / capsule-end vs box: tests/test_golden_collide.py); the LCP
-// stage is bit-compared with the reference's ODE dSolveLCP compiled from /root/reference (oracle/Makefile -> oracle/_ref/libodelcp.so).
+// stage is bit-compared with the reference's ODE dSolveLCP compiled from a reference tree (oracle/Makefile -> oracle/_ref/libodelcp.so).
 // For the dynamics and the gradients the reference ships property tests only (analytic-vs-FD, unittests/GradientTestUtils.hpp): there
 // value-level parity is UNPINNED and the oracle is held by the same properties (tests/test_oracle.py).
 //

@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE ONLY.  C-linkage shim around the reference's own ODE Dantzig solver so tests can call it
-// through ctypes.  Compiled together with the sources under /root/reference/dart/external/odelcpsolver/ (never
+// through ctypes.  Compiled together with the sources under <REF>/dart/external/odelcpsolver/ (never
 // copied) into oracle/_ref/libodelcp.so by oracle/Makefile.
 //   reference: dart/external/odelcpsolver/lcp.h:60 (dSolveLCP), common.h:141 (dPAD)
 #include "dart/external/odelcpsolver/lcp.h"

@@ -1,11 +1,12 @@
 """Lifts the literal boxed-LCP instances (A, x, lo, hi, b, fIndex) that the reference's own unit tests hold
 (unittests/unit/test_LCPUtils.cpp, captured from real solver failures) into tests/golden/lcp_fixtures.json.
-Run in the build container only:  python tests/golden/make_lcp_fixtures.py"""
+Needs a nimblephysics source tree:  NB2_REFERENCE=<nimblephysics> python tests/golden/make_lcp_fixtures.py"""
 import json
 import os
 import re
+import sys
 
-SRC = os.environ.get("NB2_REFERENCE", "/root/reference") + "/unittests/unit/test_LCPUtils.cpp"
+SRC = (os.environ.get("NB2_REFERENCE") or sys.exit("set NB2_REFERENCE to a nimblephysics source tree")) + "/unittests/unit/test_LCPUtils.cpp"
 OUT = os.path.join(os.path.dirname(__file__), "lcp_fixtures.json")
 
 

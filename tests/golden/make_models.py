@@ -1,6 +1,6 @@
 """Generates tests/golden/models/*.json (flattened RawModel fixtures) from the reference's data files.
-Run in the build container only (needs /root/reference); the JSON fixtures travel to the GPU box.
-  python tests/golden/make_models.py
+Needs a nimblephysics source tree; the JSON fixtures are committed, so tests never need it.
+  NB2_REFERENCE_DATA=<nimblephysics>/data python tests/golden/make_models.py
 Sources (read-only inputs, SURVEY §8c): data/urdf/cartpole.urdf, data/skel/half_cheetah.skel,
 data/sdf/atlas/atlas_v3_box_colliders.urdf, data/sdf/atlas/ground.urdf, data/sdf/atlas/atlas_v3_no_head.sdf."""
 import os
@@ -9,7 +9,7 @@ import sys
 sys.path.insert(0, os.path.join(os.path.dirname(__file__), "..", ".."))
 import nimblephysics_b200 as nb  # noqa: E402
 
-REF = os.environ.get("NB2_REFERENCE_DATA", "/root/reference/data")
+REF = os.environ.get("NB2_REFERENCE_DATA") or sys.exit("set NB2_REFERENCE_DATA to the data/ directory of a nimblephysics source tree")
 OUT = os.path.join(os.path.dirname(__file__), "models")
 
 

@@ -1,6 +1,6 @@
-"""The DEVICE boxed-LCP code (csrc/nb2_cw.cuh through the C ABI nb2_lcp_solve_batch) against the REFERENCE's own solver binary
-(oracle/_ref/libodelcp.so = dart/external/odelcpsolver compiled from /root/reference; it travels to the GPU box prebuilt) and the
-literal instances of unittests/unit/test_LCPUtils.cpp — no restatement in between for the Dantzig comparison."""
+"""The DEVICE boxed-LCP code (csrc/nb2_cw.cuh through the C ABI nb2_lcp_solve_batch) against the REFERENCE's own solver
+(dart/external/odelcpsolver's dSolveLCP: the live oracle/_ref/libodelcp.so when it has been built, else the record in
+tests/golden/dantzig_seeded.npz, whose `source` names the solver that answered; see tests/test_lcp.py::reference_dantzig) and the literal instances of unittests/unit/test_LCPUtils.cpp."""
 import json
 import os
 
@@ -10,7 +10,7 @@ import torch
 
 import nimblephysics_b200 as nb
 from oracle import binding as ob
-from tests.test_lcp import _contact_lcp, _with_duplicate_contacts
+from tests.test_lcp import _contact_lcp, _with_duplicate_contacts, dantzig_problems, reference_dantzig
 from tests.util import ROOT
 
 pytestmark = pytest.mark.gpu
@@ -27,17 +27,14 @@ def _pack(problems, mcap):
     return t(A), t(b), t(lo), t(hi), t(fi), t(m)
 
 
-@pytest.mark.skipif(ob.ref_ode() is None, reason="oracle/_ref/libodelcp.so not present (built where /root/reference exists)")
 @pytest.mark.parametrize("early", [True, False])
 def test_device_dantzig_matches_reference_dSolveLCP(oracle_mod, early):
     """300 random contact LCPs (1..8 contacts, regularised like a cfm'd A): same success flag, x within 1e-7."""
-    rng = np.random.default_rng(1)
-    probs = [_contact_lcp(rng, int(rng.integers(1, 9)), 1e-6) for _ in range(300)]
+    probs = dantzig_problems("regularised")
     A, b, lo, hi, fi, m = _pack(probs, 24)
     x, st = nb.solve_boxed_lcp_batch(A, b, lo, hi, fi, m, chain=False, early_termination=early)
     x, st = x.cpu().numpy(), st.cpu().numpy()
-    for k, (Ak, bk, lok, hik, fik) in enumerate(probs):
-        xr, okr = ob.ref_dsolve_lcp(Ak, bk, lok, hik, fik, early)
+    for k, (bk, (xr, okr)) in enumerate(zip((p[1] for p in probs), reference_dantzig("regularised", early))):
         assert bool(okr) == (st[k] == 1), (k, okr, st[k])
         if okr:
             assert np.abs(xr - x[k, : len(bk)]).max() <= 1e-7 * max(1.0, np.abs(xr).max()), k

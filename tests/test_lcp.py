@@ -1,11 +1,14 @@
 """LCP stage of the oracle, pinned against the real reference code and the reference's literal instances.
   * oracle/dantzig_serial.hpp (the ORACLE's serial Dantzig restatement; the CUDA library has its own warp-cooperative one) vs the
-    reference's own dSolveLCP compiled from /root/reference/dart/external/odelcpsolver (oracle/_ref/libodelcp.so);
+    reference's own dSolveLCP from dart/external/odelcpsolver: the live library oracle/_ref/libodelcp.so when it has been built
+    (oracle/Makefile, REF=<nimblephysics tree>), else the record in tests/golden/dantzig_seeded.npz (its `source` names the solver
+    that answered: dSolveLCP, or this restatement as it stood when it last matched dSolveLCP);
   * the product's chain (csrc/nb2_cw.cuh, host build) vs the oracle's chain, and — on the GPU, tests/test_gpu_lcp.py — the DEVICE chain
     directly vs the reference's dSolveLCP;
   * the literal (A, x, lo, hi, b, fIndex) instances of unittests/unit/test_LCPUtils.cpp (tests/golden/lcp_fixtures.json):
     the chain's answer must satisfy LCPUtils::isLCPSolutionValid, as the reference's tests assert;
   * pinv_solve vs numpy.linalg.lstsq/pinv (Eigen completeOrthogonalDecomposition semantics: min-norm least squares)."""
+import hashlib
 import json
 import os
 
@@ -30,28 +33,51 @@ def _contact_lcp(rng, nc, reg):
     return A, b, lo, hi, fi
 
 
-@pytest.mark.skipif(ob.ref_ode() is None, reason="oracle/_ref/libodelcp.so not built (needs /root/reference)")
+# The seeded problem sets compared with dSolveLCP: name -> (seed, regularisation of A); 300 problems of 1..8 contacts each
+DANTZIG_SETS = {"regularised": (1, 1e-6), "singular": (2, 0.0)}
+DANTZIG_GOLDEN = os.path.join(ROOT, "tests", "golden", "dantzig_seeded.npz")
+
+
+def dantzig_problems(name):
+    seed, reg = DANTZIG_SETS[name]
+    rng = np.random.default_rng(seed)
+    return [_contact_lcp(rng, int(rng.integers(1, 9)), reg) for _ in range(300)]
+
+
+def problems_digest(probs):
+    h = hashlib.sha256()
+    for p in probs:
+        for v in p:
+            h.update(np.ascontiguousarray(v, np.float64).tobytes())
+    return h.hexdigest()
+
+
+def reference_dantzig(name, early):
+    """[(x, ok)] the Dantzig solvers are held to on dantzig_problems(name): dSolveLCP's own when oracle/_ref/libodelcp.so is present, else
+    the record in tests/golden/dantzig_seeded.npz (tests/golden/make_dantzig_golden.py; its `source` entry names what answered)."""
+    probs = dantzig_problems(name)
+    if ob.ref_ode() is not None:
+        return [ob.ref_dsolve_lcp(*p, early) for p in probs]
+    g = np.load(DANTZIG_GOLDEN)
+    assert str(g[f"{name}_digest"]) == problems_digest(probs), "the seeded problems differ from the ones the record was made from"
+    key = f"{name}_{'early' if early else 'full'}"
+    return [(g[key + "_x"][k, :len(p[1])], bool(g[key + "_ok"][k])) for k, p in enumerate(probs)]
+
+
 @pytest.mark.parametrize("early", [True, False])
 def test_dantzig_matches_reference_dSolveLCP(oracle_mod, early):
-    rng = np.random.default_rng(1)
-    for trial in range(300):
-        A, b, lo, hi, fi = _contact_lcp(rng, int(rng.integers(1, 9)), 1e-6)
-        xr, okr = ob.ref_dsolve_lcp(A, b, lo, hi, fi, early)
+    for (A, b, lo, hi, fi), (xr, okr) in zip(dantzig_problems("regularised"), reference_dantzig("regularised", early)):
         xo, oko = ob.dantzig(A, b, lo, hi, fi, early)
         assert okr == oko
         if okr:
             assert np.abs(xr - xo).max() <= 1e-7 * max(1.0, np.abs(xr).max())
 
 
-@pytest.mark.skipif(ob.ref_ode() is None, reason="oracle/_ref/libodelcp.so not built (needs /root/reference)")
 def test_dantzig_on_exactly_singular_problems_mostly_matches(oracle_mod, capfd):
     """A = J J^T with redundant rows: pivoting on a singular factor is decided by rounding; the two implementations
     use different (mathematically equal) factor updates, so a few percent of such instances may differ."""
-    rng = np.random.default_rng(2)
     agree = total = 0
-    for trial in range(300):
-        A, b, lo, hi, fi = _contact_lcp(rng, int(rng.integers(1, 9)), 0.0)
-        xr, okr = ob.ref_dsolve_lcp(A, b, lo, hi, fi, True)
+    for (A, b, lo, hi, fi), (xr, okr) in zip(dantzig_problems("singular"), reference_dantzig("singular", True)):
         xo, oko = ob.dantzig(A, b, lo, hi, fi, True)
         total += 1
         if okr == oko and (not okr or np.abs(xr - xo).max() <= 1e-6 * max(1.0, np.abs(xr).max())):

@@ -124,11 +124,21 @@ def test_builder_surface_matches_reference_example():
     assert cm.nb == 2 and list(cm.jtype) == [2, 1]
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/data"), reason="reference data only in the build container")
-def test_fixtures_are_current_with_reference_files():
-    import subprocess, sys, tempfile, json
+def test_urdf_loader_reproduces_the_cartpole_fixture():
+    """tests/golden/loader/cartpole.urdf describes the robot of tests/golden/models/cartpole.json: loading it (DartLoader rules: a root
+    link named `world` welds the tree to the ground, joints sorted by name, continuous joints unlimited) gives the stored model."""
+    import json
     from tests.util import MODELS, ROOT
-    w = nb.loadWorld("/root/reference/data/skel/half_cheetah.skel")
+    w = nb.loadWorld(os.path.join(ROOT, "tests", "golden", "loader", "cartpole.urdf"))
+    w.setGravity([0, -9.81, 0])
+    assert json.loads(nb.flatten_world(w).to_json()) == json.load(open(os.path.join(MODELS, "cartpole.json")))
+
+
+@pytest.mark.skipif(not os.environ.get("NB2_REFERENCE_DATA"), reason="NB2_REFERENCE_DATA does not name the reference's data/ directory")
+def test_fixtures_are_current_with_reference_files():
+    import json
+    from tests.util import MODELS
+    w = nb.loadWorld(os.path.join(os.environ["NB2_REFERENCE_DATA"], "skel", "half_cheetah.skel"))
     fresh = json.loads(nb.flatten_world(w).to_json())
     stored = json.load(open(os.path.join(MODELS, "half_cheetah.json")))
     assert fresh == stored
