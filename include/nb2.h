@@ -123,6 +123,19 @@ int nb2_step_forward_host(nb2_model* m, int B, const float* state, const float* 
 int nb2_step_backward_host(nb2_model* m, int B, const float* grad_next_state, float* grad_state, float* grad_action,
                            int precision);
 
+/* ---- per-world inertia: the *_pw variants of the step and rollout entry points ----------------------------------------------
+ * world_inertia (may be NULL = the model's table): device memory, fp64, word-major [10*nb][B] (the layout of grad_inertia): word k of
+ * canonical body i of world w at world_inertia[(10*i + k) * B + w], holding (m, h = m*c (3), Ibar xx,yy,zz,xy,xz,yz about the body origin)
+ * exactly as nb2_model_desc.inertia does.  World w then steps with its own inertia; everything else of the model is shared.
+ * A backward must be given the SAME world_inertia as the forward whose saved stream it consumes.  Masses are not checked on the device:
+ * a world with a non-positive mass gets non-finite outputs; no other world is affected.  The existing entry points are these with NULL.
+ * Not extended: the *_host entry points, nb2_forward_dynamics and the IKMapping kernels (COM entries use the model's masses). */
+int nb2_step_forward_pw(const nb2_model* m, int B, const float* state, const float* action, const double* world_inertia, float* next_state,
+                        void* saved, int precision, void* stream);
+int nb2_step_backward_pw(const nb2_model* m, int B, const float* state, const float* action, const double* world_inertia, const void* saved,
+                         const float* grad_next_state, float* grad_state, float* grad_action, float* grad_inertia,
+                         int precision, void* stream);
+
 #define NB2_MAX_CONTACTS 16
 #define NB2_MAX_ROWS 48
 /* ---- contact / boxed-LCP stage -------------------------------------------------------------------------------
@@ -162,6 +175,13 @@ size_t nb2_contact_record_bytes(const nb2_model* m, int B);
 int nb2_step_backward_contact(const nb2_model* m, int B, const float* state, const float* action, const void* saved_fp64,
                               const double* contact_record, void* workspace, const float* grad_next_state, float* grad_state,
                               float* grad_action, float* grad_inertia, int32_t* status_accum, void* stream);
+/* per-world inertia (see nb2_step_forward_pw); the contact stage itself reads no inertia: it works from the forward's articulated quantities */
+int nb2_step_forward_contact_pw(const nb2_model* m, int B, const float* state, const float* action, const double* world_inertia, float* next_state,
+                                void* saved_fp64, void* workspace, double* x_lcp, int32_t* m_lcp, int32_t* labels,
+                                int32_t* status, int32_t* ncontacts, float* cinfo, double* contact_record, int32_t* status_accum, void* stream);
+int nb2_step_backward_contact_pw(const nb2_model* m, int B, const float* state, const float* action, const double* world_inertia, const void* saved_fp64,
+                                 const double* contact_record, void* workspace, const float* grad_next_state, float* grad_state,
+                                 float* grad_action, float* grad_inertia, int32_t* status_accum, void* stream);
 /* contacts per world the shared-memory workspace of the fused contact kernels is sized for (LCP rows: 3x).  Default: 4 per box-box
  * pair + 1 per other pair, clamped to [2, NB2_MAX_CONTACTS].  Smaller = more resident worlds per SM, more worlds in the slow pool. */
 /* The same two calls with HOST buffers (pageable or pinned): copies, kernels and a synchronise inside; the solver cache, the saved stream, the
@@ -202,6 +222,13 @@ int nb2_lcp_solve_batch(int B, int mcap, int mode, int early_termination, double
 int nb2_rollout_forward(const nb2_model* m, int B, int T, float* states, const float* actions, void* saved, int precision, void* stream);
 int nb2_rollout_backward(const nb2_model* m, int B, int T, const float* states, const float* actions, const void* saved,
                          float* grad_states, float* grad_actions, int precision, void* stream);
+/* per-world inertia (see nb2_step_forward_pw), constant over the horizon.  grad_inertia (may be NULL): [10*nb][B] DOUBLES, accumulated in
+ * place: every step adds its fp32 dL/d(inertia) term, so the caller zeroes it first and gets the sum over the T steps — the same fp64
+ * sum, in the same order (t = T-1 .. 0), that chaining the single-step backward and adding its outputs gives. */
+int nb2_rollout_forward_pw(const nb2_model* m, int B, int T, float* states, const float* actions, const double* world_inertia, void* saved, int precision,
+                           void* stream);
+int nb2_rollout_backward_pw(const nb2_model* m, int B, int T, const float* states, const float* actions, const double* world_inertia, const void* saved,
+                            float* grad_states, float* grad_actions, double* grad_inertia, int precision, void* stream);
 
 /* T-step rollout of a world WITH collision pairs and its reverse sweep (SingleShot::getSnapshots / backpropGradientWrt as above; every step
  * is World::step with the constraint solve, and the solver's cached LCP solution x_lcp / m_lcp flows from step to step on the device as
@@ -219,6 +246,12 @@ int nb2_rollout_forward_contact(const nb2_model* m, int B, int T, float* states,
                                 int checkpoint_every, void* workspace, int32_t* status_accum, void* stream);
 int nb2_rollout_backward_contact(const nb2_model* m, int B, int T, const float* states, const float* actions, double* x_lcp, int32_t* m_lcp, void* tape,
                                  int checkpoint_every, float* grad_states, float* grad_actions, void* workspace, int32_t* status_accum, void* stream);
+/* per-world inertia: as nb2_rollout_forward_pw / nb2_rollout_backward_pw (grad_inertia: fp64 sum over the horizon, also under checkpointing) */
+int nb2_rollout_forward_contact_pw(const nb2_model* m, int B, int T, float* states, const float* actions, const double* world_inertia, double* x_lcp,
+                                   int32_t* m_lcp, void* tape, int checkpoint_every, void* workspace, int32_t* status_accum, void* stream);
+int nb2_rollout_backward_contact_pw(const nb2_model* m, int B, int T, const float* states, const float* actions, const double* world_inertia, double* x_lcp,
+                                    int32_t* m_lcp, void* tape, int checkpoint_every, float* grad_states, float* grad_actions, double* grad_inertia,
+                                    void* workspace, int32_t* status_accum, void* stream);
 
 /* IKMapping: task-space outputs of a state and their VJP, on the device (neural/IKMapping.cpp:146-237 getPositionsInPlace /
  * getVelocitiesInPlace; :371-476 getPosJacobian / getVelJacobian; python/nimblephysics/mapping.py:23-114 map_to_pos / map_to_vel).

@@ -152,6 +152,15 @@ def lib() -> ctypes.CDLL:
         L.nb2_step_backward.argtypes = [vp, ctypes.c_int, vp, vp, vp, vp, vp, vp, vp, ctypes.c_int, vp]
         L.nb2_rollout_forward.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp, vp, vp, ctypes.c_int, vp]
         L.nb2_rollout_backward.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp, vp, ctypes.c_int, vp]
+        # per-world inertia variants: the same arguments with `world_inertia` after the action(s) (rollout backward: + grad_inertia)
+        L.nb2_step_forward_pw.argtypes = [vp, ctypes.c_int, vp, vp, vp, vp, vp, ctypes.c_int, vp]
+        L.nb2_step_backward_pw.argtypes = [vp, ctypes.c_int, vp, vp, vp, vp, vp, vp, vp, vp, ctypes.c_int, vp]
+        L.nb2_rollout_forward_pw.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp, ctypes.c_int, vp]
+        L.nb2_rollout_backward_pw.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp, vp, vp, vp, ctypes.c_int, vp]
+        L.nb2_step_forward_contact_pw.argtypes = [vp, ctypes.c_int] + [vp] * 15
+        L.nb2_step_backward_contact_pw.argtypes = [vp, ctypes.c_int] + [vp] * 12
+        L.nb2_rollout_forward_contact_pw.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp, vp, vp, ctypes.c_int, vp, vp, vp]
+        L.nb2_rollout_backward_contact_pw.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp, vp, vp, ctypes.c_int, vp, vp, vp, vp, vp, vp]
         L.nb2_ik_create.argtypes = [vp, ctypes.c_int, vp, vp, vp, ctypes.POINTER(ctypes.c_void_p)]
         L.nb2_ik_destroy.argtypes = [vp]
         L.nb2_ik_destroy.restype = None

@@ -123,7 +123,16 @@ template <class R> NB2_HD Xf<R> xf_pris(const Nb2ModelDev<R>& M, const R* bt, in
   return T;
 }
 template <class R> NB2_HD Xf<R> xf_pris(const Nb2ModelDev<R>& M, int i, R d) { return xf_pris<R>(M, (const R*)nullptr, i, d); }
-template <class R> NB2_HD void inertia_of(const Nb2ModelDev<R>& M, const R* bt, int i, R* m, V3<R>* h, S3<R>* Ib) {
+// wi: optional PER-WORLD inertia table (fp64, word-major [10*nb][wiB] like grad_inertia, already offset to the world) that replaces
+// the model's: the worlds of a warp are adjacent, so its loads coalesce.  nullptr = the model's table (kernel parameter or `bt`).
+template <class R> NB2_HD void inertia_of(const Nb2ModelDev<R>& M, const R* bt, const double* wi, size_t wiB, int i, R* m, V3<R>* h, S3<R>* Ib) {
+  if (wi) {
+    const double* t = wi + (size_t)(10 * i) * wiB;
+    *m = (R)t[0]; *h = mk3<R>((R)t[wiB], (R)t[2 * wiB], (R)t[3 * wiB]);
+    Ib->xx = (R)t[4 * wiB]; Ib->yy = (R)t[5 * wiB]; Ib->zz = (R)t[6 * wiB];
+    Ib->xy = (R)t[7 * wiB]; Ib->xz = (R)t[8 * wiB]; Ib->yz = (R)t[9 * wiB];
+    return;
+  }
   if (bt) {
     const R* t = bt + NB2_BT_WORDS * i + 12;
     *m = t[0]; *h = mk3<R>(t[1], t[2], t[3]);
@@ -135,7 +144,7 @@ template <class R> NB2_HD void inertia_of(const Nb2ModelDev<R>& M, const R* bt, 
   Ib->xx = M.inertia[i][4]; Ib->yy = M.inertia[i][5]; Ib->zz = M.inertia[i][6];
   Ib->xy = M.inertia[i][7]; Ib->xz = M.inertia[i][8]; Ib->yz = M.inertia[i][9];
 }
-template <class R> NB2_HD void inertia_of(const Nb2ModelDev<R>& M, int i, R* m, V3<R>* h, S3<R>* Ib) { inertia_of<R>(M, (const R*)nullptr, i, m, h, Ib); }
+template <class R> NB2_HD void inertia_of(const Nb2ModelDev<R>& M, int i, R* m, V3<R>* h, S3<R>* Ib) { inertia_of<R>(M, (const R*)nullptr, nullptr, 0, i, m, h, Ib); }
 template <class R, int ST> NB2_HD Xf<R> ldXf(const R* p) {
   Xf<R> T;
   T.R_.m00 = p[0]; T.R_.m01 = p[ST]; T.R_.m02 = p[2 * ST]; T.R_.m10 = p[3 * ST]; T.R_.m11 = p[4 * ST]; T.R_.m12 = p[5 * ST];
@@ -207,7 +216,8 @@ NB2_HD void fwd_pass1(const Nb2ModelDev<R>& M, R* scr, int lo, int hi, const R* 
 }
 
 template <class R, int ST>
-NB2_HD void fwd_pass2(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool save, int lo, int hi, const R* bt = nullptr, R* iinv_out = nullptr) {
+NB2_HD void fwd_pass2(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool save, int lo, int hi, const R* bt = nullptr, R* iinv_out = nullptr,
+                      const double* wi = nullptr, size_t wiB = 0) {
   const int nb = M.nb, n = M.ndof;
   const FwdLayout L = fwd_layout(nb, n, M.nslots, M.nfree);
   const R dt = M.dt;
@@ -220,7 +230,7 @@ NB2_HD void fwd_pass2(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool sav
   for (int i = hi - 1; i >= lo; i--) {
     const int jt = M.jtype[i], p = M.parent[i], o = M.dof_off[i], fl = M.flags[i];
     R* bs = scr + (size_t)(L.oBody + NB2_FWD_BODY_WORDS * i) * ST;
-    R m; V3<R> h; S3<R> Ib; inertia_of(M, bt, i, &m, &h, &Ib);
+    R m; V3<R> h; S3<R> Ib; inertia_of(M, bt, wi, wiB, i, &m, &h, &Ib);
     const V6<R> V = ld6<R, ST>(bs);
     SI<R> IA = rigidSI(m, h, Ib);
     V6<R> pA = crf(V, mulG(m, h, Ib, V));
@@ -479,7 +489,8 @@ NB2_HD void fwd_store(const Nb2ModelDev<R>& M, const R* scr0, float* out0, int n
 #define NB2_FWD_SYNC_MASK 0x6Bu       /* after stages 0, 1, 3, 5, 6 */
 #define NB2_FWD_SYNC_MASK_1LANE 0x41u /* lanes == 1: only the group load / store exchange data between threads */
 template <class R, int ST>
-NB2_HD void world_forward_stage(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool save, int lane, int stage, const R* bt = nullptr, R* iinv_out = nullptr) {
+NB2_HD void world_forward_stage(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool save, int lane, int stage, const R* bt = nullptr, R* iinv_out = nullptr,
+                                const double* wi = nullptr, size_t wiB = 0) {
   const int pass = (stage + 1) >> 1;                          // stages 1..6 -> passes 1, 2, 3
   const bool trunk = (stage == 1) | (stage == 4) | (stage == 5);
   if (trunk && lane != 0) return;
@@ -488,7 +499,7 @@ NB2_HD void world_forward_stage(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B
     const int r = (pass == 2) ? nr - 1 - rr : rr;
     const int lo = trunk ? M.trunk_lo[r] : M.limb_lo[lane][r], hi = trunk ? M.trunk_hi[r] : M.limb_hi[lane][r];
     if (pass == 1) fwd_pass1<R, ST>(M, scr, lo, hi, bt);
-    else if (pass == 2) fwd_pass2<R, ST>(M, scr, sv, B, save, lo, hi, bt, iinv_out);
+    else if (pass == 2) fwd_pass2<R, ST>(M, scr, sv, B, save, lo, hi, bt, iinv_out, wi, wiB);
     else fwd_pass3<R, ST>(M, scr, sv, B, save, lo, hi, bt);
   }
 }
@@ -517,13 +528,34 @@ struct BwdContactData {
   int bounce = 0, pass2 = 0;
 };
 
+// Products rounded on their own (never contracted into an FMA): which product of a*b + c*d the compiler fuses depends on the
+// surrounding code, and the inertia gradient must have the same bits in the shared-table and the per-world-inertia
+// instantiations of the reverse sweep.
+NB2_HD float mul_rn(float a, float b) {
+#ifdef __CUDA_ARCH__
+  return __fmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+NB2_HD double mul_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+template <class R> NB2_HD V3<R> cross_rn(const V3<R>& a, const V3<R>& b) {
+  return mk3<R>(mul_rn(a.y, b.z) - mul_rn(a.z, b.y), mul_rn(a.z, b.x) - mul_rn(a.x, b.z), mul_rn(a.x, b.y) - mul_rn(a.y, b.x));
+}
 // d(Y^T G X)/d(m, h(3), Ibar(xx,yy,zz,xy,xz,yz)) for G X = [Ibar w + h x v ; m v - h x w]
 template <class R> NB2_HD void inertia_param_form(const V6<R>& Y, const V6<R>& X, R* t) {
-  t[0] = dot(Y.l, X.l);
-  const V3<R> dh = cross(X.l, Y.a) + cross(Y.l, X.a);
+  t[0] = mul_rn(Y.l.x, X.l.x) + mul_rn(Y.l.y, X.l.y) + mul_rn(Y.l.z, X.l.z);
+  const V3<R> dh = cross_rn(X.l, Y.a) + cross_rn(Y.l, X.a);
   t[1] = dh.x; t[2] = dh.y; t[3] = dh.z;
-  t[4] = Y.a.x * X.a.x; t[5] = Y.a.y * X.a.y; t[6] = Y.a.z * X.a.z;
-  t[7] = Y.a.x * X.a.y + Y.a.y * X.a.x; t[8] = Y.a.x * X.a.z + Y.a.z * X.a.x; t[9] = Y.a.y * X.a.z + Y.a.z * X.a.y;
+  t[4] = mul_rn(Y.a.x, X.a.x); t[5] = mul_rn(Y.a.y, X.a.y); t[6] = mul_rn(Y.a.z, X.a.z);
+  t[7] = mul_rn(Y.a.x, X.a.y) + mul_rn(Y.a.y, X.a.x); t[8] = mul_rn(Y.a.x, X.a.z) + mul_rn(Y.a.z, X.a.x);
+  t[9] = mul_rn(Y.a.y, X.a.z) + mul_rn(Y.a.z, X.a.y);
 }
 
 // =====================================================================================================
@@ -610,7 +642,7 @@ NB2_HD void bwd_B2(const Nb2ModelDev<R>& M, R* scr, const float* st, const R* sv
 
 template <class R, int ST, bool CONTACT>
 NB2_HD void bwd_B3(const Nb2ModelDev<R>& M, R* scr, const float* st, const R* sv, size_t B, const BwdContactData<ST>& cd, int lo, int hi,
-                   float* gI = nullptr, const R* bt = nullptr, size_t gIB = 0) {
+                   float* gI = nullptr, const R* bt = nullptr, size_t gIB = 0, const double* wi = nullptr, size_t wiB = 0, double* gIa = nullptr) {
   const int nb = M.nb, n = M.ndof;
   constexpr int SLOTW = CONTACT ? 42 : 18;
   const BwdLayout L = bwd_layout(nb, n, M.nslots, M.nfree, SLOTW);
@@ -630,19 +662,21 @@ NB2_HD void bwd_B3(const Nb2ModelDev<R>& M, R* scr, const float* st, const R* sv
   for (int i = hi - 1; i >= lo; i--) {
     const int jt = M.jtype[i], p = M.parent[i], o = M.dof_off[i], fl = M.flags[i];
     const R* s = sv + (size_t)(i * 21) * B;
-    R m; V3<R> h; S3<R> Ib; inertia_of(M, bt, i, &m, &h, &Ib);
+    R m; V3<R> h; S3<R> Ib; inertia_of(M, bt, wi, wiB, i, &m, &h, &Ib);
     const V6<R> V = sv_ld6<R>(s, B, 0);
     V6<R> A = sv_ld6<R>(s, B, 6);
     if (CONTACT && cd.active && !cd.pass2) { const auto a6 = cd.Aacc + 6 * i; A.a = mk3<R>((R)a6[0], (R)a6[1], (R)a6[2]); A.l = mk3<R>((R)a6[3], (R)a6[4], (R)a6[5]); }
     const V6<R> W = ld6<R, ST>(scr + (size_t)(L.oBody + 7 * i + 1) * ST);
     const V6<R> GV = mulG(m, h, Ib, V);
     V6<R> f = mulG(m, h, Ib, A) + crf(V, GV);
-    if (gI) {
+    if (gI || gIa) {
       // dL/d(inertia parameters of body i) = -dt * W . d(G A + V x* G V) = -dt * [ t(W, A) - t(ad(V, W), V) ] with
       // t(Y, X) = d(Y^T G X)/d(m, h, Ibar)   (the mass-vel Jacobian of BackpropSnapshot.cpp:580-640 contracted with g_v').
       // With active contacts W is the field of w = lambda - nu and A the REALISED acceleration: same identity (the
       // constraint rows do not depend on the inertias).
-      const V6<R> Y2 = ad(V, W);
+      V6<R> Y2;  // ad(V, W), products rounded on their own (see mul_rn)
+      Y2.a = cross_rn(V.a, W.a);
+      Y2.l = cross_rn(V.a, W.l) + cross_rn(V.l, W.a);
       R t[10];
       inertia_param_form(W, A, t);
       R t2[10];
@@ -650,7 +684,10 @@ NB2_HD void bwd_B3(const Nb2ModelDev<R>& M, R* scr, const float* st, const R* sv
 #pragma unroll
       for (int k = 0; k < 10; k++) {
         const float gk = (float)(-dt * (t[k] - t2[k]));
-        if (CONTACT && cd.pass2) gI[(size_t)(10 * i + k) * gIB] += gk; else gI[(size_t)(10 * i + k) * gIB] = gk;
+        // gIa (rollouts): every pass ADDS its fp32 term to an fp64 sum over the horizon, the same sum the step-by-step loop forms in
+        // autograd (one thread owns the world's row: no atomics)
+        if (gIa) gIa[(size_t)(10 * i + k) * gIB] += (double)gk;
+        else if (CONTACT && cd.pass2) gI[(size_t)(10 * i + k) * gIB] += gk; else gI[(size_t)(10 * i + k) * gIB] = gk;
       }
     }
     V6<R> Abar = mulG(m, h, Ib, W);
@@ -858,7 +895,8 @@ NB2_HD void bwd_store(const Nb2ModelDev<R>& M, const R* scr0, float* gstate0, fl
 #define NB2_BWD_SYNC_MASK_1LANE 0x101u  /* lanes == 1: after the group load and before the group store */
 template <class R, int ST, bool CONTACT = false>
 NB2_HD void world_backward_stage(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, int lane, int stage, float* gI = nullptr, const R* bt = nullptr,
-                                 size_t gIB = 0, const BwdContactData<ST>* cdp = nullptr) {
+                                 size_t gIB = 0, const BwdContactData<ST>* cdp = nullptr, const double* wi = nullptr, size_t wiB = 0,
+                                 double* gIa = nullptr) {
   const float* st = nullptr;  // the passes read the state from the scratch (oSt)
   BwdContactData<ST> cd;
   if (CONTACT && cdp) cd = *cdp; else { cd.active = 0; cd.error = 0; cd.inj_of_body = nullptr; }
@@ -872,7 +910,7 @@ NB2_HD void world_backward_stage(const Nb2ModelDev<R>& M, R* scr, const R* sv, s
     const int lo = trunk ? M.trunk_lo[r] : M.limb_lo[lane][r], hi = trunk ? M.trunk_hi[r] : M.limb_hi[lane][r];
     if (pass == 1) bwd_B1<R, ST, CONTACT>(M, scr, st, sv, B, lo, hi, bt);
     else if (pass == 2) bwd_B2<R, ST, CONTACT>(M, scr, st, sv, B, lo, hi, bt);
-    else if (pass == 3) bwd_B3<R, ST, CONTACT>(M, scr, st, sv, B, cd, lo, hi, gI, bt, gIB ? gIB : B);
+    else if (pass == 3) bwd_B3<R, ST, CONTACT>(M, scr, st, sv, B, cd, lo, hi, gI, bt, gIB ? gIB : B, wi, wiB, gIa);
     else bwd_assemble<R, ST, CONTACT>(M, scr, st, cd, lo, hi);
   }
 }

@@ -89,12 +89,14 @@ template <int K> __host__ __device__ constexpr size_t staging_bytes(int floats_p
   return (((size_t)floats_per_world * CoopShape<K>::WPW * sizeof(float) + 15) & ~(size_t)15) + 16;
 }
 
-template <class R, int K>
+// PW: the variant with a per-world inertia table (nb2_step_forward_pw).  A compile-time switch: as a run-time pointer test it cost the
+// shared-table kernels registers (fp32) and spills (fp64).
+template <class R, int K, bool PW>
 __global__ void __launch_bounds__(128)
 k_step_fwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, const float* __restrict__ state,
            const float* __restrict__ action, float* __restrict__ next, R* __restrict__ saved, int words,
-           float* __restrict__ state_copy, float* __restrict__ action_copy) {
-  // worlds [w0, w0 + count) of a batch of B (B is the stride of the saved stream; the host entry points launch chunks)
+           float* __restrict__ state_copy, float* __restrict__ action_copy, const double* __restrict__ winertia) {
+  // worlds [w0, w0 + count) of a batch of B (B is the stride of the saved stream and of the per-world inertia; the host entry points launch chunks)
   extern __shared__ __align__(16) unsigned char nb2_smem[];
   constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
   const int li = threadIdx.x & 31, slot = li / K, lane = li % K;
@@ -106,6 +108,7 @@ k_step_fwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
   R* scr0 = reinterpret_cast<R*>(nb2_smem) + body_table_words<K>(M.nb) + (size_t)(threadIdx.x >> 5) * words * ST;
   R* scr = scr0 + slot;
   R* sv = saved ? saved + wg + (valid ? slot : 0) : nullptr;
+  const double* wi = PW ? winertia + wg + (valid ? slot : 0) : nullptr;
   constexpr unsigned sync_mask = (K > 1) ? NB2_FWD_SYNC_MASK : NB2_FWD_SYNC_MASK_1LANE;
   // input rows of the group: through the bulk-copy staging buffer when they qualify, else read in place
   const float* st_src = state + wg * 2 * M.ndof;
@@ -135,17 +138,17 @@ k_step_fwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
                                             state_copy ? state_copy + wg * 2 * M.ndof : nullptr, action_copy ? action_copy + wg * M.na : nullptr);
     }
     else if (sg == NB2_FWD_STAGES - 1) { if (nworlds > 0) nb2::fwd_store<R, ST>(M, scr0, next + wg * 2 * M.ndof, nworlds, li, 32); }
-    else if (valid) nb2::world_forward_stage<R, ST>(M, scr, sv, (size_t)B, saved != nullptr, lane, sg, bt);
+    else if (valid) nb2::world_forward_stage<R, ST>(M, scr, sv, (size_t)B, saved != nullptr, lane, sg, bt, nullptr, wi, (size_t)B);
     if ((sync_mask >> sg) & 1u) __syncwarp();
   }
 }
 
-template <class R, int K>
+template <class R, int K, bool PW>
 __global__ void __launch_bounds__(128)
 k_step_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, const float* __restrict__ state,
            const float* __restrict__ action, const R* __restrict__ saved, const float* __restrict__ gnext,
            float* __restrict__ gstate, float* __restrict__ gaction, float* __restrict__ ginertia, int words,
-           int stage_saved, int accumulate_state, unsigned in_stage_off) {
+           int stage_saved, int accumulate_state, unsigned in_stage_off, const double* __restrict__ winertia, double* __restrict__ ginertia_acc) {
   extern __shared__ __align__(16) unsigned char nb2_smem[];
   constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
   const int li = threadIdx.x & 31, slot = li / K, lane = li % K;
@@ -208,7 +211,8 @@ k_step_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
     if (sg == 0) { if (nworlds > 0) nb2::bwd_load<R, ST, false>(M, scr0, st_src, act_src, g_src, nworlds, li, 32); }
     else if (sg == NB2_BWD_STAGES - 1) {
       if (nworlds > 0) nb2::bwd_store<R, ST, false>(M, scr0, gstate + wg * 2 * M.ndof, gaction + wg * M.na, false, nworlds, li, 32, accumulate_state != 0);
-    } else if (valid) nb2::world_backward_stage<R, ST>(M, scr, svp, svB, lane, sg, ginertia ? ginertia + w : nullptr, bt, (size_t)B);
+    } else if (valid) nb2::world_backward_stage<R, ST>(M, scr, svp, svB, lane, sg, ginertia ? ginertia + w : nullptr, bt, (size_t)B, nullptr,
+                                                       (PW && winertia) ? winertia + w : nullptr, (size_t)B, (PW && ginertia_acc) ? ginertia_acc + w : nullptr);
     if (sg == 0 && stage_saved) asm volatile("cp.async.wait_group 0;" ::: "memory");
     if (((sync_mask >> sg) & 1u) || (sg == 0 && stage_saved)) __syncwarp();
   }
@@ -240,10 +244,12 @@ __global__ void __launch_bounds__(32, NB2_CSTEP_MINB)
 k_cstep_fwd(const __grid_constant__ Nb2ModelDev<double> M, const __grid_constant__ Nb2ContactDev C, const __grid_constant__ CStepArgs P,
             const float* __restrict__ state, const float* __restrict__ action, float* __restrict__ next, double* __restrict__ saved,
             double* __restrict__ x_lcp, int* __restrict__ m_lcp, int* __restrict__ labels, int* __restrict__ status,
-            int* __restrict__ ncontacts, float* __restrict__ cinfo, double* __restrict__ crec, int* __restrict__ status_accum) {
+            int* __restrict__ ncontacts, float* __restrict__ cinfo, double* __restrict__ crec, int* __restrict__ status_accum,
+            const double* __restrict__ winertia) {
   extern __shared__ __align__(16) unsigned char nb2_smem[];
   const int w = blockIdx.x, lane = threadIdx.x & 31;
   if (w >= P.B) return;
+  const double* wi = winertia ? winertia + w : nullptr;
   double* scr = reinterpret_cast<double*>(nb2_smem);
   nb2::cw::Ws* wsm = reinterpret_cast<nb2::cw::Ws*>(scr + ((P.fwd_words + 1) & ~1));
   double* wsb = reinterpret_cast<double*>(wsm) + NB2_WS_DESC_DOUBLES;
@@ -258,7 +264,7 @@ k_cstep_fwd(const __grid_constant__ Nb2ModelDev<double> M, const __grid_constant
   __syncwarp();
 #pragma unroll 1
   for (int sg = 1; sg < NB2_FWD_STAGES - 1; sg++) {
-    if (lane < M.lanes) nb2::world_forward_stage<double, 1>(M, scr, sv, 1, sv != nullptr, lane, sg, nullptr, ws0.Iinv);
+    if (lane < M.lanes) nb2::world_forward_stage<double, 1>(M, scr, sv, 1, sv != nullptr, lane, sg, nullptr, ws0.Iinv, wi, (size_t)P.B);
     if ((NB2_FWD_SYNC_MASK >> sg) & 1u) __syncwarp();
   }
   __syncwarp();
@@ -281,12 +287,13 @@ __global__ void __launch_bounds__(32 * NB2_CBUILD_MAXW, 1)
 k_cbuild(const __grid_constant__ Nb2ModelDev<double> M, const __grid_constant__ Nb2ContactDev C, const __grid_constant__ CStepArgs P,
          const float* __restrict__ state, const float* __restrict__ action, float* __restrict__ next, double* __restrict__ saved,
          int* __restrict__ m_lcp, int* __restrict__ status, int* __restrict__ ncontacts, float* __restrict__ cinfo, double* __restrict__ crec,
-         size_t smem_per_warp) {
+         size_t smem_per_warp, const double* __restrict__ winertia) {
   extern __shared__ __align__(16) unsigned char nb2_smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
   const int w = blockIdx.x * wpb + warp;
   const bool live = w < P.B;
   const int wc = live ? w : P.B - 1;  // a warp without a world redoes the last one (reads only) so that it walks the same code
+  const double* wi = winertia ? winertia + wc : nullptr;
   double* scr = reinterpret_cast<double*>(nb2_smem + (size_t)warp * smem_per_warp);
   nb2::cw::Ws* wsm = reinterpret_cast<nb2::cw::Ws*>(scr + ((P.fwd_words + 1) & ~1));
   double* wsb = reinterpret_cast<double*>(wsm) + NB2_WS_DESC_DOUBLES;
@@ -302,7 +309,7 @@ k_cbuild(const __grid_constant__ Nb2ModelDev<double> M, const __grid_constant__ 
 #pragma unroll 1
   for (int sg = 1; sg < NB2_FWD_STAGES - 1; sg++) {
     __syncthreads();  // lockstep: every warp of the block sweeps the same stage
-    if (lane < M.lanes) nb2::world_forward_stage<double, 1>(M, scr, sv, 1, sv != nullptr, lane, sg, nullptr, ws0.Iinv);
+    if (lane < M.lanes) nb2::world_forward_stage<double, 1>(M, scr, sv, 1, sv != nullptr, lane, sg, nullptr, ws0.Iinv, wi, (size_t)P.B);
     if ((NB2_FWD_SYNC_MASK >> sg) & 1u) __syncwarp();
   }
   __syncwarp();
@@ -375,7 +382,8 @@ __global__ void __launch_bounds__(32 * NB2_CBWD_MAXW, 1)
 k_cstep_bwd(const __grid_constant__ Nb2ModelDev<double> M, const __grid_constant__ Nb2ContactDev C, const __grid_constant__ CStepArgs P,
             const float* __restrict__ state, const float* __restrict__ action, const double* __restrict__ saved, const double* __restrict__ crec,
             const float* __restrict__ gnext, float* __restrict__ gstate, float* __restrict__ gaction, float* __restrict__ ginertia,
-            int* __restrict__ status, size_t smem_per_warp, int stage_saved, int accumulate_state) {
+            int* __restrict__ status, size_t smem_per_warp, int stage_saved, int accumulate_state, const double* __restrict__ winertia,
+            double* __restrict__ ginertia_acc) {
   extern __shared__ __align__(16) unsigned char nb2_smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
   const int w = blockIdx.x * wpb + warp;
@@ -404,6 +412,8 @@ k_cstep_bwd(const __grid_constant__ Nb2ModelDev<double> M, const __grid_constant
   nb2::BwdContactData<1> cd; cd.active = 0; cd.error = 0; cd.inj_of_body = nullptr;
   nb2::BwdContactData<1> c2 = cd;
   float* gI = (ginertia && live) ? ginertia + w : nullptr;
+  double* gIa = (ginertia_acc && live) ? ginertia_acc + w : nullptr;
+  const double* wi = winertia ? winertia + wc : nullptr;
   // stage order: B1 limbs, B1 trunk, B2 trunk, B2 limbs | contact adjoint | B3 limbs, B3 trunk | (worlds in which restitution was active: a
   // SECOND B3 over limbs and trunk, see contact_backward) | assembly limbs, trunk.  One call site for all of them (code size), one block-wide
   // barrier per entry (lockstep, see k_csolve): worlds without a bounce only wait at the two extra barriers.
@@ -430,7 +440,8 @@ k_cstep_bwd(const __grid_constant__ Nb2ModelDev<double> M, const __grid_constant
       if (it == 6) c2 = nb2::cw::bounce_pass2_begin(M, C, *wsm, cd, scr, L.oLam, L.oBody);
       if (it == 8 && cd.bounce) nb2::cw::bounce_pass2_end(M, *wsm, scr, L.oLam);
     }
-    if (lane < M.lanes) nb2::world_backward_stage<double, 1, true>(M, scr, sv, 1, lane, sg, gI, nullptr, (size_t)P.B, (BOUNCE && second) ? &c2 : &cd);
+    if (lane < M.lanes) nb2::world_backward_stage<double, 1, true>(M, scr, sv, 1, lane, sg, gI, nullptr, (size_t)P.B, (BOUNCE && second) ? &c2 : &cd,
+                                                                   wi, (size_t)P.B, gIa);
     __syncwarp();
   }
   __syncwarp();
@@ -757,12 +768,14 @@ template <class R, int K> struct StepKernels {
     const size_t per_warp = (size_t)(dir ? v.bwd_words : v.fwd_words) * ST * sizeof(R) + (dir ? staging_bytes<K>(4 * v.mf.ndof + v.mf.na) : staging_bytes<K>(2 * v.mf.ndof + v.mf.na));
     const size_t per_block = (size_t)body_table_words<K>(v.mf.nb) * sizeof(R) + 16;
     if (per_warp + per_block > (size_t)kMaxSmem) { g_err = "model needs " + std::to_string(per_warp) + " B of shared memory per warp (> 227 KB)"; return NB2_ERR_UNSUPPORTED; }
-    if (dir == 0) {
-      NB2_CUDA(cudaFuncSetAttribute(k_step_fwd<R, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
-      sh = occupancy_shape(k_step_fwd<R, K>, per_warp, per_block);
+    if (dir == 0) {  // the per-world-inertia variant launches with the shape of the shared-table kernel
+      NB2_CUDA(cudaFuncSetAttribute(k_step_fwd<R, K, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
+      NB2_CUDA(cudaFuncSetAttribute(k_step_fwd<R, K, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
+      sh = occupancy_shape(k_step_fwd<R, K, false>, per_warp, per_block);
     } else {
-      NB2_CUDA(cudaFuncSetAttribute(k_step_bwd<R, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
-      sh = occupancy_shape(k_step_bwd<R, K>, per_warp, per_block);
+      NB2_CUDA(cudaFuncSetAttribute(k_step_bwd<R, K, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
+      NB2_CUDA(cudaFuncSetAttribute(k_step_bwd<R, K, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
+      sh = occupancy_shape(k_step_bwd<R, K, false>, per_warp, per_block);
     }
     if (!sh.warps_per_block) { g_err = "no launch shape fits this model"; return NB2_ERR_UNSUPPORTED; }
     return NB2_OK;
@@ -801,30 +814,32 @@ static int pick_variant(nb2_model* m, int B, int dir, nb2_variant** out) {
 
 template <class R, int K>
 static int launch_fwd_k(const nb2_variant& v, int sm_count, int Btot, int w0, int B, const float* state, const float* action,
-                        float* next, R* saved, cudaStream_t st, float* state_copy, float* action_copy) {
+                        float* next, R* saved, cudaStream_t st, float* state_copy, float* action_copy, const double* wi) {
   constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
   const LaunchShape& sh = v.shape[0][sizeof(R) == 8];
   const size_t per_warp = (size_t)v.fwd_words * ST * sizeof(R) + staging_bytes<K>(2 * v.mf.ndof + v.mf.na);  // scratch + input staging
   const int total_warps = (B + WPW - 1) / WPW;
   const int warps = block_warps(total_warps, sm_count, sh, per_warp);
   const int blocks = (total_warps + warps - 1) / warps;
-  k_step_fwd<R, K><<<blocks, warps * 32, per_warp * warps + (size_t)body_table_words<K>(v.mf.nb) * sizeof(R) + 16, st>>>(model_of<R>(v), Btot, w0, B, state, action, next, saved, v.fwd_words, state_copy, action_copy);
+  const size_t smem = per_warp * warps + (size_t)body_table_words<K>(v.mf.nb) * sizeof(R) + 16;
+  if (wi) k_step_fwd<R, K, true><<<blocks, warps * 32, smem, st>>>(model_of<R>(v), Btot, w0, B, state, action, next, saved, v.fwd_words, state_copy, action_copy, wi);
+  else k_step_fwd<R, K, false><<<blocks, warps * 32, smem, st>>>(model_of<R>(v), Btot, w0, B, state, action, next, saved, v.fwd_words, state_copy, action_copy, nullptr);
   g_launches++;
   NB2_CUDA(cudaGetLastError());
   return NB2_OK;
 }
 template <class R>
 static int launch_fwd(nb2_model* m, int B, const float* state, const float* action, float* next, R* saved, cudaStream_t st,
-                      int Btot = -1, int w0 = 0, float* state_copy = nullptr, float* action_copy = nullptr) {
+                      int Btot = -1, int w0 = 0, float* state_copy = nullptr, float* action_copy = nullptr, const double* wi = nullptr) {
   if (Btot < 0) Btot = B;
   nb2_variant* pv = nullptr;
   int rc = pick_variant<R>(m, B, 0, &pv);
   if (rc) return rc;
   switch (pv->mf.lanes) {
-    case 1: return launch_fwd_k<R, 1>(*pv, m->sm_count, Btot, w0, B, state, action, next, saved, st, state_copy, action_copy);
-    case 2: return launch_fwd_k<R, 2>(*pv, m->sm_count, Btot, w0, B, state, action, next, saved, st, state_copy, action_copy);
-    case 4: return launch_fwd_k<R, 4>(*pv, m->sm_count, Btot, w0, B, state, action, next, saved, st, state_copy, action_copy);
-    case 8: return launch_fwd_k<R, 8>(*pv, m->sm_count, Btot, w0, B, state, action, next, saved, st, state_copy, action_copy);
+    case 1: return launch_fwd_k<R, 1>(*pv, m->sm_count, Btot, w0, B, state, action, next, saved, st, state_copy, action_copy, wi);
+    case 2: return launch_fwd_k<R, 2>(*pv, m->sm_count, Btot, w0, B, state, action, next, saved, st, state_copy, action_copy, wi);
+    case 4: return launch_fwd_k<R, 4>(*pv, m->sm_count, Btot, w0, B, state, action, next, saved, st, state_copy, action_copy, wi);
+    case 8: return launch_fwd_k<R, 8>(*pv, m->sm_count, Btot, w0, B, state, action, next, saved, st, state_copy, action_copy, wi);
   }
   g_err = "bad lane count"; return NB2_ERR_INVALID;
 }
@@ -834,7 +849,8 @@ static bool no_stage_saved() {
 }
 template <class R, int K>
 static int launch_bwd_k(const nb2_variant& v, int sm_count, int Btot, int w0, int B, const float* state, const float* action,
-                        const R* saved, const float* gnext, float* gstate, float* gaction, float* ginertia, cudaStream_t st, int accumulate) {
+                        const R* saved, const float* gnext, float* gstate, float* gaction, float* ginertia, cudaStream_t st, int accumulate,
+                        const double* wi, double* gIa) {
   constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
   const LaunchShape& sh = v.shape[1][sizeof(R) == 8];
   const size_t per_warp = (size_t)v.bwd_words * ST * sizeof(R);
@@ -852,9 +868,11 @@ static int launch_bwd_k(const nb2_variant& v, int sm_count, int Btot, int w0, in
   const bool stage = aligned && (smem_staged + in_per_warp * warps) * blocks_per_sm + 1024 * blocks_per_sm <= (size_t)kMaxSmem && !no_stage_saved();
   const size_t base = ((stage ? smem_staged : per_warp * warps + tab) + 15) & ~(size_t)15;
   const bool in_stage = base + in_per_warp * warps <= (size_t)kMaxSmem;
-  k_step_bwd<R, K><<<blocks, warps * 32, in_stage ? base + in_per_warp * warps : base, st>>>(model_of<R>(v), Btot, w0, B, state, action, saved, gnext, gstate,
-                                                                                         gaction, ginertia, v.bwd_words, stage ? 1 : 0, accumulate,
-                                                                                         in_stage ? (unsigned)base : 0u);
+  const size_t smem = in_stage ? base + in_per_warp * warps : base;
+  if (wi || gIa) k_step_bwd<R, K, true><<<blocks, warps * 32, smem, st>>>(model_of<R>(v), Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia,
+                                                                   v.bwd_words, stage ? 1 : 0, accumulate, in_stage ? (unsigned)base : 0u, wi, gIa);
+  else k_step_bwd<R, K, false><<<blocks, warps * 32, smem, st>>>(model_of<R>(v), Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia,
+                                                                 v.bwd_words, stage ? 1 : 0, accumulate, in_stage ? (unsigned)base : 0u, nullptr, nullptr);
   g_launches++;
   NB2_CUDA(cudaGetLastError());
   return NB2_OK;
@@ -862,16 +880,16 @@ static int launch_bwd_k(const nb2_variant& v, int sm_count, int Btot, int w0, in
 template <class R>
 static int launch_bwd(nb2_model* m, int B, const float* state, const float* action,
                       const R* saved, const float* gnext, float* gstate, float* gaction, float* ginertia, cudaStream_t st,
-                      int Btot = -1, int w0 = 0, int accumulate = 0) {
+                      int Btot = -1, int w0 = 0, int accumulate = 0, const double* wi = nullptr, double* gIa = nullptr) {
   if (Btot < 0) Btot = B;
   nb2_variant* pv = nullptr;
   int rc = pick_variant<R>(m, B, 1, &pv);
   if (rc) return rc;
   switch (pv->mf.lanes) {
-    case 1: return launch_bwd_k<R, 1>(*pv, m->sm_count, Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia, st, accumulate);
-    case 2: return launch_bwd_k<R, 2>(*pv, m->sm_count, Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia, st, accumulate);
-    case 4: return launch_bwd_k<R, 4>(*pv, m->sm_count, Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia, st, accumulate);
-    case 8: return launch_bwd_k<R, 8>(*pv, m->sm_count, Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia, st, accumulate);
+    case 1: return launch_bwd_k<R, 1>(*pv, m->sm_count, Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia, st, accumulate, wi, gIa);
+    case 2: return launch_bwd_k<R, 2>(*pv, m->sm_count, Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia, st, accumulate, wi, gIa);
+    case 4: return launch_bwd_k<R, 4>(*pv, m->sm_count, Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia, st, accumulate, wi, gIa);
+    case 8: return launch_bwd_k<R, 8>(*pv, m->sm_count, Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia, st, accumulate, wi, gIa);
   }
   g_err = "bad lane count"; return NB2_ERR_INVALID;
 }
@@ -1069,6 +1087,12 @@ size_t nb2_contact_workspace_bytes(const nb2_model* m, int B) {
 int nb2_step_forward_contact(const nb2_model* cm, int B, const float* state, const float* action, float* next_state,
                              void* saved_fp64, void* workspace, double* x_lcp, int32_t* m_lcp, int32_t* labels,
                              int32_t* status, int32_t* ncontacts, float* cinfo, double* contact_record, int32_t* status_accum, void* stream) {
+  return nb2_step_forward_contact_pw(cm, B, state, action, nullptr, next_state, saved_fp64, workspace, x_lcp, m_lcp, labels, status, ncontacts, cinfo,
+                                     contact_record, status_accum, stream);
+}
+int nb2_step_forward_contact_pw(const nb2_model* cm, int B, const float* state, const float* action, const double* world_inertia, float* next_state,
+                                void* saved_fp64, void* workspace, double* x_lcp, int32_t* m_lcp, int32_t* labels,
+                                int32_t* status, int32_t* ncontacts, float* cinfo, double* contact_record, int32_t* status_accum, void* stream) {
   nb2_model* m = const_cast<nb2_model*>(cm);
   if (m && B == 0) return NB2_OK;  // an empty batch has no buffers to check
   if (!m || B < 0 || !state || !action || !next_state || !workspace || !x_lcp || !m_lcp || !labels || !status || !ncontacts) {
@@ -1088,7 +1112,7 @@ int nb2_step_forward_contact(const nb2_model* cm, int B, const float* state, con
   if (contact_fused() || !saved_fp64) {
     // one kernel does everything (also the only form that runs without a saved stream: the apply kernel reads the tree data from it)
     k_cstep_fwd<<<B, 32, smem, st>>>(v.md, m->contact, P, state, action, next_state, (double*)saved_fp64, x_lcp, m_lcp, labels, status, ncontacts, cinfo,
-                                     contact_record, status_accum);
+                                     contact_record, status_accum, world_inertia);
     g_launches++;
     NB2_CUDA(cudaGetLastError());
     return NB2_OK;
@@ -1100,7 +1124,7 @@ int nb2_step_forward_contact(const nb2_model* cm, int B, const float* state, con
   const int wpb_b = pick_wpb(B, m->sm_count, smem, NB2_CBUILD_MAXW, 0), wpb_s = pick_wpb(B, m->sm_count, smem_s, NB2_CSOLVE_MAXW, 1),
             wpb_a = pick_wpb(B, m->sm_count, smem_a, NB2_CAPPLY_MAXW, 2);
   k_cbuild<<<(B + wpb_b - 1) / wpb_b, 32 * wpb_b, smem * wpb_b, st>>>(v.md, m->contact, P, state, action, next_state, (double*)saved_fp64, m_lcp, status, ncontacts, cinfo,
-                                                                      contact_record, smem);
+                                                                      contact_record, smem, world_inertia);
   k_csolve<0><<<(B + wpb_s - 1) / wpb_s, 32 * wpb_s, smem_s * wpb_s, st>>>(m->contact, P, m->md.ndof, x_lcp, m_lcp, labels, status, contact_record, status_accum, smem_s,
                                                                          P.todo, P.todo_count);
   k_csolve<1><<<(B + wpb_s - 1) / wpb_s, 32 * wpb_s, smem_s * wpb_s, st>>>(m->contact, P, m->md.ndof, x_lcp, m_lcp, labels, status, contact_record, status_accum, smem_s,
@@ -1119,7 +1143,7 @@ size_t nb2_contact_record_bytes(const nb2_model* m, int B) {
 // accumulate: grad_state += clip(J^T grad_next_state) instead of = (rollouts: the loss gradient of x_t is already in the buffer)
 static int cbwd_launch(nb2_model* m, int B, const float* state, const float* action, const void* saved_fp64, const double* contact_record, void* workspace,
                        const float* grad_next_state, float* grad_state, float* grad_action, float* grad_inertia, int32_t* status_accum, cudaStream_t st,
-                       int accumulate) {
+                       int accumulate, const double* wi = nullptr, double* gIa = nullptr) {
   const nb2_variant& v = m->variants[m->contact_variant];
   const CStepArgs P = cstep_args(m, v, B, workspace, 1);
   const size_t smem_base = ((((size_t)P.bwd_words + 1) & ~(size_t)1) + NB2_WS_DESC_DOUBLES + ((P.ws_small_doubles + 1) & ~(size_t)1)) * sizeof(double);
@@ -1134,10 +1158,10 @@ static int cbwd_launch(nb2_model* m, int B, const float* state, const float* act
   const int wpb = pick_wpb(B, m->sm_count, smem, NB2_CBWD_MAXW, 3);
   if (bounce)
     k_cstep_bwd<true><<<(B + wpb - 1) / wpb, 32 * wpb, smem * wpb, st>>>(v.md, m->contact, P, state, action, (const double*)saved_fp64, contact_record, grad_next_state,
-                                                                         grad_state, grad_action, grad_inertia, status_accum, smem, stage, accumulate);
+                                                                         grad_state, grad_action, grad_inertia, status_accum, smem, stage, accumulate, wi, gIa);
   else
     k_cstep_bwd<false><<<(B + wpb - 1) / wpb, 32 * wpb, smem * wpb, st>>>(v.md, m->contact, P, state, action, (const double*)saved_fp64, contact_record, grad_next_state,
-                                                                          grad_state, grad_action, grad_inertia, status_accum, smem, stage, accumulate);
+                                                                          grad_state, grad_action, grad_inertia, status_accum, smem, stage, accumulate, wi, gIa);
   g_launches++;
   NB2_CUDA(cudaGetLastError());
   return NB2_OK;
@@ -1146,6 +1170,12 @@ extern "C" {
 int nb2_step_backward_contact(const nb2_model* cm, int B, const float* state, const float* action, const void* saved_fp64,
                               const double* contact_record, void* workspace, const float* grad_next_state, float* grad_state,
                               float* grad_action, float* grad_inertia, int32_t* status_accum, void* stream) {
+  return nb2_step_backward_contact_pw(cm, B, state, action, nullptr, saved_fp64, contact_record, workspace, grad_next_state, grad_state, grad_action,
+                                      grad_inertia, status_accum, stream);
+}
+int nb2_step_backward_contact_pw(const nb2_model* cm, int B, const float* state, const float* action, const double* world_inertia, const void* saved_fp64,
+                                 const double* contact_record, void* workspace, const float* grad_next_state, float* grad_state,
+                                 float* grad_action, float* grad_inertia, int32_t* status_accum, void* stream) {
   nb2_model* m = const_cast<nb2_model*>(cm);
   if (m && B == 0) return NB2_OK;
   if (!m || B < 0 || !state || !action || !saved_fp64 || !contact_record || !workspace || !grad_next_state || !grad_state || !grad_action) {
@@ -1154,7 +1184,7 @@ int nb2_step_backward_contact(const nb2_model* cm, int B, const float* state, co
   if (!m->has_contacts) { g_err = "nb2_step_backward_contact: the model has no collision pairs"; return NB2_ERR_INVALID; }
   if (B == 0) return NB2_OK;
   return cbwd_launch(m, B, state, action, saved_fp64, contact_record, workspace, grad_next_state, grad_state, grad_action, grad_inertia, status_accum,
-                     (cudaStream_t)stream, 0);
+                     (cudaStream_t)stream, 0, world_inertia);
 }
 
 // ---- whole-horizon rollouts of contact worlds (row f1): the T steps are queued from C, the LCP cache flows on the device, and the tape of
@@ -1204,6 +1234,10 @@ static int snap_copy(double* tape, const RolloutTape& L, int idx, double* x_lcp,
 }
 int nb2_rollout_forward_contact(const nb2_model* cm, int B, int T, float* states, const float* actions, double* x_lcp, int32_t* m_lcp, void* tape_,
                                 int checkpoint_every, void* workspace, int32_t* status_accum, void* stream) {
+  return nb2_rollout_forward_contact_pw(cm, B, T, states, actions, nullptr, x_lcp, m_lcp, tape_, checkpoint_every, workspace, status_accum, stream);
+}
+int nb2_rollout_forward_contact_pw(const nb2_model* cm, int B, int T, float* states, const float* actions, const double* world_inertia, double* x_lcp,
+                                   int32_t* m_lcp, void* tape_, int checkpoint_every, void* workspace, int32_t* status_accum, void* stream) {
   nb2_model* m = const_cast<nb2_model*>(cm);
   if (m && (B == 0 || T == 0)) return NB2_OK;
   if (!m || B < 0 || T < 0 || !states || (!actions && T > 0) || !x_lcp || !m_lcp || !tape_ || !workspace) { g_err = "nb2_rollout_forward_contact: bad argument"; return NB2_ERR_INVALID; }
@@ -1222,8 +1256,8 @@ int nb2_rollout_forward_contact(const nb2_model* cm, int B, int T, float* states
     if (ckpt && t % L.k == 0 && (rc = snap_copy(tape, L, t / L.k, x_lcp, m_lcp, B, false, st))) return rc;
     double* slot = tape + L.o_slots + L.slot_doubles * (t % L.nslots);
     // with checkpoints the forward's records are thrown away (the reverse sweep regenerates them): do not write them
-    rc = nb2_step_forward_contact(m, B, states + n2 * B * t, actions + na * B * t, states + n2 * B * (t + 1), slot, workspace, x_lcp, m_lcp, labels, status, nc,
-                                  nullptr, ckpt ? nullptr : slot + L.saved_doubles, status_accum, stream);
+    rc = nb2_step_forward_contact_pw(m, B, states + n2 * B * t, actions + na * B * t, world_inertia, states + n2 * B * (t + 1), slot, workspace, x_lcp, m_lcp,
+                                     labels, status, nc, nullptr, ckpt ? nullptr : slot + L.saved_doubles, status_accum, stream);
     if (rc) return rc;
   }
   if (ckpt) return snap_copy(tape, L, L.nseg, x_lcp, m_lcp, B, false, st);
@@ -1231,6 +1265,12 @@ int nb2_rollout_forward_contact(const nb2_model* cm, int B, int T, float* states
 }
 int nb2_rollout_backward_contact(const nb2_model* cm, int B, int T, const float* states, const float* actions, double* x_lcp, int32_t* m_lcp, void* tape_,
                                  int checkpoint_every, float* grad_states, float* grad_actions, void* workspace, int32_t* status_accum, void* stream) {
+  return nb2_rollout_backward_contact_pw(cm, B, T, states, actions, nullptr, x_lcp, m_lcp, tape_, checkpoint_every, grad_states, grad_actions, nullptr,
+                                         workspace, status_accum, stream);
+}
+int nb2_rollout_backward_contact_pw(const nb2_model* cm, int B, int T, const float* states, const float* actions, const double* world_inertia, double* x_lcp,
+                                    int32_t* m_lcp, void* tape_, int checkpoint_every, float* grad_states, float* grad_actions, double* grad_inertia,
+                                    void* workspace, int32_t* status_accum, void* stream) {
   nb2_model* m = const_cast<nb2_model*>(cm);
   if (m && (B == 0 || T == 0)) return NB2_OK;
   if (!m || B < 0 || T < 0 || !states || (!actions && T > 0) || !x_lcp || !m_lcp || !tape_ || !grad_states || (!grad_actions && T > 0) || !workspace) {
@@ -1256,15 +1296,15 @@ int nb2_rollout_backward_contact(const nb2_model* cm, int B, int T, const float*
       if ((rc = snap_copy(tape, L, seg, x_lcp, m_lcp, B, true, st))) return rc;
       for (int t = t0; t < t1; t++) {
         double* slot = tape + L.o_slots + L.slot_doubles * (t - t0);
-        rc = nb2_step_forward_contact(m, B, states + n2 * B * t, actions + na * B * t, next_scratch, slot, workspace, x_lcp, m_lcp, labels, status, nc, nullptr,
-                                      slot + L.saved_doubles, nullptr, stream);
+        rc = nb2_step_forward_contact_pw(m, B, states + n2 * B * t, actions + na * B * t, world_inertia, next_scratch, slot, workspace, x_lcp, m_lcp, labels,
+                                         status, nc, nullptr, slot + L.saved_doubles, nullptr, stream);
         if (rc) return rc;
       }
     }
     for (int t = t1 - 1; t >= t0; t--) {
       const double* slot = tape + L.o_slots + L.slot_doubles * (t - t0);
       rc = cbwd_launch(m, B, states + n2 * B * t, actions + na * B * t, slot, slot + L.saved_doubles, workspace, grad_states + n2 * B * (t + 1),
-                       grad_states + n2 * B * t, grad_actions + na * B * t, nullptr, status_accum, st, 1);
+                       grad_states + n2 * B * t, grad_actions + na * B * t, nullptr, status_accum, st, 1, world_inertia, grad_inertia);
       if (rc) return rc;
     }
   }
@@ -1370,18 +1410,27 @@ int nb2_saved_words_per_world(const nb2_model* m) { return m ? m->saved_words : 
 
 int nb2_step_forward(const nb2_model* cm, int B, const float* state, const float* action, float* next_state,
                      void* saved, int precision, void* stream) {
+  return nb2_step_forward_pw(cm, B, state, action, nullptr, next_state, saved, precision, stream);
+}
+int nb2_step_forward_pw(const nb2_model* cm, int B, const float* state, const float* action, const double* world_inertia, float* next_state,
+                        void* saved, int precision, void* stream) {
   nb2_model* m = const_cast<nb2_model*>(cm);
   if (!m || B < 0 || !state || !action || !next_state) { g_err = "nb2_step_forward: bad argument"; return NB2_ERR_INVALID; }
   if (m->has_contacts) { g_err = "nb2_step_forward: the model has collision pairs: use nb2_step_forward_contact (or build the model without shapes for a contact-free step)"; return NB2_ERR_INVALID; }
   if (B == 0) return NB2_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  if (precision == NB2_FP64) return launch_fwd<double>(m, B, state, action, next_state, (double*)saved, st);
-  return launch_fwd<float>(m, B, state, action, next_state, (float*)saved, st);
+  if (precision == NB2_FP64) return launch_fwd<double>(m, B, state, action, next_state, (double*)saved, st, -1, 0, nullptr, nullptr, world_inertia);
+  return launch_fwd<float>(m, B, state, action, next_state, (float*)saved, st, -1, 0, nullptr, nullptr, world_inertia);
 }
 
 int nb2_step_backward(const nb2_model* cm, int B, const float* state, const float* action, const void* saved,
                       const float* grad_next_state, float* grad_state, float* grad_action, float* grad_inertia,
                       int precision, void* stream) {
+  return nb2_step_backward_pw(cm, B, state, action, nullptr, saved, grad_next_state, grad_state, grad_action, grad_inertia, precision, stream);
+}
+int nb2_step_backward_pw(const nb2_model* cm, int B, const float* state, const float* action, const double* world_inertia, const void* saved,
+                         const float* grad_next_state, float* grad_state, float* grad_action, float* grad_inertia,
+                         int precision, void* stream) {
   nb2_model* m = const_cast<nb2_model*>(cm);
   if (!m || B < 0 || !state || !action || !saved || !grad_next_state || !grad_state || !grad_action) {
     g_err = "nb2_step_backward: bad argument"; return NB2_ERR_INVALID;
@@ -1389,11 +1438,15 @@ int nb2_step_backward(const nb2_model* cm, int B, const float* state, const floa
   if (m->has_contacts) { g_err = "nb2_step_backward: the model has collision pairs: use nb2_step_backward_contact"; return NB2_ERR_INVALID; }
   if (B == 0) return NB2_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  if (precision == NB2_FP64) return launch_bwd<double>(m, B, state, action, (const double*)saved, grad_next_state, grad_state, grad_action, grad_inertia, st);
-  return launch_bwd<float>(m, B, state, action, (const float*)saved, grad_next_state, grad_state, grad_action, grad_inertia, st);
+  if (precision == NB2_FP64) return launch_bwd<double>(m, B, state, action, (const double*)saved, grad_next_state, grad_state, grad_action, grad_inertia, st, -1, 0, 0, world_inertia);
+  return launch_bwd<float>(m, B, state, action, (const float*)saved, grad_next_state, grad_state, grad_action, grad_inertia, st, -1, 0, 0, world_inertia);
 }
 
 int nb2_rollout_forward(const nb2_model* cm, int B, int T, float* states, const float* actions, void* saved, int precision, void* stream) {
+  return nb2_rollout_forward_pw(cm, B, T, states, actions, nullptr, saved, precision, stream);
+}
+int nb2_rollout_forward_pw(const nb2_model* cm, int B, int T, float* states, const float* actions, const double* world_inertia, void* saved, int precision,
+                           void* stream) {
   nb2_model* m = const_cast<nb2_model*>(cm);
   if (!m || B < 0 || T < 0 || !states || (!actions && T > 0)) { g_err = "nb2_rollout_forward: bad argument"; return NB2_ERR_INVALID; }
   if (m->has_contacts) { g_err = "nb2_rollout_forward: contact worlds roll out through nb2_step_forward_contact (one call per step)"; return NB2_ERR_INVALID; }
@@ -1402,7 +1455,7 @@ int nb2_rollout_forward(const nb2_model* cm, int B, int T, float* states, const 
   const size_t sv_step = (size_t)m->saved_words * B * (precision == NB2_FP64 ? sizeof(double) : sizeof(float));
   for (int t = 0; t < T; t++) {  // x_{t+1} = step(x_t, u_t): every launch reads the rows the previous one wrote (stream order)
     void* sv = saved ? (char*)saved + sv_step * t : nullptr;
-    int rc = nb2_step_forward(m, B, states + n2 * B * t, actions + na * B * t, states + n2 * B * (t + 1), sv, precision, stream);
+    int rc = nb2_step_forward_pw(m, B, states + n2 * B * t, actions + na * B * t, world_inertia, states + n2 * B * (t + 1), sv, precision, stream);
     if (rc) return rc;
   }
   return NB2_OK;
@@ -1410,6 +1463,10 @@ int nb2_rollout_forward(const nb2_model* cm, int B, int T, float* states, const 
 
 int nb2_rollout_backward(const nb2_model* cm, int B, int T, const float* states, const float* actions, const void* saved,
                          float* grad_states, float* grad_actions, int precision, void* stream) {
+  return nb2_rollout_backward_pw(cm, B, T, states, actions, nullptr, saved, grad_states, grad_actions, nullptr, precision, stream);
+}
+int nb2_rollout_backward_pw(const nb2_model* cm, int B, int T, const float* states, const float* actions, const double* world_inertia, const void* saved,
+                            float* grad_states, float* grad_actions, double* grad_inertia, int precision, void* stream) {
   nb2_model* m = const_cast<nb2_model*>(cm);
   if (!m || B < 0 || T < 0 || !states || !saved || !grad_states || (!actions && T > 0) || (!grad_actions && T > 0)) { g_err = "nb2_rollout_backward: bad argument"; return NB2_ERR_INVALID; }
   if (m->has_contacts) { g_err = "nb2_rollout_backward: contact worlds back-propagate through nb2_step_backward_contact"; return NB2_ERR_INVALID; }
@@ -1420,8 +1477,8 @@ int nb2_rollout_backward(const nb2_model* cm, int B, int T, const float* states,
   for (int t = T - 1; t >= 0; t--) {  // grad_states[t] += clip(J_t^T grad_states[t+1]) ; grad_actions[t] = ...
     const char* sv = (const char*)saved + sv_step * t;
     int rc;
-    if (precision == NB2_FP64) rc = launch_bwd<double>(m, B, states + n2 * B * t, actions + na * B * t, (const double*)sv, grad_states + n2 * B * (t + 1), grad_states + n2 * B * t, grad_actions + na * B * t, nullptr, st, -1, 0, 1);
-    else rc = launch_bwd<float>(m, B, states + n2 * B * t, actions + na * B * t, (const float*)sv, grad_states + n2 * B * (t + 1), grad_states + n2 * B * t, grad_actions + na * B * t, nullptr, st, -1, 0, 1);
+    if (precision == NB2_FP64) rc = launch_bwd<double>(m, B, states + n2 * B * t, actions + na * B * t, (const double*)sv, grad_states + n2 * B * (t + 1), grad_states + n2 * B * t, grad_actions + na * B * t, nullptr, st, -1, 0, 1, world_inertia, grad_inertia);
+    else rc = launch_bwd<float>(m, B, states + n2 * B * t, actions + na * B * t, (const float*)sv, grad_states + n2 * B * (t + 1), grad_states + n2 * B * t, grad_actions + na * B * t, nullptr, st, -1, 0, 1, world_inertia, grad_inertia);
     if (rc) return rc;
   }
   return NB2_OK;

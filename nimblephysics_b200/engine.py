@@ -100,33 +100,38 @@ class DeviceModel:
             pass
 
     # ---- device pointers (torch tensors on the current CUDA device) ----
-    def forward_device(self, B, state_ptr, action_ptr, next_ptr, saved_ptr, stream, precision=FP32):
-        _cabi.check(_cabi.lib().nb2_step_forward(self.handle, B, state_ptr, action_ptr, next_ptr, saved_ptr, precision, stream))
+    # wi_ptr (optional, every step / rollout call): per-world canonical inertia, fp64 [10*nb, B] (include/nb2.h nb2_step_forward_pw);
+    # None = the model's table.  A backward takes the same wi_ptr as its forward.
+    def forward_device(self, B, state_ptr, action_ptr, next_ptr, saved_ptr, stream, precision=FP32, wi_ptr=None):
+        _cabi.check(_cabi.lib().nb2_step_forward_pw(self.handle, B, state_ptr, action_ptr, wi_ptr, next_ptr, saved_ptr, precision, stream))
 
     def backward_device(self, B, state_ptr, action_ptr, saved_ptr, gnext_ptr, gstate_ptr, gaction_ptr, stream,
-                        precision=FP32, ginertia_ptr=None):
+                        precision=FP32, ginertia_ptr=None, wi_ptr=None):
         """ginertia_ptr: optional [10*nb, B] float32 buffer receiving dL/d(inertia parameters) per body and world."""
-        _cabi.check(_cabi.lib().nb2_step_backward(self.handle, B, state_ptr, action_ptr, saved_ptr, gnext_ptr,
-                                                  gstate_ptr, gaction_ptr, ginertia_ptr, precision, stream))
+        _cabi.check(_cabi.lib().nb2_step_backward_pw(self.handle, B, state_ptr, action_ptr, wi_ptr, saved_ptr, gnext_ptr,
+                                                     gstate_ptr, gaction_ptr, ginertia_ptr, precision, stream))
 
-    def rollout_forward_device(self, B, T, states_ptr, actions_ptr, saved_ptr, stream, precision=FP32):
-        _cabi.check(_cabi.lib().nb2_rollout_forward(self.handle, B, T, states_ptr, actions_ptr, saved_ptr, precision, stream))
+    def rollout_forward_device(self, B, T, states_ptr, actions_ptr, saved_ptr, stream, precision=FP32, wi_ptr=None):
+        _cabi.check(_cabi.lib().nb2_rollout_forward_pw(self.handle, B, T, states_ptr, actions_ptr, wi_ptr, saved_ptr, precision, stream))
 
-    def rollout_backward_device(self, B, T, states_ptr, actions_ptr, saved_ptr, gstates_ptr, gactions_ptr, stream, precision=FP32):
-        _cabi.check(_cabi.lib().nb2_rollout_backward(self.handle, B, T, states_ptr, actions_ptr, saved_ptr, gstates_ptr,
-                                                     gactions_ptr, precision, stream))
+    def rollout_backward_device(self, B, T, states_ptr, actions_ptr, saved_ptr, gstates_ptr, gactions_ptr, stream, precision=FP32,
+                                wi_ptr=None, ginertia_ptr=None):
+        """ginertia_ptr: optional [10*nb, B] float64 buffer to which every step ADDS its dL/d(inertia parameters)."""
+        _cabi.check(_cabi.lib().nb2_rollout_backward_pw(self.handle, B, T, states_ptr, actions_ptr, wi_ptr, saved_ptr, gstates_ptr,
+                                                        gactions_ptr, ginertia_ptr, precision, stream))
 
     def rollout_contact_tape_bytes(self, B, T, checkpoint_every):
         return int(_cabi.lib().nb2_rollout_contact_tape_bytes(self.handle, B, T, checkpoint_every))
 
-    def rollout_forward_contact_device(self, B, T, states_ptr, actions_ptr, x_ptr, m_ptr, tape_ptr, checkpoint_every, ws_ptr, sticky_ptr, stream):
-        _cabi.check(_cabi.lib().nb2_rollout_forward_contact(self.handle, B, T, states_ptr, actions_ptr, x_ptr, m_ptr, tape_ptr, checkpoint_every,
-                                                            ws_ptr, sticky_ptr, stream))
+    def rollout_forward_contact_device(self, B, T, states_ptr, actions_ptr, x_ptr, m_ptr, tape_ptr, checkpoint_every, ws_ptr, sticky_ptr, stream,
+                                       wi_ptr=None):
+        _cabi.check(_cabi.lib().nb2_rollout_forward_contact_pw(self.handle, B, T, states_ptr, actions_ptr, wi_ptr, x_ptr, m_ptr, tape_ptr,
+                                                               checkpoint_every, ws_ptr, sticky_ptr, stream))
 
     def rollout_backward_contact_device(self, B, T, states_ptr, actions_ptr, x_ptr, m_ptr, tape_ptr, checkpoint_every, gstates_ptr, gactions_ptr,
-                                        ws_ptr, sticky_ptr, stream):
-        _cabi.check(_cabi.lib().nb2_rollout_backward_contact(self.handle, B, T, states_ptr, actions_ptr, x_ptr, m_ptr, tape_ptr, checkpoint_every,
-                                                             gstates_ptr, gactions_ptr, ws_ptr, sticky_ptr, stream))
+                                        ws_ptr, sticky_ptr, stream, wi_ptr=None, ginertia_ptr=None):
+        _cabi.check(_cabi.lib().nb2_rollout_backward_contact_pw(self.handle, B, T, states_ptr, actions_ptr, wi_ptr, x_ptr, m_ptr, tape_ptr,
+                                                                checkpoint_every, gstates_ptr, gactions_ptr, ginertia_ptr, ws_ptr, sticky_ptr, stream))
 
     def forward_dynamics(self, pos, vel, force):
         """q-ddot [B, n] (float64 CUDA tensors in and out): pointer-style ABA, no integration, no contact stage
@@ -149,16 +154,16 @@ class DeviceModel:
         return int(_cabi.lib().nb2_contact_record_bytes(self.handle, B))
 
     def forward_contact_device(self, B, state_ptr, action_ptr, next_ptr, saved_ptr, ws_ptr, x_ptr, m_ptr, labels_ptr,
-                               status_ptr, nc_ptr, cinfo_ptr, crec_ptr, status_accum_ptr, stream):
+                               status_ptr, nc_ptr, cinfo_ptr, crec_ptr, status_accum_ptr, stream, wi_ptr=None):
         """fused fp64 step with the contact / boxed-LCP stage, one warp per world (include/nb2.h nb2_step_forward_contact)."""
-        _cabi.check(_cabi.lib().nb2_step_forward_contact(self.handle, B, state_ptr, action_ptr, next_ptr, saved_ptr, ws_ptr, x_ptr,
-                                                         m_ptr, labels_ptr, status_ptr, nc_ptr, cinfo_ptr, crec_ptr, status_accum_ptr, stream))
+        _cabi.check(_cabi.lib().nb2_step_forward_contact_pw(self.handle, B, state_ptr, action_ptr, wi_ptr, next_ptr, saved_ptr, ws_ptr, x_ptr,
+                                                            m_ptr, labels_ptr, status_ptr, nc_ptr, cinfo_ptr, crec_ptr, status_accum_ptr, stream))
 
     def backward_contact_device(self, B, state_ptr, action_ptr, saved_ptr, crec_ptr, ws_ptr, gnext_ptr, gstate_ptr, gaction_ptr,
-                                stream, ginertia_ptr=None, status_ptr=None):
+                                stream, ginertia_ptr=None, status_ptr=None, wi_ptr=None):
         """status_ptr: the forward's status array; worlds that cannot be back-propagated get bit 2048 (and NaN gradients)."""
-        _cabi.check(_cabi.lib().nb2_step_backward_contact(self.handle, B, state_ptr, action_ptr, saved_ptr, crec_ptr, ws_ptr,
-                                                          gnext_ptr, gstate_ptr, gaction_ptr, ginertia_ptr, status_ptr, stream))
+        _cabi.check(_cabi.lib().nb2_step_backward_contact_pw(self.handle, B, state_ptr, action_ptr, wi_ptr, saved_ptr, crec_ptr, ws_ptr,
+                                                             gnext_ptr, gstate_ptr, gaction_ptr, ginertia_ptr, status_ptr, stream))
 
     def set_contact_capacity(self, max_contacts: int):
         _cabi.check(_cabi.lib().nb2_model_set_contact_capacity(self.handle, int(max_contacts)))

@@ -378,6 +378,90 @@ def inertia_param_jacobian(raw: RawModel, cm: "CanonModel", entries) -> np.ndarr
     return np.array(rows).reshape(len(rows), cm.nb * 10)
 
 
+def _mass_map_constants(world, raw: RawModel, cm: "CanonModel", device):
+    """What mass_to_inertia needs besides the mass vectors, as tensors on `device`: the canonical table of every body that is NOT
+    registered with tuneMass (fixed), and per registered body its current (mass, com, moment), its frame in the owner and the
+    mass-vector columns that overwrite those values."""
+    import torch
+
+    entries = world._mass_entries()
+    reg = {bi for bi, _ in entries}
+    cur = {i: (raw.mass[i], raw.com[i], raw.moment[i]) for i in range(raw.nb)}
+    base = np.zeros((cm.nb, 10))
+    for i in range(raw.nb):
+        o = int(cm.body_owner[i])
+        if o >= 0 and i not in reg:
+            base[o] += body_inertia_contribution(cm.body_T[i], *cur[i])
+    E = len(entries)
+    p0 = np.zeros((E, 10))       # (mass, com(3), moment(6)) before the mass vector is applied
+    Rs, ps = np.zeros((E, 3, 3)), np.zeros((E, 3))
+    owner = np.zeros((cm.nb, E))  # one-hot: canonical body <- registered raw body (0 for static bodies)
+    dst, src, scaled = [], [], []  # columns of the mass vector -> (entry, parameter) slots; INERTIA_MASS entries whose moment scales
+    col = 0
+    for e, (bi, kind) in enumerate(entries):
+        m0, c0, mom0 = cur[bi]
+        p0[e] = np.concatenate([[m0], c0, mom0])
+        T = cm.body_T[bi]
+        Rs[e], ps[e] = T[:3, :3], T[:3, 3]
+        if cm.body_owner[bi] >= 0:
+            owner[int(cm.body_owner[bi]), e] = 1.0
+        slots = {INERTIA_MASS: [0], INERTIA_COM: [1, 2, 3], INERTIA_DIAGONAL: [4, 5, 6], INERTIA_OFF_DIAGONAL: [7, 8, 9],
+                 INERTIA_FULL: list(range(10))}.get(kind)
+        if slots is None:
+            raise NotImplementedError("INERTIA_COM_MU needs BodyNode::getBeta(), which this builder surface does not carry")
+        dst += [10 * e + s for s in slots]
+        src += list(range(col, col + len(slots)))
+        if kind == INERTIA_MASS and m0 > 0 and np.any(mom0 != 0):  # Inertia::setMass keeps the body's dimensions (_apply_mass_entry)
+            scaled.append((e, col))
+        col += len(slots)
+    t = lambda a, dt=torch.float64: torch.as_tensor(np.asarray(a), dtype=dt, device=device)
+    return dict(base=t(base), p0=t(p0), R=t(Rs), p=t(ps), owner=t(owner), dst=t(dst, torch.long), src=t(src, torch.long),
+                sc_e=t([e for e, _ in scaled], torch.long), sc_col=t([c for _, c in scaled], torch.long))
+
+
+def mass_to_inertia(world, mass):
+    """Per-world canonical inertia of B mass vectors: mass [B, getMassDims()] -> [B, nb, 10] float64 on mass's device, row w = the
+    (m, h, Ibar) table that world.setMasses(mass[w]) followed by DeviceModel.refresh_inertia would produce from the World's current
+    body parameters (INERTIA_MASS scales the moment by mass[w] / current mass).  The World is not modified.  Written in torch, so autograd
+    carries a gradient with respect to the table (the kernels' per-world grad_inertia) back to `mass`.  The bodies that are not registered
+    are folded into a constant table that is rebuilt only when the model or the body parameters change."""
+    import torch
+
+    from .world import edit_epoch
+
+    if mass.dim() != 2 or mass.shape[1] != world.getMassDims():
+        raise ValueError(f"mass_to_inertia(): mass has shape {tuple(mass.shape)}, expected [B, {world.getMassDims()}] (= getMassDims())")
+    regs = [(id(b), t, b.mass, np.asarray(b.com).tobytes(), np.asarray(b.moment).tobytes()) for b, t, _, _ in getattr(world, "_wrt_mass", [])]
+    key = (edit_epoch(), tuple(regs), str(mass.device))
+    c = getattr(world, "_mass_map", None)
+    if c is None or c[0] != key:
+        raw = flatten_world(world)  # the current body parameters; the canonical numbering is the device model's (any lane count)
+        c = (key, _mass_map_constants(world, raw, compile_model(raw), mass.device))
+        world._mass_map = c
+    K = c[1]
+    B, E = mass.shape[0], K["p0"].shape[0]
+    x = mass.to(torch.float64)
+    prm = K["p0"].reshape(1, E * 10).expand(B, E * 10).clone()
+    prm[:, K["dst"]] = x[:, K["src"]]
+    prm = prm.reshape(B, E, 10)
+    if K["sc_e"].numel():
+        mom = prm[:, :, 4:].clone()
+        mom[:, K["sc_e"]] = K["p0"][K["sc_e"], 4:] * (x[:, K["sc_col"]] / K["p0"][K["sc_e"], 0]).unsqueeze(-1)
+        prm = torch.cat([prm[:, :, :4], mom], -1)
+    m, com, m6 = prm[..., 0], prm[..., 1:4], prm[..., 4:]
+    # body_inertia_contribution, batched: c = R com + p ; Ibar = R Ic R^T + m (|c|^2 1 - c c^T) ; h = m c
+    Ic = torch.stack([m6[..., 0], m6[..., 3], m6[..., 4], m6[..., 3], m6[..., 1], m6[..., 5], m6[..., 4], m6[..., 5], m6[..., 2]], -1).reshape(B, E, 3, 3)
+    cw = torch.einsum("eij,bej->bei", K["R"], com) + K["p"]
+    RIR = K["R"] @ Ic @ K["R"].transpose(-1, -2)
+    cc = (cw * cw).sum(-1)
+    I3 = torch.eye(3, dtype=torch.float64, device=mass.device)
+    Ibar = RIR + m[..., None, None] * (cc[..., None, None] * I3 - cw[..., :, None] * cw[..., None, :])
+    h = m[..., None] * cw
+    contrib = torch.stack([m, h[..., 0], h[..., 1], h[..., 2], Ibar[..., 0, 0], Ibar[..., 1, 1], Ibar[..., 2, 2],
+                           Ibar[..., 0, 1], Ibar[..., 0, 2], Ibar[..., 1, 2]], -1)      # [B, E, 10]
+    return K["base"] + torch.einsum("ke,bej->bkj", K["owner"], contrib)
+
+
 def _ranges(idx):
     """sorted indices -> list of contiguous [lo, hi) ranges"""
     out = []

@@ -13,16 +13,18 @@ from typing import Callable, List, Optional, Sequence, Tuple
 
 import torch
 
-from .timestep import timestep
+from .timestep import TimestepLayer, per_world_inertia, timestep
 
 
-def rollout(world, state0: torch.Tensor, actions: Sequence[torch.Tensor], keep_states: bool = False):
-    """Unroll len(actions) differentiable steps.  state0: [B, 2n]; actions[t]: [B, a].
+def rollout(world, state0: torch.Tensor, actions: Sequence[torch.Tensor], keep_states: bool = False, mass: Optional[torch.Tensor] = None):
+    """Unroll len(actions) differentiable steps.  state0: [B, 2n]; actions[t]: [B, a]; mass: as for timestep() (a 2-D [B, m] mass is
+    mapped to the per-world inertia once and held constant over the horizon).
     Returns the final state (and the list of intermediate states when keep_states)."""
     x = state0
     states: List[torch.Tensor] = []
+    wi = per_world_inertia(world, state0, mass) if mass is not None and mass.dim() == 2 else None
     for a in actions:
-        x = timestep(world, x, a)
+        x = TimestepLayer.apply(world, x, a, None, wi) if wi is not None else timestep(world, x, a, mass)
         if keep_states:
             states.append(x)
     return (x, states) if keep_states else x
@@ -34,7 +36,7 @@ class _FusedRollout(torch.autograd.Function):
     autograd sees a single node instead of T."""
 
     @staticmethod
-    def forward(ctx, world, state0, actions):
+    def forward(ctx, world, state0, actions, world_inertia=None):
         from .engine import FP32, device_model_for
 
         dm = device_model_for(world)
@@ -46,29 +48,33 @@ class _FusedRollout(torch.autograd.Function):
         states = torch.empty((T + 1, B, n2), dtype=torch.float32, device=dev)
         states[0].copy_(state0.detach())
         acts = actions.detach().to(dtype=torch.float32).contiguous()
-        need = any(ctx.needs_input_grad[1:3])
+        wi = _word_major_inertia(dm, world_inertia, B, dev)
+        need = any(ctx.needs_input_grad[1:4])
         saved = torch.empty((T, dm.saved_words, B), dtype=torch.float32, device=dev) if need else None
         with torch.cuda.device(dev):
             dm.rollout_forward_device(B, T, states.data_ptr(), acts.data_ptr(), saved.data_ptr() if need else None,
-                                      torch.cuda.current_stream().cuda_stream, FP32)
+                                      torch.cuda.current_stream().cuda_stream, FP32, wi_ptr=wi.data_ptr() if wi is not None else None)
         ctx.dm, ctx.T, ctx.B = dm, T, B
         ctx.dtypes = (state0.dtype, actions.dtype)
+        ctx.wi_like = world_inertia
         if need:
-            ctx.save_for_backward(states, acts, saved)
+            ctx.save_for_backward(states, acts, saved, wi)
         return states.to(state0.dtype)
 
     @staticmethod
     def backward(ctx, grad_states):
         from .engine import FP32
 
-        states, acts, saved = ctx.saved_tensors
+        states, acts, saved, wi = ctx.saved_tensors
         dm, T, B = ctx.dm, ctx.T, ctx.B
         gs = grad_states.detach().to(dtype=torch.float32).contiguous().clone()  # in: loss gradient per state; out: total dL/dx_t
         ga = torch.empty_like(acts)
+        gi = torch.zeros((10 * dm.cm.nb, B), dtype=torch.float64, device=states.device) if ctx.needs_input_grad[3] else None
         with torch.cuda.device(states.device):
             dm.rollout_backward_device(B, T, states.data_ptr(), acts.data_ptr(), saved.data_ptr(), gs.data_ptr(), ga.data_ptr(),
-                                       torch.cuda.current_stream().cuda_stream, FP32)
-        return None, gs[0].to(ctx.dtypes[0]), ga.to(ctx.dtypes[1])
+                                       torch.cuda.current_stream().cuda_stream, FP32, wi_ptr=wi.data_ptr() if wi is not None else None,
+                                       ginertia_ptr=gi.data_ptr() if gi is not None else None)
+        return None, gs[0].to(ctx.dtypes[0]), ga.to(ctx.dtypes[1]), _inertia_grad(gi, ctx.wi_like)
 
 
 class _ContactRollout(torch.autograd.Function):
@@ -77,7 +83,7 @@ class _ContactRollout(torch.autograd.Function):
     (saved streams + contact records) is one device buffer, optionally checkpointed every k steps."""
 
     @staticmethod
-    def forward(ctx, world, state0, actions, checkpoint_every):
+    def forward(ctx, world, state0, actions, checkpoint_every, world_inertia=None):
         from .engine import device_model_for
         from .timestep import contact_cache
 
@@ -95,42 +101,68 @@ class _ContactRollout(torch.autograd.Function):
         k = int(checkpoint_every or 0)
         cache = contact_cache(world, B, dev)
         tape = torch.empty((dm.rollout_contact_tape_bytes(B, T, k) // 8,), dtype=torch.float64, device=dev)
+        wi = _word_major_inertia(dm, world_inertia, B, dev)
         with torch.cuda.device(dev):
             dm.rollout_forward_contact_device(B, T, states.data_ptr(), acts.data_ptr(), cache["x"].data_ptr(), cache["m"].data_ptr(), tape.data_ptr(), k,
-                                              cache["ws"].data_ptr(), cache["sticky"].data_ptr(), torch.cuda.current_stream().cuda_stream)
+                                              cache["ws"].data_ptr(), cache["sticky"].data_ptr(), torch.cuda.current_stream().cuda_stream,
+                                              wi_ptr=wi.data_ptr() if wi is not None else None)
         ctx.dm, ctx.T, ctx.B, ctx.k, ctx.cache = dm, T, B, k, cache
         ctx.dtypes = (state0.dtype, actions.dtype)
         ctx.peak_tape_bytes = tape.numel() * 8
-        if any(ctx.needs_input_grad[1:3]):
-            ctx.save_for_backward(states, acts, tape)
+        ctx.wi_like = world_inertia
+        if any(ctx.needs_input_grad[1:3]) or ctx.needs_input_grad[4]:
+            ctx.save_for_backward(states, acts, tape, wi)
         return states.to(state0.dtype)
 
     @staticmethod
     def backward(ctx, grad_states):
-        states, acts, tape = ctx.saved_tensors
+        states, acts, tape, wi = ctx.saved_tensors
         dm, T, B, cache = ctx.dm, ctx.T, ctx.B, ctx.cache
         gs = grad_states.detach().to(dtype=torch.float32).contiguous().clone()  # in: loss gradient per state; out: total dL/dx_t
         ga = torch.empty_like(acts)
+        gi = torch.zeros((10 * dm.cm.nb, B), dtype=torch.float64, device=states.device) if ctx.needs_input_grad[4] else None
         with torch.cuda.device(states.device):
             dm.rollout_backward_contact_device(B, T, states.data_ptr(), acts.data_ptr(), cache["x"].data_ptr(), cache["m"].data_ptr(), tape.data_ptr(),
                                                ctx.k, gs.data_ptr(), ga.data_ptr(), cache["ws"].data_ptr(), cache["sticky"].data_ptr(),
-                                               torch.cuda.current_stream().cuda_stream)
-        return None, gs[0].to(ctx.dtypes[0]), ga.to(ctx.dtypes[1]), None
+                                               torch.cuda.current_stream().cuda_stream, wi_ptr=wi.data_ptr() if wi is not None else None,
+                                               ginertia_ptr=gi.data_ptr() if gi is not None else None)
+        return None, gs[0].to(ctx.dtypes[0]), ga.to(ctx.dtypes[1]), None, _inertia_grad(gi, ctx.wi_like)
 
 
-def rollout_fused(world, state0: torch.Tensor, actions: torch.Tensor, checkpoint_every: int = 0) -> torch.Tensor:
+def _word_major_inertia(dm, world_inertia, B, dev):
+    """[B, nb, 10] per-world inertia -> the kernels' word-major [10*nb, B] fp64 layout on `dev` (None stays None)."""
+    if world_inertia is None:
+        return None
+    return world_inertia.detach().to(device=dev, dtype=torch.float64).reshape(B, 10 * dm.cm.nb).t().contiguous()
+
+
+def _inertia_grad(gi, like):
+    """[10*nb, B] gradient summed over the horizon -> the [B, nb, 10] layout (dtype, device) of the per-world inertia input."""
+    if gi is None:
+        return None
+    return gi.t().reshape(like.shape).to(device=like.device, dtype=like.dtype)
+
+
+def rollout_fused(world, state0: torch.Tensor, actions: torch.Tensor, checkpoint_every: int = 0, mass: Optional[torch.Tensor] = None) -> torch.Tensor:
     """states[T+1, B, 2n] of the T-step rollout x_{t+1} = timestep(x_t, actions[t])
     (SingleShot::getSnapshots, dart/trajectory/SingleShot.cpp:635-686), differentiable with respect to state0 and every
     action (SingleShot::backpropGradientWrt, :539-631); losses may look at any state of the trajectory.  One C call per direction.
     Worlds with collision pairs run the contact / boxed-LCP stage every step with the world's LCP cache flowing exactly as when
     chaining timestep() (bit-identical states and gradients); `checkpoint_every=k` keeps the backward tape of k steps instead of T and
     re-runs each segment's forward in the reverse sweep.  Problems (dropped contacts, worlds that cannot be back-propagated) are
-    reported by check_contact_status(world), one host sync per rollout."""
+    reported by check_contact_status(world), one host sync per rollout.
+    mass (optional) [B, getMassDims()]: world w rolls out with masses mass[w], constant over the horizon; mass.grad sums over the steps
+    (bit-identical to rollout(..., mass=)); the World is not modified."""
     from .engine import device_model_for
 
+    wi = None
+    if mass is not None:
+        if mass.dim() != 2:
+            raise ValueError(f"rollout_fused(): mass must be [B, getMassDims()], got shape {tuple(mass.shape)}")
+        wi = per_world_inertia(world, state0, mass)
     if device_model_for(world).has_contacts:
-        return _ContactRollout.apply(world, state0, actions, checkpoint_every)
-    return _FusedRollout.apply(world, state0, actions)
+        return _ContactRollout.apply(world, state0, actions, checkpoint_every, wi)
+    return _FusedRollout.apply(world, state0, actions, wi)
 
 
 def rollout_tape_bytes(world, B: int, T: int, checkpoint_every: int = 0) -> int:
