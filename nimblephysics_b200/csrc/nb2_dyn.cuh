@@ -144,7 +144,6 @@ template <class R> NB2_HD void inertia_of(const Nb2ModelDev<R>& M, const R* bt, 
   Ib->xx = M.inertia[i][4]; Ib->yy = M.inertia[i][5]; Ib->zz = M.inertia[i][6];
   Ib->xy = M.inertia[i][7]; Ib->xz = M.inertia[i][8]; Ib->yz = M.inertia[i][9];
 }
-template <class R> NB2_HD void inertia_of(const Nb2ModelDev<R>& M, int i, R* m, V3<R>* h, S3<R>* Ib) { inertia_of<R>(M, (const R*)nullptr, nullptr, 0, i, m, h, Ib); }
 template <class R, int ST> NB2_HD Xf<R> ldXf(const R* p) {
   Xf<R> T;
   T.R_.m00 = p[0]; T.R_.m01 = p[ST]; T.R_.m02 = p[2 * ST]; T.R_.m10 = p[3 * ST]; T.R_.m11 = p[4 * ST]; T.R_.m12 = p[5 * ST];
@@ -502,16 +501,6 @@ NB2_HD void world_forward_stage(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B
     else if (pass == 2) fwd_pass2<R, ST>(M, scr, sv, B, save, lo, hi, bt, iinv_out, wi, wiB);
     else fwd_pass3<R, ST>(M, scr, sv, B, save, lo, hi, bt);
   }
-}
-
-// single-thread convenience (any model: one thread plays every lane in turn)
-template <class R, int ST>
-NB2_HD void world_forward(const Nb2ModelDev<R>& M, R* scr, const float* st, const float* act, float* out, R* sv,
-                          size_t B, bool save) {
-  fwd_load<R, ST>(M, scr, st, act, 1, 0, 1);
-  for (int sg = 1; sg < NB2_FWD_STAGES - 1; sg++)
-    for (int lane = 0; lane < M.lanes; lane++) world_forward_stage<R, ST>(M, scr, sv, B, save, lane, sg);
-  fwd_store<R, ST>(M, scr, out, 1, 0, 1);
 }
 
 // what the contact-stage adjoint (nb2_cw.cuh, contact_backward) hands to the reverse sweep B3 / the assembly: per-world arrays
@@ -893,6 +882,15 @@ NB2_HD void bwd_store(const Nb2ModelDev<R>& M, const R* scr0, float* gstate0, fl
 #define NB2_BWD_STAGES 10
 #define NB2_BWD_SYNC_MASK 0x14Bu        /* after stages 0, 1, 3, 6, 8 */
 #define NB2_BWD_SYNC_MASK_1LANE 0x101u  /* lanes == 1: after the group load and before the group store */
+// The fused contact backward (k_cstep_bwd, and the host harness that emulates it) walks stages 1..8 in this order over
+// NB2_CBWD_ITERS iterations: B1 limbs, B1 trunk, B2 trunk, B2 limbs | contact adjoint (before iteration 4) | B3 limbs, B3 trunk |
+// iterations 6, 7: the SECOND B3 over limbs and trunk of a world in which restitution was active (see contact_backward) |
+// assembly limbs, trunk.
+#define NB2_CBWD_ITERS 10
+struct CBwdIter { int stage; bool second; };
+NB2_HD constexpr CBwdIter cbwd_iter(int it) {
+  return {(it < 4) ? it + 1 : (it == 4 || it == 6) ? 5 : (it == 5 || it == 7) ? 7 : (it == 8) ? 6 : 8, static_cast<bool>((it == 6) | (it == 7))};
+}
 template <class R, int ST, bool CONTACT = false>
 NB2_HD void world_backward_stage(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, int lane, int stage, float* gI = nullptr, const R* bt = nullptr,
                                  size_t gIB = 0, const BwdContactData<ST>* cdp = nullptr, const double* wi = nullptr, size_t wiB = 0,
@@ -913,20 +911,6 @@ NB2_HD void world_backward_stage(const Nb2ModelDev<R>& M, R* scr, const R* sv, s
     else if (pass == 3) bwd_B3<R, ST, CONTACT>(M, scr, st, sv, B, cd, lo, hi, gI, bt, gIB ? gIB : B, wi, wiB, gIa);
     else bwd_assemble<R, ST, CONTACT>(M, scr, st, cd, lo, hi);
   }
-}
-
-// single-thread backward of a contact-free step (any schedule: one thread sweeps all bodies in order)
-template <class R, int ST>
-NB2_HD void world_backward(const Nb2ModelDev<R>& M, R* scr, const float* st, const float* act, const float* gnext,
-                           const R* sv, size_t B, float* gstate, float* gaction, float* gI = nullptr) {
-  const int nb = M.nb;
-  bwd_load<R, ST, false>(M, scr, st, act, gnext, 1, 0, 1);
-  bwd_B1<R, ST, false>(M, scr, st, sv, B, 0, nb);
-  bwd_B2<R, ST, false>(M, scr, st, sv, B, 0, nb);
-  BwdContactData<ST> cd; cd.active = 0; cd.error = 0; cd.inj_of_body = nullptr;
-  bwd_B3<R, ST, false>(M, scr, st, sv, B, cd, 0, nb, gI, (const R*)nullptr, B);
-  bwd_assemble<R, ST, false>(M, scr, st, cd, 0, nb);
-  bwd_store<R, ST, false>(M, scr, gstate, gaction, false, 1, 0, 1);
 }
 
 }  // namespace nb2

@@ -12,6 +12,7 @@
 #include <atomic>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/nb2.h"
@@ -225,6 +226,13 @@ k_step_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
 // (the saved stream, world-major, and a ~1 KB record).  Backward: the lambda sweeps, the contact adjoint, the reverse RNEA sweep.
 // Blocks are one warp: no block-level barrier exists in these kernels, and a warp whose world is out of range simply leaves.
 #define NB2_WS_DESC_DOUBLES ((int)((sizeof(nb2::cw::Ws) + 15) / 16 * 2))  // the workspace descriptor sits in front of the arrays
+// the warp's contact workspace at `at`: lane 0 carves the arrays after the descriptor and writes it, the warp syncs before reading it
+__device__ __forceinline__ nb2::cw::Ws* warp_workspace(void* at, const nb2::cw::Dims& d, int lane) {
+  nb2::cw::Ws* wsm = reinterpret_cast<nb2::cw::Ws*>(at);
+  if (lane == 0) *wsm = nb2::cw::carve(reinterpret_cast<double*>(wsm) + NB2_WS_DESC_DOUBLES, d);
+  __syncwarp();
+  return wsm;
+}
 #ifndef NB2_CSTEP_MINB
 #define NB2_CSTEP_MINB 1   // resident warps per SM the register allocation of the fused contact kernels aims at
 #endif
@@ -251,10 +259,7 @@ k_cstep_fwd(const __grid_constant__ Nb2ModelDev<double> M, const __grid_constant
   if (w >= P.B) return;
   const double* wi = winertia ? winertia + w : nullptr;
   double* scr = reinterpret_cast<double*>(nb2_smem);
-  nb2::cw::Ws* wsm = reinterpret_cast<nb2::cw::Ws*>(scr + ((P.fwd_words + 1) & ~1));
-  double* wsb = reinterpret_cast<double*>(wsm) + NB2_WS_DESC_DOUBLES;
-  if (lane == 0) *wsm = nb2::cw::carve(wsb, P.ds);
-  __syncwarp();
+  nb2::cw::Ws* wsm = warp_workspace(scr + ((P.fwd_words + 1) & ~1), P.ds, lane);
   const nb2::cw::Ws& ws0 = *wsm;
   const float* st = state + (size_t)w * 2 * M.ndof;
   double* sv = saved ? saved + (size_t)w * P.saved_words : nullptr;
@@ -295,10 +300,7 @@ k_cbuild(const __grid_constant__ Nb2ModelDev<double> M, const __grid_constant__ 
   const int wc = live ? w : P.B - 1;  // a warp without a world redoes the last one (reads only) so that it walks the same code
   const double* wi = winertia ? winertia + wc : nullptr;
   double* scr = reinterpret_cast<double*>(nb2_smem + (size_t)warp * smem_per_warp);
-  nb2::cw::Ws* wsm = reinterpret_cast<nb2::cw::Ws*>(scr + ((P.fwd_words + 1) & ~1));
-  double* wsb = reinterpret_cast<double*>(wsm) + NB2_WS_DESC_DOUBLES;
-  if (lane == 0) *wsm = nb2::cw::carve(wsb, P.ds);
-  __syncwarp();
+  nb2::cw::Ws* wsm = warp_workspace(scr + ((P.fwd_words + 1) & ~1), P.ds, lane);
   const nb2::cw::Ws& ws0 = *wsm;
   const float* st = state + (size_t)wc * 2 * M.ndof;
   double* sv = live ? saved + (size_t)w * P.saved_words : nullptr;
@@ -343,10 +345,7 @@ k_csolve(const __grid_constant__ Nb2ContactDev C, const __grid_constant__ CStepA
     w = live ? todo[idx] : 0;
   }
   double* X = live ? P.exch + (size_t)w * P.exch_stride : nullptr;
-  nb2::cw::Ws* wsm = reinterpret_cast<nb2::cw::Ws*>(nb2_smem + (size_t)warp * smem_per_warp);
-  double* wsb = reinterpret_cast<double*>(wsm) + NB2_WS_DESC_DOUBLES;
-  if (lane == 0) *wsm = nb2::cw::carve(wsb, P.ds_solve);
-  __syncwarp();
+  nb2::cw::Ws* wsm = warp_workspace(nb2_smem + (size_t)warp * smem_per_warp, P.ds_solve, lane);
   nb2::cw::FwdIO io;
   const int wc = live ? w : 0;
   io.x_io = x_lcp + (size_t)wc * NB2_MAX_ROWS; io.m_io = m_lcp + wc; io.labels = labels + (size_t)wc * NB2_MAX_ROWS; io.status = status + wc;
@@ -365,10 +364,7 @@ k_capply(const __grid_constant__ Nb2ModelDev<double> M, const __grid_constant__ 
   const bool live = w < P.B;
   const int wc = live ? w : 0;
   const double* X = live ? P.exch + (size_t)w * P.exch_stride : nullptr;
-  nb2::cw::Ws* wsm = reinterpret_cast<nb2::cw::Ws*>(nb2_smem + (size_t)warp * smem_per_warp);
-  double* wsb = reinterpret_cast<double*>(wsm) + NB2_WS_DESC_DOUBLES;
-  if (lane == 0) *wsm = nb2::cw::carve(wsb, P.ds_apply);
-  __syncwarp();
+  nb2::cw::Ws* wsm = warp_workspace(nb2_smem + (size_t)warp * smem_per_warp, P.ds_apply, lane);
   nb2::cw::FwdIO io;
   io.x_io = x_lcp + (size_t)wc * NB2_MAX_ROWS; io.m_io = nullptr; io.labels = labels + (size_t)wc * NB2_MAX_ROWS; io.status = nullptr;
   io.nc = nullptr; io.cinfo = nullptr; io.rec = crec ? crec + (size_t)wc * P.rec_doubles : nullptr;
@@ -390,9 +386,8 @@ k_cstep_bwd(const __grid_constant__ Nb2ModelDev<double> M, const __grid_constant
   const bool live = w < P.B;
   const int wc = live ? w : P.B - 1;  // a warp without a world redoes the last one without storing anything
   double* scr = reinterpret_cast<double*>(nb2_smem + (size_t)warp * smem_per_warp);
-  nb2::cw::Ws* wsm = reinterpret_cast<nb2::cw::Ws*>(scr + ((P.bwd_words + 1) & ~1));
+  nb2::cw::Ws* wsm = warp_workspace(scr + ((P.bwd_words + 1) & ~1), P.ds, lane);
   double* wsb = reinterpret_cast<double*>(wsm) + NB2_WS_DESC_DOUBLES;
-  if (lane == 0) *wsm = nb2::cw::carve(wsb, P.ds);
   const float* st = state + (size_t)wc * 2 * M.ndof;
   // when shared memory allows it WITHOUT costing a resident world, the world's saved stream (world-major, ~5 KB) is pulled into shared
   // memory by one bulk copy (TMA) while the group load runs: the sweeps walk it body by body, each a dependent L2 / DRAM round trip
@@ -414,14 +409,12 @@ k_cstep_bwd(const __grid_constant__ Nb2ModelDev<double> M, const __grid_constant
   float* gI = (ginertia && live) ? ginertia + w : nullptr;
   double* gIa = (ginertia_acc && live) ? ginertia_acc + w : nullptr;
   const double* wi = winertia ? winertia + wc : nullptr;
-  // stage order: B1 limbs, B1 trunk, B2 trunk, B2 limbs | contact adjoint | B3 limbs, B3 trunk | (worlds in which restitution was active: a
-  // SECOND B3 over limbs and trunk, see contact_backward) | assembly limbs, trunk.  One call site for all of them (code size), one block-wide
-  // barrier per entry (lockstep, see k_csolve): worlds without a bounce only wait at the two extra barriers.
+  // stage order: nb2::cbwd_iter.  One call site for all of them (code size), one block-wide barrier per entry (lockstep, see k_csolve):
+  // worlds without a bounce only wait at the two extra barriers.
 #pragma unroll 1
-  for (int it = 0; it < 10; it++) {
-    const bool second = (it == 6) | (it == 7);
+  for (int it = 0; it < NB2_CBWD_ITERS; it++) {
+    const auto [sg, second] = nb2::cbwd_iter(it);
     if (!BOUNCE && second) continue;
-    const int sg = (it < 4) ? it + 1 : (it == 4 || it == 6) ? 5 : (it == 5 || it == 7) ? 7 : (it == 8) ? 6 : 8;
     if (it == 4) {  // lambda and its fields are complete: the contact adjoint turns them into w and prepares the injections
       __syncwarp();
       CW_PROF(20);
@@ -647,10 +640,7 @@ k_lcp_batch(nb2::cw::Dims d, int B, int mcap, double cfm, int mode, int early_te
   extern __shared__ __align__(16) unsigned char nb2_smem[];
   const int w = blockIdx.x, lane = threadIdx.x & 31;
   if (w >= B) return;
-  nb2::cw::Ws* wsm = reinterpret_cast<nb2::cw::Ws*>(nb2_smem);
-  double* wsb = reinterpret_cast<double*>(wsm) + NB2_WS_DESC_DOUBLES;
-  if (lane == 0) *wsm = nb2::cw::carve(wsb, d);
-  __syncwarp();
+  nb2::cw::Ws* wsm = warp_workspace(nb2_smem, d, lane);
   const nb2::cw::Ws ws = *wsm;
   const int m = ms[w], ld = m | 1;
   const size_t ov = (size_t)w * mcap;
@@ -677,6 +667,30 @@ k_lcp_batch(nb2::cw::Dims d, int B, int mcap, double cfm, int mode, int early_te
 constexpr int kMaxSmem = 227 * 1024;
 
 }  // namespace
+
+// Calls f with the lane count as a compile-time std::integral_constant (the step kernels are instantiated for 1, 2, 4 and 8 lanes).
+template <class F> static int with_lanes(int lanes, F&& f) {
+  switch (lanes) {
+    case 1: return f(std::integral_constant<int, 1>());
+    case 2: return f(std::integral_constant<int, 2>());
+    case 4: return f(std::integral_constant<int, 4>());
+    case 8: return f(std::integral_constant<int, 8>());
+  }
+  g_err = "bad lane count"; return NB2_ERR_INVALID;
+}
+// Calls f with a value of the real type of `precision`: NB2_FP64 runs the fp64 kernels, any other value the fp32 ones.
+template <class F> static int with_precision(int precision, F&& f) { return precision == NB2_FP64 ? f(double()) : f(float()); }
+// The dynamic shared-memory limit of a kernel is a per-device attribute (a model may be used from several GPUs of one process): raise it
+// to kMaxSmem once per kernel and device.
+template <auto Kern> static int allow_max_smem() {
+  static std::atomic<bool> done[64];
+  int dev = 0; NB2_CUDA(cudaGetDevice(&dev));
+  if (!done[dev & 63].load(std::memory_order_acquire)) {
+    NB2_CUDA(cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
+    done[dev & 63].store(true, std::memory_order_release);
+  }
+  return NB2_OK;
+}
 
 // one sweep schedule of the model (same bodies, different lane count / slot assignment)
 struct LaunchShape { int warps_per_block = 0; int resident_warps = 0; };  // filled lazily from the occupancy API
@@ -757,39 +771,31 @@ static int block_warps(int total_warps, int sm_count, const LaunchShape& sh, siz
   return w;
 }
 
-template <class R, int K> struct StepKernels {
-  static constexpr int ST = CoopShape<K>::ST, WPW = CoopShape<K>::WPW;
-  static int prepare(nb2_variant& v, int dir) {  // dir 0 forward, 1 backward
-    LaunchShape& sh = v.shape[dir][sizeof(R) == 8];
-    static bool attr_done[2][64] = {};  // function attributes are per device: a model may be used from several GPUs of one process
-    int dev = 0; NB2_CUDA(cudaGetDevice(&dev));
-    if (sh.warps_per_block && attr_done[dir][dev & 63]) return NB2_OK;
-    attr_done[dir][dev & 63] = true;
-    const size_t per_warp = (size_t)(dir ? v.bwd_words : v.fwd_words) * ST * sizeof(R) + (dir ? staging_bytes<K>(4 * v.mf.ndof + v.mf.na) : staging_bytes<K>(2 * v.mf.ndof + v.mf.na));
-    const size_t per_block = (size_t)body_table_words<K>(v.mf.nb) * sizeof(R) + 16;
-    if (per_warp + per_block > (size_t)kMaxSmem) { g_err = "model needs " + std::to_string(per_warp) + " B of shared memory per warp (> 227 KB)"; return NB2_ERR_UNSUPPORTED; }
-    if (dir == 0) {  // the per-world-inertia variant launches with the shape of the shared-table kernel
-      NB2_CUDA(cudaFuncSetAttribute(k_step_fwd<R, K, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
-      NB2_CUDA(cudaFuncSetAttribute(k_step_fwd<R, K, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
-      sh = occupancy_shape(k_step_fwd<R, K, false>, per_warp, per_block);
-    } else {
-      NB2_CUDA(cudaFuncSetAttribute(k_step_bwd<R, K, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
-      NB2_CUDA(cudaFuncSetAttribute(k_step_bwd<R, K, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
-      sh = occupancy_shape(k_step_bwd<R, K, false>, per_warp, per_block);
-    }
-    if (!sh.warps_per_block) { g_err = "no launch shape fits this model"; return NB2_ERR_UNSUPPORTED; }
-    return NB2_OK;
+template <class R, int K>
+static int prepare_k(nb2_variant& v, int dir) {  // dir 0 forward, 1 backward
+  constexpr int ST = CoopShape<K>::ST;
+  LaunchShape& sh = v.shape[dir][sizeof(R) == 8];
+  // the occupancy query sizes a warp with its scratch AND its input-staging buffer, in both directions
+  const size_t scratch_and_staging = (size_t)(dir ? v.bwd_words : v.fwd_words) * ST * sizeof(R) +
+                                     (dir ? staging_bytes<K>(4 * v.mf.ndof + v.mf.na) : staging_bytes<K>(2 * v.mf.ndof + v.mf.na));
+  const size_t per_block = (size_t)body_table_words<K>(v.mf.nb) * sizeof(R) + 16;
+  if (scratch_and_staging + per_block > (size_t)kMaxSmem) {
+    g_err = "model needs " + std::to_string(scratch_and_staging) + " B of shared memory per warp (> 227 KB)"; return NB2_ERR_UNSUPPORTED;
   }
-};
+  int rc;
+  if (dir == 0) {  // the per-world-inertia variant launches with the shape of the shared-table kernel
+    if ((rc = allow_max_smem<k_step_fwd<R, K, false>>()) || (rc = allow_max_smem<k_step_fwd<R, K, true>>())) return rc;
+    if (!sh.warps_per_block) sh = occupancy_shape(k_step_fwd<R, K, false>, scratch_and_staging, per_block);
+  } else {
+    if ((rc = allow_max_smem<k_step_bwd<R, K, false>>()) || (rc = allow_max_smem<k_step_bwd<R, K, true>>())) return rc;
+    if (!sh.warps_per_block) sh = occupancy_shape(k_step_bwd<R, K, false>, scratch_and_staging, per_block);
+  }
+  if (!sh.warps_per_block) { g_err = "no launch shape fits this model"; return NB2_ERR_UNSUPPORTED; }
+  return NB2_OK;
+}
 template <class R>
 static int prepare_variant(nb2_variant& v, int dir) {
-  switch (v.mf.lanes) {
-    case 1: return StepKernels<R, 1>::prepare(v, dir);
-    case 2: return StepKernels<R, 2>::prepare(v, dir);
-    case 4: return StepKernels<R, 4>::prepare(v, dir);
-    case 8: return StepKernels<R, 8>::prepare(v, dir);
-  }
-  g_err = "bad lane count"; return NB2_ERR_INVALID;
+  return with_lanes(v.mf.lanes, [&](auto k) { return prepare_k<R, decltype(k)::value>(v, dir); });
 }
 
 template <class R>
@@ -835,13 +841,9 @@ static int launch_fwd(nb2_model* m, int B, const float* state, const float* acti
   nb2_variant* pv = nullptr;
   int rc = pick_variant<R>(m, B, 0, &pv);
   if (rc) return rc;
-  switch (pv->mf.lanes) {
-    case 1: return launch_fwd_k<R, 1>(*pv, m->sm_count, Btot, w0, B, state, action, next, saved, st, state_copy, action_copy, wi);
-    case 2: return launch_fwd_k<R, 2>(*pv, m->sm_count, Btot, w0, B, state, action, next, saved, st, state_copy, action_copy, wi);
-    case 4: return launch_fwd_k<R, 4>(*pv, m->sm_count, Btot, w0, B, state, action, next, saved, st, state_copy, action_copy, wi);
-    case 8: return launch_fwd_k<R, 8>(*pv, m->sm_count, Btot, w0, B, state, action, next, saved, st, state_copy, action_copy, wi);
-  }
-  g_err = "bad lane count"; return NB2_ERR_INVALID;
+  return with_lanes(pv->mf.lanes, [&](auto k) {
+    return launch_fwd_k<R, decltype(k)::value>(*pv, m->sm_count, Btot, w0, B, state, action, next, saved, st, state_copy, action_copy, wi);
+  });
 }
 static bool no_stage_saved() {
   static const bool off = [] { const char* e = getenv("NB2_NO_STAGE_SAVED"); return e && atoi(e); }();
@@ -853,9 +855,10 @@ static int launch_bwd_k(const nb2_variant& v, int sm_count, int Btot, int w0, in
                         const double* wi, double* gIa) {
   constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
   const LaunchShape& sh = v.shape[1][sizeof(R) == 8];
-  const size_t per_warp = (size_t)v.bwd_words * ST * sizeof(R);
+  // the warps per block are sized with the scratch only, while prepare_k's occupancy query (scratch_and_staging) also counts the input staging
+  const size_t scratch_per_warp = (size_t)v.bwd_words * ST * sizeof(R);
   const int total_warps = (B + WPW - 1) / WPW;
-  const int warps = block_warps(total_warps, sm_count, sh, per_warp);
+  const int warps = block_warps(total_warps, sm_count, sh, scratch_per_warp);
   const int blocks = (total_warps + warps - 1) / warps;
   const size_t tab = (size_t)body_table_words<K>(v.mf.nb) * sizeof(R);
   // stage the saved stream in shared memory when the whole batch is resident at once anyway (see the kernel)
@@ -863,10 +866,10 @@ static int launch_bwd_k(const nb2_variant& v, int sm_count, int Btot, int w0, in
   const bool aligned = (((size_t)Btot * sizeof(R)) % 16 == 0) && (((size_t)w0 * sizeof(R)) % 16 == 0) && ((reinterpret_cast<size_t>(saved) & 15) == 0) &&
                        ((WPW * sizeof(R)) % 16 == 0);
   const size_t in_per_warp = staging_bytes<K>(4 * v.mf.ndof + v.mf.na);  // bulk-copy staging of dL/dx', x, u rows
-  const size_t smem_staged = (per_warp + stage_per_warp) * warps + tab + 16;
+  const size_t smem_staged = (scratch_per_warp + stage_per_warp) * warps + tab + 16;
   const int blocks_per_sm = (blocks + sm_count - 1) / sm_count;
   const bool stage = aligned && (smem_staged + in_per_warp * warps) * blocks_per_sm + 1024 * blocks_per_sm <= (size_t)kMaxSmem && !no_stage_saved();
-  const size_t base = ((stage ? smem_staged : per_warp * warps + tab) + 15) & ~(size_t)15;
+  const size_t base = ((stage ? smem_staged : scratch_per_warp * warps + tab) + 15) & ~(size_t)15;
   const bool in_stage = base + in_per_warp * warps <= (size_t)kMaxSmem;
   const size_t smem = in_stage ? base + in_per_warp * warps : base;
   if (wi || gIa) k_step_bwd<R, K, true><<<blocks, warps * 32, smem, st>>>(model_of<R>(v), Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia,
@@ -885,13 +888,9 @@ static int launch_bwd(nb2_model* m, int B, const float* state, const float* acti
   nb2_variant* pv = nullptr;
   int rc = pick_variant<R>(m, B, 1, &pv);
   if (rc) return rc;
-  switch (pv->mf.lanes) {
-    case 1: return launch_bwd_k<R, 1>(*pv, m->sm_count, Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia, st, accumulate, wi, gIa);
-    case 2: return launch_bwd_k<R, 2>(*pv, m->sm_count, Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia, st, accumulate, wi, gIa);
-    case 4: return launch_bwd_k<R, 4>(*pv, m->sm_count, Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia, st, accumulate, wi, gIa);
-    case 8: return launch_bwd_k<R, 8>(*pv, m->sm_count, Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia, st, accumulate, wi, gIa);
-  }
-  g_err = "bad lane count"; return NB2_ERR_INVALID;
+  return with_lanes(pv->mf.lanes, [&](auto k) {
+    return launch_bwd_k<R, decltype(k)::value>(*pv, m->sm_count, Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia, st, accumulate, wi, gIa);
+  });
 }
 
 // The host entry points take host buffers.  When every buffer of a call is page-locked memory visible to the device
@@ -966,9 +965,8 @@ static CStepArgs cstep_args(const nb2_model* m, const nb2_variant& v, int B, voi
   P.todo = (int*)(P.exch + (size_t)B * P.exch_stride);  // list of the worlds the first solve kernel hands to the second
   return P;
 }
-template <class Kern> static int cstep_smem_attr(Kern kern, size_t smem, bool* done) {
-  int dev = 0; NB2_CUDA(cudaGetDevice(&dev));
-  if (!done[dev & 63]) { NB2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem)); done[dev & 63] = true; }  // per device
+template <auto Kern> static int cstep_smem_attr(size_t smem) {
+  if (int rc = allow_max_smem<Kern>()) return rc;
   if (smem > (size_t)kMaxSmem) { g_err = "the fused contact kernel needs " + std::to_string(smem) + " B of shared memory per world (> 227 KB)"; return NB2_ERR_UNSUPPORTED; }
   return NB2_OK;
 }
@@ -1066,7 +1064,7 @@ int nb2_model_set_lanes(nb2_model* m, int lanes) {
 int nb2_model_lanes_for(nb2_model* m, int B, int backward, int precision) {
   if (!m || B <= 0) return -1;
   nb2_variant* pv = nullptr;
-  const int rc = (precision == NB2_FP64) ? pick_variant<double>(m, B, backward ? 1 : 0, &pv) : pick_variant<float>(m, B, backward ? 1 : 0, &pv);
+  const int rc = with_precision(precision, [&](auto r) { return pick_variant<decltype(r)>(m, B, backward ? 1 : 0, &pv); });
   return rc ? -1 : pv->mf.lanes;
 }
 
@@ -1105,8 +1103,7 @@ int nb2_step_forward_contact_pw(const nb2_model* cm, int B, const float* state, 
   const nb2_variant& v = m->variants[m->contact_variant];
   const CStepArgs P = cstep_args(m, v, B, workspace, 0);
   const size_t smem = ((((size_t)P.fwd_words + 1) & ~(size_t)1) + NB2_WS_DESC_DOUBLES + P.ws_small_doubles) * sizeof(double);
-  static bool attr_done[64] = {};
-  int rc = cstep_smem_attr(k_cstep_fwd, smem, attr_done);
+  int rc = cstep_smem_attr<k_cstep_fwd>(smem);
   if (rc) return rc;
   NB2_CUDA(cudaMemsetAsync(workspace, 0, 64, st));  // pool counters
   if (contact_fused() || !saved_fp64) {
@@ -1117,10 +1114,11 @@ int nb2_step_forward_contact_pw(const nb2_model* cm, int B, const float* state, 
     NB2_CUDA(cudaGetLastError());
     return NB2_OK;
   }
-  static bool attr_b[64] = {}, attr_s[64] = {}, attr_s2[64] = {}, attr_a[64] = {};
   const size_t smem_s = (NB2_WS_DESC_DOUBLES + nb2::cw::ws_doubles(P.ds_solve)) * sizeof(double);
   const size_t smem_a = (NB2_WS_DESC_DOUBLES + nb2::cw::ws_doubles(P.ds_apply)) * sizeof(double);
-  if ((rc = cstep_smem_attr(k_cbuild, smem, attr_b)) || (rc = cstep_smem_attr(k_csolve<0>, smem_s, attr_s)) || (rc = cstep_smem_attr(k_csolve<1>, smem_s, attr_s2)) || (rc = cstep_smem_attr(k_capply, smem_a, attr_a))) return rc;
+  if ((rc = cstep_smem_attr<k_cbuild>(smem)) || (rc = cstep_smem_attr<k_csolve<0>>(smem_s)) || (rc = cstep_smem_attr<k_csolve<1>>(smem_s)) ||
+      (rc = cstep_smem_attr<k_capply>(smem_a)))
+    return rc;
   const int wpb_b = pick_wpb(B, m->sm_count, smem, NB2_CBUILD_MAXW, 0), wpb_s = pick_wpb(B, m->sm_count, smem_s, NB2_CSOLVE_MAXW, 1),
             wpb_a = pick_wpb(B, m->sm_count, smem_a, NB2_CAPPLY_MAXW, 2);
   k_cbuild<<<(B + wpb_b - 1) / wpb_b, 32 * wpb_b, smem * wpb_b, st>>>(v.md, m->contact, P, state, action, next_state, (double*)saved_fp64, m_lcp, status, ncontacts, cinfo,
@@ -1150,9 +1148,8 @@ static int cbwd_launch(nb2_model* m, int B, const float* state, const float* act
   const size_t smem_staged = smem_base + ((((size_t)P.saved_words + 1) & ~(size_t)1) + 2) * sizeof(double);
   const int stage = pick_wpb(B, m->sm_count, smem_staged, NB2_CBWD_MAXW, 3) == pick_wpb(B, m->sm_count, smem_base, NB2_CBWD_MAXW, 3);
   const size_t smem = stage ? smem_staged : smem_base;
-  static bool attr_done[64] = {}, attr_done_b[64] = {};
   const bool bounce = m->contact_restitution;  // some body has a restitution coefficient: the kernel with the second reverse sweep
-  int rc = bounce ? cstep_smem_attr(k_cstep_bwd<true>, smem, attr_done_b) : cstep_smem_attr(k_cstep_bwd<false>, smem, attr_done);
+  int rc = bounce ? cstep_smem_attr<k_cstep_bwd<true>>(smem) : cstep_smem_attr<k_cstep_bwd<false>>(smem);
   if (rc) return rc;
   NB2_CUDA(cudaMemsetAsync(workspace, 0, 64, st));
   const int wpb = pick_wpb(B, m->sm_count, smem, NB2_CBWD_MAXW, 3);
@@ -1194,9 +1191,21 @@ struct RolloutTape {
   int k, nseg, nslots;
   size_t slot_doubles, saved_doubles, rec_doubles, snap_doubles, x_doubles;
   size_t o_slots, o_snaps, o_next, o_labels, o_status, o_nc, total_doubles;
+  double* base;  // the tape buffer (nullptr when only its size is wanted)
+  // slot i holds a step's saved stream followed by its contact record
+  double* saved(int i) const { return base + o_slots + slot_doubles * i; }
+  double* record(int i) const { return saved(i) + saved_doubles; }
+  int32_t* labels() const { return reinterpret_cast<int32_t*>(base + o_labels); }
+  int32_t* status() const { return reinterpret_cast<int32_t*>(base + o_status); }
+  int32_t* nc() const { return reinterpret_cast<int32_t*>(base + o_nc); }
+  float* next_scratch() const { return reinterpret_cast<float*>(base + o_next); }
+  // snapshot i of the LCP cache: x, then m
+  double* snap_x(int i) const { return base + o_snaps + snap_doubles * i; }
+  int32_t* snap_m(int i) const { return reinterpret_cast<int32_t*>(snap_x(i) + x_doubles); }
 };
-static RolloutTape rollout_tape(const nb2_model* m, int B, int T, int checkpoint_every) {
+static RolloutTape rollout_tape(const nb2_model* m, int B, int T, int checkpoint_every, void* tape = nullptr) {
   RolloutTape L;
+  L.base = (double*)tape;
   L.k = (checkpoint_every <= 0 || checkpoint_every >= T) ? (T > 0 ? T : 1) : checkpoint_every;
   L.nseg = T > 0 ? (T + L.k - 1) / L.k : 0;
   L.nslots = L.k;
@@ -1220,9 +1229,9 @@ size_t nb2_rollout_contact_tape_bytes(const nb2_model* m, int B, int T, int chec
   if (!m || !m->has_contacts || B <= 0 || T < 0) return 0;
   return rollout_tape(m, B, T, checkpoint_every).total_doubles * sizeof(double);
 }
-static int snap_copy(double* tape, const RolloutTape& L, int idx, double* x_lcp, int32_t* m_lcp, int B, bool restore, cudaStream_t st) {
-  double* sx = tape + L.o_snaps + L.snap_doubles * idx;
-  int32_t* sm = reinterpret_cast<int32_t*>(sx + L.x_doubles);
+static int snap_copy(const RolloutTape& L, int idx, double* x_lcp, int32_t* m_lcp, int B, bool restore, cudaStream_t st) {
+  double* sx = L.snap_x(idx);
+  int32_t* sm = L.snap_m(idx);
   if (restore) {
     NB2_CUDA(cudaMemcpyAsync(x_lcp, sx, L.x_doubles * sizeof(double), cudaMemcpyDeviceToDevice, st));
     NB2_CUDA(cudaMemcpyAsync(m_lcp, sm, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
@@ -1244,23 +1253,19 @@ int nb2_rollout_forward_contact_pw(const nb2_model* cm, int B, int T, float* sta
   if (!m->has_contacts) { g_err = "nb2_rollout_forward_contact: the model has no collision pairs (use nb2_rollout_forward)"; return NB2_ERR_INVALID; }
   if (B == 0 || T == 0) return NB2_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  double* tape = (double*)tape_;
-  const RolloutTape L = rollout_tape(m, B, T, checkpoint_every);
+  const RolloutTape L = rollout_tape(m, B, T, checkpoint_every, tape_);
   const size_t n2 = (size_t)2 * m->mf.ndof, na = (size_t)m->mf.na;
-  int32_t* labels = reinterpret_cast<int32_t*>(tape + L.o_labels);
-  int32_t* status = reinterpret_cast<int32_t*>(tape + L.o_status);
-  int32_t* nc = reinterpret_cast<int32_t*>(tape + L.o_nc);
   const bool ckpt = L.nseg > 1;
   for (int t = 0; t < T; t++) {
     int rc;
-    if (ckpt && t % L.k == 0 && (rc = snap_copy(tape, L, t / L.k, x_lcp, m_lcp, B, false, st))) return rc;
-    double* slot = tape + L.o_slots + L.slot_doubles * (t % L.nslots);
+    if (ckpt && t % L.k == 0 && (rc = snap_copy(L, t / L.k, x_lcp, m_lcp, B, false, st))) return rc;
+    const int slot = t % L.nslots;
     // with checkpoints the forward's records are thrown away (the reverse sweep regenerates them): do not write them
-    rc = nb2_step_forward_contact_pw(m, B, states + n2 * B * t, actions + na * B * t, world_inertia, states + n2 * B * (t + 1), slot, workspace, x_lcp, m_lcp,
-                                     labels, status, nc, nullptr, ckpt ? nullptr : slot + L.saved_doubles, status_accum, stream);
+    rc = nb2_step_forward_contact_pw(m, B, states + n2 * B * t, actions + na * B * t, world_inertia, states + n2 * B * (t + 1), L.saved(slot), workspace,
+                                     x_lcp, m_lcp, L.labels(), L.status(), L.nc(), nullptr, ckpt ? nullptr : L.record(slot), status_accum, stream);
     if (rc) return rc;
   }
-  if (ckpt) return snap_copy(tape, L, L.nseg, x_lcp, m_lcp, B, false, st);
+  if (ckpt) return snap_copy(L, L.nseg, x_lcp, m_lcp, B, false, st);
   return NB2_OK;
 }
 int nb2_rollout_backward_contact(const nb2_model* cm, int B, int T, const float* states, const float* actions, double* x_lcp, int32_t* m_lcp, void* tape_,
@@ -1279,13 +1284,8 @@ int nb2_rollout_backward_contact_pw(const nb2_model* cm, int B, int T, const flo
   if (!m->has_contacts) { g_err = "nb2_rollout_backward_contact: the model has no collision pairs (use nb2_rollout_backward)"; return NB2_ERR_INVALID; }
   if (B == 0 || T == 0) return NB2_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  double* tape = (double*)tape_;
-  const RolloutTape L = rollout_tape(m, B, T, checkpoint_every);
+  const RolloutTape L = rollout_tape(m, B, T, checkpoint_every, tape_);
   const size_t n2 = (size_t)2 * m->mf.ndof, na = (size_t)m->mf.na;
-  int32_t* labels = reinterpret_cast<int32_t*>(tape + L.o_labels);
-  int32_t* status = reinterpret_cast<int32_t*>(tape + L.o_status);
-  int32_t* nc = reinterpret_cast<int32_t*>(tape + L.o_nc);
-  float* next_scratch = reinterpret_cast<float*>(tape + L.o_next);
   const bool ckpt = L.nseg > 1;
   for (int seg = L.nseg - 1; seg >= 0; seg--) {
     const int t0 = seg * L.k, t1 = (t0 + L.k < T) ? t0 + L.k : T;
@@ -1293,22 +1293,20 @@ int nb2_rollout_backward_contact_pw(const nb2_model* cm, int B, int T, const flo
     if (ckpt) {
       // refill the tape: the segment's forward again, from the stored states and the LCP cache as it was at the segment start.  The stored
       // trajectory is NOT overwritten (the recomputed next states go to a scratch row; they are the same bits).
-      if ((rc = snap_copy(tape, L, seg, x_lcp, m_lcp, B, true, st))) return rc;
+      if ((rc = snap_copy(L, seg, x_lcp, m_lcp, B, true, st))) return rc;
       for (int t = t0; t < t1; t++) {
-        double* slot = tape + L.o_slots + L.slot_doubles * (t - t0);
-        rc = nb2_step_forward_contact_pw(m, B, states + n2 * B * t, actions + na * B * t, world_inertia, next_scratch, slot, workspace, x_lcp, m_lcp, labels,
-                                         status, nc, nullptr, slot + L.saved_doubles, nullptr, stream);
+        rc = nb2_step_forward_contact_pw(m, B, states + n2 * B * t, actions + na * B * t, world_inertia, L.next_scratch(), L.saved(t - t0), workspace, x_lcp,
+                                         m_lcp, L.labels(), L.status(), L.nc(), nullptr, L.record(t - t0), nullptr, stream);
         if (rc) return rc;
       }
     }
     for (int t = t1 - 1; t >= t0; t--) {
-      const double* slot = tape + L.o_slots + L.slot_doubles * (t - t0);
-      rc = cbwd_launch(m, B, states + n2 * B * t, actions + na * B * t, slot, slot + L.saved_doubles, workspace, grad_states + n2 * B * (t + 1),
+      rc = cbwd_launch(m, B, states + n2 * B * t, actions + na * B * t, L.saved(t - t0), L.record(t - t0), workspace, grad_states + n2 * B * (t + 1),
                        grad_states + n2 * B * t, grad_actions + na * B * t, nullptr, status_accum, st, 1, world_inertia, grad_inertia);
       if (rc) return rc;
     }
   }
-  if (ckpt) return snap_copy(tape, L, L.nseg, x_lcp, m_lcp, B, true, st);  // leave the solver cache as the forward left it
+  if (ckpt) return snap_copy(L, L.nseg, x_lcp, m_lcp, B, true, st);  // leave the solver cache as the forward left it
   return NB2_OK;
 }
 int nb2_model_set_contact_capacity(nb2_model* m, int max_contacts_in_shared_memory) {
@@ -1396,8 +1394,7 @@ int nb2_lcp_solve_batch(int B, int mcap, int mode, int early_termination, double
   if (B == 0) return NB2_OK;
   const nb2::cw::Dims d = nb2::cw::make_dims(1, 1, 0, (mcap + 2) / 3 + 1, mcap < 3 ? 3 : mcap, 1, 1, 0, NB2_WS_SOLVE);
   const size_t smem = (NB2_WS_DESC_DOUBLES + nb2::cw::ws_doubles(d)) * sizeof(double);
-  static bool attr_done[64] = {};
-  int rc = cstep_smem_attr(k_lcp_batch, smem, attr_done);
+  int rc = cstep_smem_attr<k_lcp_batch>(smem);
   if (rc) return rc;
   k_lcp_batch<<<B, 32, smem, (cudaStream_t)stream>>>(d, B, mcap, fallback_cfm, mode, early_termination, m, A, b, lo, hi, findex, x0, x, labels, status);
   g_launches++;
@@ -1419,8 +1416,10 @@ int nb2_step_forward_pw(const nb2_model* cm, int B, const float* state, const fl
   if (m->has_contacts) { g_err = "nb2_step_forward: the model has collision pairs: use nb2_step_forward_contact (or build the model without shapes for a contact-free step)"; return NB2_ERR_INVALID; }
   if (B == 0) return NB2_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  if (precision == NB2_FP64) return launch_fwd<double>(m, B, state, action, next_state, (double*)saved, st, -1, 0, nullptr, nullptr, world_inertia);
-  return launch_fwd<float>(m, B, state, action, next_state, (float*)saved, st, -1, 0, nullptr, nullptr, world_inertia);
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    return launch_fwd<R>(m, B, state, action, next_state, (R*)saved, st, -1, 0, nullptr, nullptr, world_inertia);
+  });
 }
 
 int nb2_step_backward(const nb2_model* cm, int B, const float* state, const float* action, const void* saved,
@@ -1438,8 +1437,10 @@ int nb2_step_backward_pw(const nb2_model* cm, int B, const float* state, const f
   if (m->has_contacts) { g_err = "nb2_step_backward: the model has collision pairs: use nb2_step_backward_contact"; return NB2_ERR_INVALID; }
   if (B == 0) return NB2_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  if (precision == NB2_FP64) return launch_bwd<double>(m, B, state, action, (const double*)saved, grad_next_state, grad_state, grad_action, grad_inertia, st, -1, 0, 0, world_inertia);
-  return launch_bwd<float>(m, B, state, action, (const float*)saved, grad_next_state, grad_state, grad_action, grad_inertia, st, -1, 0, 0, world_inertia);
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    return launch_bwd<R>(m, B, state, action, (const R*)saved, grad_next_state, grad_state, grad_action, grad_inertia, st, -1, 0, 0, world_inertia);
+  });
 }
 
 int nb2_rollout_forward(const nb2_model* cm, int B, int T, float* states, const float* actions, void* saved, int precision, void* stream) {
@@ -1472,16 +1473,17 @@ int nb2_rollout_backward_pw(const nb2_model* cm, int B, int T, const float* stat
   if (m->has_contacts) { g_err = "nb2_rollout_backward: contact worlds back-propagate through nb2_step_backward_contact"; return NB2_ERR_INVALID; }
   if (B == 0) return NB2_OK;
   const size_t n2 = (size_t)2 * m->mf.ndof, na = (size_t)m->mf.na;
-  const size_t sv_step = (size_t)m->saved_words * B * (precision == NB2_FP64 ? sizeof(double) : sizeof(float));
   cudaStream_t st = (cudaStream_t)stream;
-  for (int t = T - 1; t >= 0; t--) {  // grad_states[t] += clip(J_t^T grad_states[t+1]) ; grad_actions[t] = ...
-    const char* sv = (const char*)saved + sv_step * t;
-    int rc;
-    if (precision == NB2_FP64) rc = launch_bwd<double>(m, B, states + n2 * B * t, actions + na * B * t, (const double*)sv, grad_states + n2 * B * (t + 1), grad_states + n2 * B * t, grad_actions + na * B * t, nullptr, st, -1, 0, 1, world_inertia, grad_inertia);
-    else rc = launch_bwd<float>(m, B, states + n2 * B * t, actions + na * B * t, (const float*)sv, grad_states + n2 * B * (t + 1), grad_states + n2 * B * t, grad_actions + na * B * t, nullptr, st, -1, 0, 1, world_inertia, grad_inertia);
-    if (rc) return rc;
-  }
-  return NB2_OK;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    for (int t = T - 1; t >= 0; t--) {  // grad_states[t] += clip(J_t^T grad_states[t+1]) ; grad_actions[t] = ...
+      const R* sv = (const R*)saved + (size_t)m->saved_words * B * t;
+      int rc = launch_bwd<R>(m, B, states + n2 * B * t, actions + na * B * t, sv, grad_states + n2 * B * (t + 1), grad_states + n2 * B * t,
+                             grad_actions + na * B * t, nullptr, st, -1, 0, 1, world_inertia, grad_inertia);
+      if (rc) return rc;
+    }
+    return (int)NB2_OK;
+  });
 }
 
 static int ensure_host_buffers(nb2_model* m, int B) {
@@ -1516,8 +1518,10 @@ int nb2_step_forward_host(nb2_model* m, int B, const float* state, const float* 
     const float* zs = mapped_alias(state); const float* za = mapped_alias(action); float* zn = mapped_alias(next_state);
     if (zs && za && zn) {
       cudaStream_t st = m->host_streams[0];
-      if (precision == NB2_FP64) rc = launch_fwd<double>(m, B, zs, za, zn, keep_for_backward ? (double*)m->d_saved : nullptr, st, B, 0, m->d_state, m->d_action);
-      else rc = launch_fwd<float>(m, B, zs, za, zn, keep_for_backward ? (float*)m->d_saved : nullptr, st, B, 0, m->d_state, m->d_action);
+      rc = with_precision(precision, [&](auto r) {
+        using R = decltype(r);
+        return launch_fwd<R>(m, B, zs, za, zn, keep_for_backward ? (R*)m->d_saved : nullptr, st, B, 0, m->d_state, m->d_action);
+      });
       if (rc) return rc;
       NB2_CUDA(cudaStreamSynchronize(st));
       m->host_B = keep_for_backward ? B : 0;
@@ -1530,8 +1534,10 @@ int nb2_step_forward_host(nb2_model* m, int B, const float* state, const float* 
     cudaStream_t st = m->host_streams[c];
     NB2_CUDA(cudaMemcpyAsync(m->d_state + n2 * lo, state + n2 * lo, n2 * cnt * sizeof(float), cudaMemcpyHostToDevice, st));
     NB2_CUDA(cudaMemcpyAsync(m->d_action + na * lo, action + na * lo, na * cnt * sizeof(float), cudaMemcpyHostToDevice, st));
-    if (precision == NB2_FP64) rc = launch_fwd<double>(m, cnt, m->d_state, m->d_action, m->d_next, keep_for_backward ? (double*)m->d_saved : nullptr, st, B, lo);
-    else rc = launch_fwd<float>(m, cnt, m->d_state, m->d_action, m->d_next, keep_for_backward ? (float*)m->d_saved : nullptr, st, B, lo);
+    rc = with_precision(precision, [&](auto r) {
+      using R = decltype(r);
+      return launch_fwd<R>(m, cnt, m->d_state, m->d_action, m->d_next, keep_for_backward ? (R*)m->d_saved : nullptr, st, B, lo);
+    });
     if (rc) return rc;
     NB2_CUDA(cudaMemcpyAsync(next_state + n2 * lo, m->d_next + n2 * lo, n2 * cnt * sizeof(float), cudaMemcpyDeviceToHost, st));
   }
@@ -1550,9 +1556,10 @@ int nb2_step_backward_host(nb2_model* m, int B, const float* grad_next_state, fl
     const float* zg = mapped_alias(grad_next_state); float* zgs = mapped_alias(grad_state); float* zga = mapped_alias(grad_action);
     if (zg && zgs && zga) {
       cudaStream_t st = m->host_streams[0];
-      int rc;
-      if (precision == NB2_FP64) rc = launch_bwd<double>(m, B, m->d_state, m->d_action, (const double*)m->d_saved, zg, zgs, zga, nullptr, st);
-      else rc = launch_bwd<float>(m, B, m->d_state, m->d_action, (const float*)m->d_saved, zg, zgs, zga, nullptr, st);
+      int rc = with_precision(precision, [&](auto r) {
+        using R = decltype(r);
+        return launch_bwd<R>(m, B, m->d_state, m->d_action, (const R*)m->d_saved, zg, zgs, zga, nullptr, st);
+      });
       if (rc) return rc;
       NB2_CUDA(cudaStreamSynchronize(st));
       return NB2_OK;
@@ -1563,9 +1570,10 @@ int nb2_step_backward_host(nb2_model* m, int B, const float* grad_next_state, fl
     const int lo = (int)((long long)B * c / C), cnt = (int)((long long)B * (c + 1) / C) - lo;
     cudaStream_t st = m->host_streams[c];
     NB2_CUDA(cudaMemcpyAsync(m->d_gnext + n2 * lo, grad_next_state + n2 * lo, n2 * cnt * sizeof(float), cudaMemcpyHostToDevice, st));
-    int rc;
-    if (precision == NB2_FP64) rc = launch_bwd<double>(m, cnt, m->d_state, m->d_action, (const double*)m->d_saved, m->d_gnext, m->d_gstate, m->d_gaction, nullptr, st, B, lo);
-    else rc = launch_bwd<float>(m, cnt, m->d_state, m->d_action, (const float*)m->d_saved, m->d_gnext, m->d_gstate, m->d_gaction, nullptr, st, B, lo);
+    int rc = with_precision(precision, [&](auto r) {
+      using R = decltype(r);
+      return launch_bwd<R>(m, cnt, m->d_state, m->d_action, (const R*)m->d_saved, m->d_gnext, m->d_gstate, m->d_gaction, nullptr, st, B, lo);
+    });
     if (rc) return rc;
     NB2_CUDA(cudaMemcpyAsync(grad_state + n2 * lo, m->d_gstate + n2 * lo, n2 * cnt * sizeof(float), cudaMemcpyDeviceToHost, st));
     NB2_CUDA(cudaMemcpyAsync(grad_action + na * lo, m->d_gaction + na * lo, na * cnt * sizeof(float), cudaMemcpyDeviceToHost, st));

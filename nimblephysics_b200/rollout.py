@@ -13,7 +13,7 @@ from typing import Callable, List, Optional, Sequence, Tuple
 
 import torch
 
-from .timestep import TimestepLayer, per_world_inertia, timestep
+from .timestep import TimestepLayer, _inertia_grad, _word_major_inertia, per_world_inertia, timestep
 
 
 def rollout(world, state0: torch.Tensor, actions: Sequence[torch.Tensor], keep_states: bool = False, mass: Optional[torch.Tensor] = None):
@@ -127,20 +127,6 @@ class _ContactRollout(torch.autograd.Function):
                                                torch.cuda.current_stream().cuda_stream, wi_ptr=wi.data_ptr() if wi is not None else None,
                                                ginertia_ptr=gi.data_ptr() if gi is not None else None)
         return None, gs[0].to(ctx.dtypes[0]), ga.to(ctx.dtypes[1]), None, _inertia_grad(gi, ctx.wi_like)
-
-
-def _word_major_inertia(dm, world_inertia, B, dev):
-    """[B, nb, 10] per-world inertia -> the kernels' word-major [10*nb, B] fp64 layout on `dev` (None stays None)."""
-    if world_inertia is None:
-        return None
-    return world_inertia.detach().to(device=dev, dtype=torch.float64).reshape(B, 10 * dm.cm.nb).t().contiguous()
-
-
-def _inertia_grad(gi, like):
-    """[10*nb, B] gradient summed over the horizon -> the [B, nb, 10] layout (dtype, device) of the per-world inertia input."""
-    if gi is None:
-        return None
-    return gi.t().reshape(like.shape).to(device=like.device, dtype=like.dtype)
 
 
 def rollout_fused(world, state0: torch.Tensor, actions: torch.Tensor, checkpoint_every: int = 0, mass: Optional[torch.Tensor] = None) -> torch.Tensor:

@@ -24,6 +24,22 @@ def _ptr(t: torch.Tensor) -> int:
     return t.data_ptr()
 
 
+def _word_major_inertia(dm, world_inertia, B, dev):
+    """[B, nb, 10] per-world inertia -> the kernels' word-major [10*nb, B] fp64 layout on `dev`, so that the worlds of a warp read
+    adjacent words (None stays None)."""
+    if world_inertia is None:
+        return None
+    return world_inertia.detach().to(device=dev, dtype=torch.float64).reshape(B, 10 * dm.cm.nb).t().contiguous()
+
+
+def _inertia_grad(gi, like):
+    """The kernels' [10*nb, B] inertia gradient -> world w's own dL/d(inertia) in the [B, nb, 10] layout (dtype, device) of the
+    per-world inertia input (None stays None)."""
+    if gi is None:
+        return None
+    return gi.t().to(torch.float64).reshape(like.shape).to(device=like.device, dtype=like.dtype)
+
+
 class TimestepLayer(torch.autograd.Function):
     """world_inertia (optional): per-world canonical inertia [B, nb, 10] (modelspec.mass_to_inertia); it replaces the model's table for
     world w only, and its gradient is the kernels' per-world dL/d(inertia).  Exclusive with the 1-D `mass` argument."""
@@ -66,13 +82,10 @@ class TimestepLayer(torch.autograd.Function):
         sd = s2.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
         ad = a2.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
         B = sd.shape[0]
-        wi = None
-        if world_inertia is not None:
-            if legacy or tuple(world_inertia.shape) != (B, dm.cm.nb, 10):
-                raise ValueError(f"timestep(): per-world inertia has shape {tuple(world_inertia.shape)}, expected [{B}, {dm.cm.nb}, 10] "
-                                 "with a 2-D state")
-            # word-major [10*nb, B] on the step's device: the worlds of a warp read adjacent words
-            wi = world_inertia.detach().to(device=dev, dtype=torch.float64).reshape(B, 10 * dm.cm.nb).t().contiguous()
+        if world_inertia is not None and (legacy or tuple(world_inertia.shape) != (B, dm.cm.nb, 10)):
+            raise ValueError(f"timestep(): per-world inertia has shape {tuple(world_inertia.shape)}, expected [{B}, {dm.cm.nb}, 10] "
+                             "with a 2-D state")
+        wi = _word_major_inertia(dm, world_inertia, B, dev)
         wi_ptr = _ptr(wi) if wi is not None else None
         ctx.wi_grad = world_inertia is not None and ctx.needs_input_grad[4]
         ctx.wi_like = world_inertia
@@ -151,9 +164,7 @@ class TimestepLayer(torch.autograd.Function):
         if ctx.mass_grad:
             # lossWrtMass = massVel^T g_v' (BackpropSnapshot.cpp:177-178), summed over the worlds that share the model
             gm = (ctx.mass_P @ gi.to(torch.float64).sum(dim=1)).to(device=ctx.mass_like.device, dtype=ctx.mass_like.dtype)
-        gw = None
-        if ctx.wi_grad:  # world w's own dL/d(inertia): [10*nb, B] -> [B, nb, 10]
-            gw = gi.t().to(torch.float64).reshape(ctx.wi_like.shape).to(device=ctx.wi_like.device, dtype=ctx.wi_like.dtype)
+        gw = _inertia_grad(gi, ctx.wi_like) if ctx.wi_grad else None
         if ctx.legacy:
             # reference returns fp64 grads (timestep.py:55-60)
             gs = gs[0].to(device=ctx.in_device, dtype=torch.float64 if ctx.in_dtype == torch.float64 else ctx.in_dtype)

@@ -26,27 +26,37 @@ def lib():
 
 
 def _p(a):
-    return a.ctypes.data_as(ctypes.c_void_p)
+    return a.ctypes.data_as(ctypes.c_void_p) if a is not None else None
 
 
 class EmulWorld:
+    """The four step calls take an optional per-world canonical inertia `world_inertia` [B, nb, 10] as their last keyword argument
+    (None: the model's table)."""
+
     def __init__(self, cm):
         self.cm = cm
         self.desc, self._keep = make_desc(cm)
         self.n, self.na = cm.ndof, len(cm.action_map)
         self.sw = lib().emul_saved_words(ctypes.byref(self.desc))
 
-    def forward(self, state, action, fp64=False):
+    def _wi(self, world_inertia, B):
+        if world_inertia is None:
+            return None
+        wi = np.asarray(world_inertia, np.float64).reshape(B, 10 * self.cm.nb)
+        return np.ascontiguousarray(wi.T)  # word-major [10*nb, B], the layout of the *_pw entry points
+
+    def forward(self, state, action, fp64=False, world_inertia=None):
         state = np.ascontiguousarray(state, np.float32)
         action = np.ascontiguousarray(action, np.float32)
         B = state.shape[0]
         nxt = np.empty_like(state)
         saved = np.zeros((self.sw, B), np.float64 if fp64 else np.float32)
-        rc = lib().emul_forward(ctypes.byref(self.desc), B, _p(state), _p(action), _p(nxt), _p(saved), int(fp64))
+        rc = lib().emul_forward(ctypes.byref(self.desc), B, _p(state), _p(action), _p(nxt), _p(saved), int(fp64),
+                                _p(self._wi(world_inertia, B)))
         assert rc == 0
         return nxt, saved
 
-    def backward(self, state, action, saved, gnext, fp64=False, want_inertia_grad=False):
+    def backward(self, state, action, saved, gnext, fp64=False, want_inertia_grad=False, world_inertia=None):
         state = np.ascontiguousarray(state, np.float32)
         action = np.ascontiguousarray(action, np.float32)
         gnext = np.ascontiguousarray(gnext, np.float32)
@@ -55,11 +65,11 @@ class EmulWorld:
         ga = np.empty_like(action)
         gi = np.zeros((10 * self.cm.nb, B), np.float32) if want_inertia_grad else None
         rc = lib().emul_backward(ctypes.byref(self.desc), B, _p(state), _p(action), _p(saved), _p(gnext), _p(gs),
-                                 _p(ga), int(fp64), _p(gi) if gi is not None else None)
+                                 _p(ga), int(fp64), _p(gi), _p(self._wi(world_inertia, B)))
         assert rc == 0
         return (gs, ga, gi) if want_inertia_grad else (gs, ga)
 
-    def forward_contact(self, state, action, x_lcp=None, m_lcp=None, small_mc=8, reverse=False):
+    def forward_contact(self, state, action, x_lcp=None, m_lcp=None, small_mc=8, reverse=False, world_inertia=None):
         """fp64 ABA + warp-cooperative contact stage (host build).  -> dict(next, saved, x, m, labels, status, nc, cinfo, crec).
         small_mc: contact capacity of the emulated shared-memory workspace (worlds beyond it retry in the large one);
         reverse: run every CW_FOR of the odd worlds backwards."""
@@ -78,20 +88,22 @@ class EmulWorld:
         cinfo = np.zeros((B, MAX_CONTACTS, 10), np.float32)
         crec = np.zeros((B, lib().emul_contact_rec_doubles(ctypes.byref(self.desc))), np.float64)
         rc = lib().emul_forward_contact(ctypes.byref(self.desc), B, _p(state), _p(action), _p(nxt), _p(saved), _p(x), _p(m),
-                                        _p(labels), _p(status), _p(nc), _p(cinfo), _p(crec), int(small_mc), int(reverse))
+                                        _p(labels), _p(status), _p(nc), _p(cinfo), _p(crec), int(small_mc), int(reverse),
+                                        _p(self._wi(world_inertia, B)))
         assert rc == 0
         return dict(next=nxt, saved=saved, x=x, m=m, labels=labels, status=status, nc=nc, cinfo=cinfo, crec=crec)
 
-    def backward_contact(self, state, action, saved, crec, gnext, want_inertia_grad=False, small_mc=8, reverse=False):
+    def backward_contact(self, state, action, saved, crec, gnext, want_inertia_grad=False, small_mc=8, reverse=False, world_inertia=None):
         state = np.ascontiguousarray(state, np.float32)
         action = np.ascontiguousarray(action, np.float32)
         gnext = np.ascontiguousarray(gnext, np.float32)
+        B = state.shape[0]
         gs, ga = np.empty_like(state), np.empty_like(action)
-        gi = np.zeros((10 * self.cm.nb, state.shape[0]), np.float32) if want_inertia_grad else None
-        self.bwd_status = np.zeros(state.shape[0], np.int32)
-        rc = lib().emul_backward_contact(ctypes.byref(self.desc), state.shape[0], _p(state), _p(action), _p(saved), _p(crec),
-                                         _p(gnext), _p(gs), _p(ga), _p(gi) if gi is not None else None, _p(self.bwd_status),
-                                         int(small_mc), int(reverse))
+        gi = np.zeros((10 * self.cm.nb, B), np.float32) if want_inertia_grad else None
+        self.bwd_status = np.zeros(B, np.int32)
+        rc = lib().emul_backward_contact(ctypes.byref(self.desc), B, _p(state), _p(action), _p(saved), _p(crec),
+                                         _p(gnext), _p(gs), _p(ga), _p(gi), _p(self.bwd_status),
+                                         int(small_mc), int(reverse), _p(self._wi(world_inertia, B)))
         assert rc == 0
         return (gs, ga, gi) if want_inertia_grad else (gs, ga)
 

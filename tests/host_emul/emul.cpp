@@ -1,5 +1,7 @@
 // DEVELOPMENT/TEST HARNESS ONLY — compiles the per-world device functions (csrc/nb2_dyn.cuh) as host code so that
 // the kernel math can be checked against the oracle in the GPU-less build container (tests/test_host_emul.py).
+// Every runner takes an optional per-world canonical inertia table `winertia` (fp64, word-major [10*nb][B] as the *_pw
+// entry points take it); NULL = the model's table (tests/test_per_world_mass.py).
 // It is never loaded by the nimblephysics_b200 package: the product path has no CPU fallback.
 #include <string>
 #include <vector>
@@ -12,7 +14,7 @@
 // reverse order so that a missing barrier (a cross-lane dependency inside one stage) shows up as a poisoned read.
 constexpr int G = 3, NT = 5;
 template <class R>
-static int run_fwd(const nb2_model_desc* d, int B, const float* state, const float* action, float* next, R* saved) {
+static int run_fwd(const nb2_model_desc* d, int B, const float* state, const float* action, float* next, R* saved, const double* winertia) {
   Nb2ModelDev<R> M; std::string err;
   if (!nb2_fill_model(*d, M, err)) { fprintf(stderr, "emul: %s\n", err.c_str()); return -1; }
   nb2::FwdLayout L = nb2::fwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
@@ -26,7 +28,8 @@ static int run_fwd(const nb2_model_desc* d, int B, const float* state, const flo
       for (int slot = 0; slot < nw; slot++)
         for (int l = 0; l < M.lanes; l++) {
           const int w = g0 + slot, lane = (w & 1) ? M.lanes - 1 - l : l;
-          nb2::world_forward_stage<R, G>(M, scr.data() + slot, saved ? saved + w : nullptr, (size_t)B, saved != nullptr, lane, sg);
+          nb2::world_forward_stage<R, G>(M, scr.data() + slot, saved ? saved + w : nullptr, (size_t)B, saved != nullptr, lane, sg, nullptr, nullptr,
+                                         winertia ? winertia + w : nullptr, (size_t)B);
         }
     }
   }
@@ -34,7 +37,7 @@ static int run_fwd(const nb2_model_desc* d, int B, const float* state, const flo
 }
 template <class R>
 static int run_bwd(const nb2_model_desc* d, int B, const float* state, const float* action, const R* saved,
-                   const float* gnext, float* gstate, float* gaction, float* ginertia) {
+                   const float* gnext, float* gstate, float* gaction, float* ginertia, const double* winertia) {
   Nb2ModelDev<R> M; std::string err;
   if (!nb2_fill_model(*d, M, err)) { fprintf(stderr, "emul: %s\n", err.c_str()); return -1; }
   nb2::BwdLayout L = nb2::bwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
@@ -52,7 +55,8 @@ static int run_bwd(const nb2_model_desc* d, int B, const float* state, const flo
       for (int slot = 0; slot < nw; slot++)
         for (int l = 0; l < M.lanes; l++) {
           const int w = g0 + slot, lane = (w & 1) ? M.lanes - 1 - l : l;
-          nb2::world_backward_stage<R, G>(M, scr.data() + slot, saved + w, (size_t)B, lane, sg, ginertia ? ginertia + w : nullptr);
+          nb2::world_backward_stage<R, G>(M, scr.data() + slot, saved + w, (size_t)B, lane, sg, ginertia ? ginertia + w : nullptr, nullptr, 0, nullptr,
+                                          winertia ? winertia + w : nullptr, (size_t)B);
         }
     }
   }
@@ -64,7 +68,8 @@ static nb2::cw::Dims contact_dims(const Nb2ModelDev<double>& M, const Nb2Contact
   return nb2::cw::make_dims(M.nb, M.ndof, M.nfree, MC, MR, C.ncb, C.max_chain_dofs);
 }
 static int run_fwd_contact(const nb2_model_desc* d, int B, const float* state, const float* action, float* next, double* saved,
-                           double* x_lcp, int* m_lcp, int* labels, int* status, int* nc, float* cinfo, double* crec, int small_mc, int reverse) {
+                           double* x_lcp, int* m_lcp, int* labels, int* status, int* nc, float* cinfo, double* crec, int small_mc, int reverse,
+                           const double* winertia) {
   Nb2ModelDev<double> M; Nb2ContactDev C; std::string err;
   if (!nb2_fill_model(*d, M, err) || !nb2_fill_contact(*d, C, err)) { fprintf(stderr, "emul: %s\n", err.c_str()); return -1; }
   nb2::FwdLayout L = nb2::fwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
@@ -83,7 +88,8 @@ static int run_fwd_contact(const nb2_model_desc* d, int B, const float* state, c
     for (int sg = 1; sg < NB2_FWD_STAGES - 1; sg++)
       for (int l = 0; l < M.lanes; l++) {
         const int lane = (w & 1) ? M.lanes - 1 - l : l;
-        nb2::world_forward_stage<double, 1>(M, scr.data(), saved + (size_t)w * words, 1, true, lane, sg, nullptr, ws0.Iinv);
+        nb2::world_forward_stage<double, 1>(M, scr.data(), saved + (size_t)w * words, 1, true, lane, sg, nullptr, ws0.Iinv,
+                                            winertia ? winertia + w : nullptr, (size_t)B);
       }
     nb2::cw::FwdIO io;
     io.x_io = x_lcp + (size_t)w * NB2_MAX_ROWS; io.m_io = m_lcp + w; io.labels = labels + (size_t)w * NB2_MAX_ROWS; io.status = status + w;
@@ -98,7 +104,8 @@ static int run_fwd_contact(const nb2_model_desc* d, int B, const float* state, c
 // fused backward with the contact stage, as k_cstep_bwd runs it: lambda sweeps (B1, B2) along the schedule, the warp-cooperative
 // contact adjoint, reverse RNEA sweep (B3) + assembly with the contact injections, store.
 static int run_bwd_contact(const nb2_model_desc* d, int B, const float* state, const float* action, const double* saved,
-                           const double* crec, const float* gnext, float* gstate, float* gaction, float* ginertia, int* bstatus, int small_mc, int reverse) {
+                           const double* crec, const float* gnext, float* gstate, float* gaction, float* ginertia, int* bstatus, int small_mc, int reverse,
+                           const double* winertia) {
   Nb2ModelDev<double> M; Nb2ContactDev C; std::string err;
   if (!nb2_fill_model(*d, M, err) || !nb2_fill_contact(*d, C, err)) { fprintf(stderr, "emul: %s\n", err.c_str()); return -1; }
   nb2::BwdLayout L = nb2::bwd_layout(M.nb, M.ndof, M.nslots, M.nfree, 42);
@@ -119,9 +126,8 @@ static int run_bwd_contact(const nb2_model_desc* d, int B, const float* state, c
     nb2::cw::Ws wsd = nb2::cw::carve(wss.data(), ds);
     nb2::BwdContactData<1> c2 = cd;
     float* gI = ginertia ? ginertia + w : nullptr;
-    for (int it = 0; it < 10; it++) {  // the stage order of k_cstep_bwd
-      const bool second = (it == 6) | (it == 7);
-      const int sg = (it < 4) ? it + 1 : (it == 4 || it == 6) ? 5 : (it == 5 || it == 7) ? 7 : (it == 8) ? 6 : 8;
+    for (int it = 0; it < NB2_CBWD_ITERS; it++) {  // the stage order of k_cstep_bwd
+      const auto [sg, second] = nb2::cbwd_iter(it);
       if (it == 4) {
         int pc = 0; nb2::cw::BigPool pool{&pc, wsb.data(), wsb.size(), 1};
         cd = nb2::cw::contact_backward<true>(M, C, st, sv, &wsd, ds, pool, db, crec + (size_t)w * recd, scr.data(), L.oLam, L.oBody);
@@ -131,7 +137,8 @@ static int run_bwd_contact(const nb2_model_desc* d, int B, const float* state, c
       if (it == 8 && cd.bounce) nb2::cw::bounce_pass2_end(M, wsd, scr.data(), L.oLam);
       for (int l = 0; l < M.lanes; l++) {
         const int lane = (w & 1) ? M.lanes - 1 - l : l;
-        nb2::world_backward_stage<double, 1, true>(M, scr.data(), sv, 1, lane, sg, gI, nullptr, (size_t)B, second ? &c2 : &cd);
+        nb2::world_backward_stage<double, 1, true>(M, scr.data(), sv, 1, lane, sg, gI, nullptr, (size_t)B, second ? &c2 : &cd,
+                                                   winertia ? winertia + w : nullptr, (size_t)B);
       }
     }
     nb2::bwd_store<double, 1, true>(M, scr.data(), gstate + (size_t)w * 2 * M.ndof, gaction + (size_t)w * M.na, cd.error != 0, 1, 0, 1);
@@ -161,24 +168,26 @@ int emul_cw_solve_chain(int m, const double* A, const double* b, const double* l
   return run_cw_chain(m, A, b, lo, hi, fi, x0, have_x0, cfm, x_out, mapping_out, reverse);
 }
 int emul_forward_contact(const nb2_model_desc* d, int B, const float* state, const float* action, float* next, double* saved,
-                         double* x_lcp, int* m_lcp, int* labels, int* status, int* nc, float* cinfo, double* crec, int small_mc, int reverse) {
-  return run_fwd_contact(d, B, state, action, next, saved, x_lcp, m_lcp, labels, status, nc, cinfo, crec, small_mc, reverse);
+                         double* x_lcp, int* m_lcp, int* labels, int* status, int* nc, float* cinfo, double* crec, int small_mc, int reverse,
+                         const double* winertia) {
+  return run_fwd_contact(d, B, state, action, next, saved, x_lcp, m_lcp, labels, status, nc, cinfo, crec, small_mc, reverse, winertia);
 }
 int emul_backward_contact(const nb2_model_desc* d, int B, const float* state, const float* action, const double* saved,
-                          const double* crec, const float* gnext, float* gstate, float* gaction, float* ginertia, int* bstatus, int small_mc, int reverse) {
-  return run_bwd_contact(d, B, state, action, saved, crec, gnext, gstate, gaction, ginertia, bstatus, small_mc, reverse);
+                          const double* crec, const float* gnext, float* gstate, float* gaction, float* ginertia, int* bstatus, int small_mc, int reverse,
+                          const double* winertia) {
+  return run_bwd_contact(d, B, state, action, saved, crec, gnext, gstate, gaction, ginertia, bstatus, small_mc, reverse, winertia);
 }
 int emul_contact_rec_doubles(const nb2_model_desc* d) { return (int)nb2::cw::record_doubles(d->ndof); }
 int emul_saved_words(const nb2_model_desc* d) {
   int nfree = 0; for (int i = 0; i < d->nb; i++) nfree += d->jtype[i] == NB2_JT_FREE;
   return nb2_saved_words(d->nb, d->ndof, nfree);
 }
-int emul_forward(const nb2_model_desc* d, int B, const float* state, const float* action, float* next, void* saved, int fp64) {
-  return fp64 ? run_fwd<double>(d, B, state, action, next, (double*)saved) : run_fwd<float>(d, B, state, action, next, (float*)saved);
+int emul_forward(const nb2_model_desc* d, int B, const float* state, const float* action, float* next, void* saved, int fp64, const double* winertia) {
+  return fp64 ? run_fwd<double>(d, B, state, action, next, (double*)saved, winertia) : run_fwd<float>(d, B, state, action, next, (float*)saved, winertia);
 }
 int emul_backward(const nb2_model_desc* d, int B, const float* state, const float* action, const void* saved,
-                  const float* gnext, float* gstate, float* gaction, int fp64, float* ginertia) {
-  return fp64 ? run_bwd<double>(d, B, state, action, (const double*)saved, gnext, gstate, gaction, ginertia)
-              : run_bwd<float>(d, B, state, action, (const float*)saved, gnext, gstate, gaction, ginertia);
+                  const float* gnext, float* gstate, float* gaction, int fp64, float* ginertia, const double* winertia) {
+  return fp64 ? run_bwd<double>(d, B, state, action, (const double*)saved, gnext, gstate, gaction, ginertia, winertia)
+              : run_bwd<float>(d, B, state, action, (const float*)saved, gnext, gstate, gaction, ginertia, winertia);
 }
 }

@@ -11,7 +11,6 @@ import nimblephysics_b200 as nb
 from nimblephysics_b200 import modelspec as ms
 from oracle import binding as ob
 from tests.host_emul.binding import EmulWorld
-from tests.host_emul.binding_pw import EmulWorldPW
 from tests.util import contact_inputs, load_raw, rel_err, sample_inputs
 
 KINDS = [ms.INERTIA_MASS, ms.INERTIA_COM, ms.INERTIA_DIAGONAL, ms.INERTIA_OFF_DIAGONAL, ms.INERTIA_FULL]
@@ -135,7 +134,7 @@ def test_emulated_per_world_step_matches_oracle(oracle_mod, name, fp64, lanes):
     B = 4
     raw, world, M, wi = _per_world(name, B, seed=11 + lanes)
     cm = nb.compile_model(raw, lanes=lanes)
-    ew = EmulWorldPW(cm)
+    ew = EmulWorld(cm)
     s, a, g = sample_inputs(raw, B, seed=31)
     nxt, saved = ew.forward(s, a, fp64, world_inertia=wi)
     gs, ga, gi = ew.backward(s, a, saved, g, fp64, want_inertia_grad=True, world_inertia=wi)
@@ -162,7 +161,7 @@ def test_emulated_per_world_contact_step_matches_oracle(oracle_mod, name):
     B = 4
     raw, world, M, wi = _per_world(name, B, seed=5)
     cm = nb.compile_model(raw)
-    ew = EmulWorldPW(cm)
+    ew = EmulWorld(cm)
     s, a = contact_inputs(raw, name, B, seed=3)
     g = np.random.default_rng(2).normal(size=(B, 2 * raw.ndof)).astype(np.float32)
     r = ew.forward_contact(s, a, reverse=True, world_inertia=wi)
@@ -192,19 +191,19 @@ def test_emulated_per_world_contact_step_matches_oracle(oracle_mod, name):
 
 @pytest.mark.parametrize("lanes", [1, 2, 4, 8])
 def test_emulated_replicated_model_inertia_is_bit_identical(lanes):
-    """The model's own table, replicated per world, reproduces the shared-table path (the plain harness) bit for bit."""
+    """The model's own table, replicated per world, reproduces the shared-table path (world_inertia=None) bit for bit."""
     raw = load_raw("atlas")
     cm = nb.compile_model(raw, lanes=lanes)
-    ew, ewp = EmulWorld(cm), EmulWorldPW(cm)
+    ew = EmulWorld(cm)
     B = 5
     wi = np.broadcast_to(cm.inertia, (B, cm.nb, 10))
     s, a, g = sample_inputs(raw, B, seed=8)
     for fp64 in (False, True):
         n0, sv0 = ew.forward(s, a, fp64)
-        n1, sv1 = ewp.forward(s, a, fp64, world_inertia=wi)
+        n1, sv1 = ew.forward(s, a, fp64, world_inertia=wi)
         assert np.array_equal(n0, n1) and np.array_equal(sv0, sv1)
         r0 = ew.backward(s, a, sv0, g, fp64, want_inertia_grad=True)
-        r1 = ewp.backward(s, a, sv1, g, fp64, want_inertia_grad=True, world_inertia=wi)
+        r1 = ew.backward(s, a, sv1, g, fp64, want_inertia_grad=True, world_inertia=wi)
         assert all(np.array_equal(x, y) for x, y in zip(r0, r1))
 
 
@@ -212,14 +211,14 @@ def test_emulated_replicated_model_inertia_is_bit_identical(lanes):
 def test_emulated_replicated_model_inertia_is_bit_identical_with_contacts(name):
     raw = load_raw(name)
     cm = nb.compile_model(raw)
-    ew, ewp = EmulWorld(cm), EmulWorldPW(cm)
+    ew = EmulWorld(cm)
     B = 4
     wi = np.broadcast_to(cm.inertia, (B, cm.nb, 10))
     s, a = contact_inputs(raw, name, B, seed=6)
     g = np.random.default_rng(4).normal(size=(B, 2 * raw.ndof)).astype(np.float32)
     r0 = ew.forward_contact(s, a, reverse=True, small_mc=2)
-    r1 = ewp.forward_contact(s, a, reverse=True, small_mc=2, world_inertia=wi)
+    r1 = ew.forward_contact(s, a, reverse=True, small_mc=2, world_inertia=wi)
     assert all(np.array_equal(r0[k], r1[k]) for k in r0)
     b0 = ew.backward_contact(s, a, r0["saved"], r0["crec"], g, want_inertia_grad=True, reverse=True, small_mc=2)
-    b1 = ewp.backward_contact(s, a, r1["saved"], r1["crec"], g, want_inertia_grad=True, reverse=True, small_mc=2, world_inertia=wi)
+    b1 = ew.backward_contact(s, a, r1["saved"], r1["crec"], g, want_inertia_grad=True, reverse=True, small_mc=2, world_inertia=wi)
     assert all(np.array_equal(x, y) for x, y in zip(b0, b1))
