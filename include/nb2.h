@@ -200,6 +200,26 @@ int nb2_model_contact_capacity(const nb2_model* m);
  * space (every dof). */
 int nb2_forward_dynamics(const nb2_model* m, int B, const double* pos, const double* vel, const double* force, double* accel, void* stream);
 
+/* Contact-free inverse dynamics of B worlds: the generalised force tau [B, ndof] for which the contact-free step started at
+ * state = [q ; qdot] reaches the next velocity next_vel [B, ndof]:
+ *     a = (next_vel - qdot) / dt ,   tau = M(q) a + C(q, qdot) + g(q) + K (q - q0 + qdot dt) + D qdot      (per dof)
+ * (the step's semi-implicit spring and damping).  tau is in dof space, not gathered through the action map; free joints use the step's
+ * conventions (rotation-vector positions, body-twist velocities, the 6-vector joint force in the joint frame).  Contacts, joint-limit rows
+ * and force limits are ignored: a model with collision pairs gets the tau of its tree, and no LCP cache is read or written.  The round trip
+ * holds: with an action space covering every dof, nb2_step_forward(state, tau) returns next_vel up to rounding.
+ * UNLIKE the step entry points, the rows are in the arithmetic type: state, next_vel, tau, grad_* are float with NB2_FP32 and double
+ * with NB2_FP64 (device memory, row-major, one row per world).  world_inertia (may be NULL): per-world inertia as for nb2_step_forward_pw.
+ * saved (may be NULL when no backward will follow): nb2_saved_words_per_world(m) * B words of the arithmetic type, [words][B], the step's
+ * saved-stream layout.  Launch shapes and lane schedules are picked per call as for the step (nb2_model_add_schedule). */
+int nb2_inverse_dynamics(const nb2_model* m, int B, const void* state, const void* next_vel, const double* world_inertia, void* tau, void* saved,
+                         int precision, void* stream);
+/* Vector-Jacobian product of the same call, with the SAME state, world_inertia and saved stream (next_vel is not read: the saved stream
+ * holds the accelerations it implies; it may be NULL).  grad_tau [B, ndof] -> grad_state [B, 2*ndof] = [dL/dq ; dL/dqdot], grad_next_vel
+ * [B, ndof] (all in the arithmetic type); grad_inertia (may be NULL): [10*nb][B] DOUBLES, dL/d(m, h, Ibar) of every canonical body and
+ * world, laid out as nb2_step_backward's (contract with modelspec.inertia_param_jacobian for dL/dmass).  No clipping is applied. */
+int nb2_inverse_dynamics_backward(const nb2_model* m, int B, const void* state, const void* next_vel, const double* world_inertia, const void* saved,
+                                  const void* grad_tau, void* grad_state, void* grad_next_vel, double* grad_inertia, int precision, void* stream);
+
 /* Batched boxed-LCP solves on the device: B independent problems, one warp each — the reference's pointer-style lower boundary
  * BoxedLcpSolver::solve(n, A, x, b, nub, lo, hi, findex, earlyTermination) (dart/constraint/BoxedLcpSolver.hpp:125-135) and the
  * solve chain of BoxedLcpConstraintSolver::solveLcp (BoxedLcpConstraintSolver.cpp:352-789).  Device pointers; problem w has dimension

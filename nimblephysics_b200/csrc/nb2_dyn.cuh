@@ -913,4 +913,241 @@ NB2_HD void world_backward_stage(const Nb2ModelDev<R>& M, R* scr, const R* sv, s
   }
 }
 
+// =====================================================================================================
+// inverse dynamics: tau = ID(q, qdot, a) with a = (v' - qdot) / dt, the generalised force for which the contact-free step
+// reaches the next velocity v' (RNEA over the cooperative-lane schedule; DESIGN.md §6e).  Its I/O rows are in the arithmetic
+// type R.  Forward scratch: fwd_layout — q, qdot; v' in the n action words (then tau); body record V(0..5) sin/cos(6, 7) A(8..13);
+// fwd slot k: words 0..5 hold a child's force.  With `save` it writes what bwd_B3 reads of the step's saved stream: V, A, sin/cos,
+// the free-joint transforms and qdd = a (never U, psi or the inverse articulated inertias).
+// =====================================================================================================
+template <class R> NB2_HD R comp6(const V6<R>& v, int k) {
+  return k == 0 ? v.a.x : k == 1 ? v.a.y : k == 2 ? v.a.z : k == 3 ? v.l.x : k == 4 ? v.l.y : v.l.z;
+}
+// rows [nworlds, width] of a group <-> scratch words [base, base + width) (element type R both sides)
+template <class R, int ST>
+NB2_HD void id_rows_load(R* scr0, const R* src, int width, unsigned magic, int base, int nworlds, int tid, int nthr) {
+  for (int idx = tid; idx < nworlds * width; idx += nthr) {
+    const int slot = (int)fast_div((unsigned)idx, magic), d = idx - slot * width;
+    scr0[(size_t)(base + d) * ST + slot] = src[idx];
+  }
+}
+template <class R, int ST>
+NB2_HD void id_rows_store(const R* scr0, R* dst, int width, unsigned magic, int base, int nworlds, int tid, int nthr) {
+  for (int idx = tid; idx < nworlds * width; idx += nthr) {
+    const int slot = (int)fast_div((unsigned)idx, magic), d = idx - slot * width;
+    dst[idx] = scr0[(size_t)(base + d) * ST + slot];
+  }
+}
+
+// root -> leaf: A_i = X^-1 A_p + S a + ad(V_i, S qdot), base acceleration -g (as fwd_pass3)
+template <class R, int ST>
+NB2_HD void id_pass_acc(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool save, int lo, int hi, const R* bt) {
+  const FwdLayout L = fwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
+  const R rdt = R(1) / M.dt;
+  const int kFree = M.nb * 21, kQdd = M.nb * 21 + M.nfree * 33;
+  V6<R> A0; A0.a = zero3<R>(); A0.l = mk3<R>(-M.gravity[0], -M.gravity[1], -M.gravity[2]);
+  for (int i = lo; i < hi; i++) {
+    const int jt = M.jtype[i], p = M.parent[i], o = M.dof_off[i];
+    R* bs = scr + (size_t)(L.oBody + NB2_FWD_BODY_WORDS * i) * ST;
+    const Xf<R> T = body_xf_fwd<R, ST>(M, bt, i, scr, L);
+    const V6<R> Ap = AdInvT(T, (p >= 0) ? ld6<R, ST>(scr + (size_t)(L.oBody + NB2_FWD_BODY_WORDS * p + 8) * ST) : A0);
+    const V6<R> V = ld6<R, ST>(bs);
+    V6<R> A = Ap;
+    if (jt != NB2_JT_FREE) {
+      const R vq = scr[(size_t)(L.oV + o) * ST];
+      const R a = (scr[(size_t)(L.oAct + o) * ST] - vq) * rdt;
+      if (jt == NB2_JT_REV) { A.a.z += a; A.a.x += V.a.y * vq; A.a.y -= V.a.x * vq; A.l.x += V.l.y * vq; A.l.y -= V.l.x * vq; }
+      else { A.l.z += a; A.l.x += V.a.y * vq; A.l.y -= V.a.x * vq; }
+      if (save) sv[(size_t)(kQdd + o) * B] = a;
+    } else {
+      const V6<R> Vj = ld6<R, ST>(scr + (size_t)(L.oV + o) * ST);
+      const V6<R> a = (ld6<R, ST>(scr + (size_t)(L.oAct + o) * ST) - Vj) * rdt;
+      A = Ap + a + ad(V, Vj);
+      if (save) {
+        sv_st6(sv + (size_t)(kQdd + o) * B, B, 0, a);
+        const R* fr = scr + (size_t)(L.oFree + 18 * M.free_idx[i]) * ST;
+        R* sf = sv + (size_t)(kFree + M.free_idx[i] * 33 + 21) * B;
+        for (int k = 0; k < 12; k++) sf[(size_t)k * B] = fr[(size_t)k * ST];
+      }
+    }
+    st6<R, ST>(bs + 8 * ST, A);
+    if (save) {
+      R* s = sv + (size_t)(i * 21) * B;
+      sv_st6(s, B, 0, V); sv_st6(s, B, 6, A);
+      s[19 * B] = (jt == NB2_JT_REV) ? bs[6 * ST] : R(0); s[20 * B] = (jt == NB2_JT_REV) ? bs[7 * ST] : R(0);
+    }
+  }
+}
+
+// leaf -> root: f_i = G A_i + V_i x* G V_i + sum_c X*_c f_c ; tau = S^T f_i + K (q - q0 + qdot dt) + D qdot (into the action words)
+template <class R, int ST>
+NB2_HD void id_pass_force(const Nb2ModelDev<R>& M, R* scr, int lo, int hi, const R* bt, const double* wi, size_t wiB) {
+  const FwdLayout L = fwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
+  const R dt = M.dt;
+  V6<R> hf = zero6<R>();
+  bool hvalid = false;
+  for (int i = hi - 1; i >= lo; i--) {
+    const int jt = M.jtype[i], p = M.parent[i], o = M.dof_off[i], fl = M.flags[i];
+    const R* bs = scr + (size_t)(L.oBody + NB2_FWD_BODY_WORDS * i) * ST;
+    R m; V3<R> h; S3<R> Ib; inertia_of(M, bt, wi, wiB, i, &m, &h, &Ib);
+    const V6<R> V = ld6<R, ST>(bs), A = ld6<R, ST>(bs + 8 * ST);
+    V6<R> f = mulG(m, h, Ib, A) + crf(V, mulG(m, h, Ib, V));
+    if (hvalid) f = f + hf;
+    if (fl & NB2_F_HAS_SLOT)
+      for (int k = 0; k < M.slot_count[i]; k++) f = f + ld6<R, ST>(scr + (size_t)(L.oSlot + 27 * (M.slot_self[i] + k)) * ST);
+    const int nd = (jt == NB2_JT_FREE) ? 6 : 1;
+    for (int k = 0; k < nd; k++) {
+      const int d = o + k;
+      const R qd = scr[(size_t)(L.oQ + d) * ST], vd = scr[(size_t)(L.oV + d) * ST];
+      const R fk = (jt == NB2_JT_FREE) ? comp6(f, k) : S_dot(jt, f);
+      scr[(size_t)(L.oAct + d) * ST] = fk + M.spring[d] * (qd - M.rest[d] + vd * dt) + M.damping[d] * vd;
+    }
+    hvalid = false;
+    if (p >= 0) {
+      const V6<R> fc = dAdInvT(body_xf_fwd<R, ST>(M, bt, i, scr, L), f);
+      if (fl & NB2_F_HANDOFF) { hf = fc; hvalid = true; }
+      else st6<R, ST>(scr + (size_t)(L.oSlot + 27 * M.slot_parent[i]) * ST, fc);
+    }
+  }
+}
+
+// Stages of the inverse-dynamics forward (the trunk / limb split of world_forward_stage):
+//   0 group load of [q; qdot] and v' | barrier
+//   1 trunk V, A (lane 0) | barrier      2 limb V, A      3 limb f, tau | barrier      4 trunk f, tau (lane 0) | barrier
+//   5 group store of tau
+#define NB2_ID_FWD_STAGES 6
+#define NB2_ID_FWD_SYNC_MASK 0x1Bu        /* after stages 0, 1, 3, 4 */
+#define NB2_ID_FWD_SYNC_MASK_1LANE 0x11u  /* lanes == 1: after the group load and before the group store */
+template <class R, int ST>
+NB2_HD void id_forward_stage(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool save, int lane, int stage, const R* bt,
+                             const double* wi, size_t wiB) {
+  const bool trunk = (stage == 1) | (stage == 4);
+  if (trunk && lane != 0) return;
+  const int nr = trunk ? M.trunk_n : M.limb_n[lane];
+  for (int rr = 0; rr < nr; rr++) {
+    const int r = (stage >= 3) ? nr - 1 - rr : rr;
+    const int lo = trunk ? M.trunk_lo[r] : M.limb_lo[lane][r], hi = trunk ? M.trunk_hi[r] : M.limb_hi[lane][r];
+    if (stage <= 2) { fwd_pass1<R, ST>(M, scr, lo, hi, bt); id_pass_acc<R, ST>(M, scr, sv, B, save, lo, hi, bt); }
+    else id_pass_force<R, ST>(M, scr, lo, hi, bt, wi, wiB);
+  }
+}
+template <class R, int ST>
+NB2_HD void id_load(const Nb2ModelDev<R>& M, R* scr0, const R* st0, const R* nv0, int nworlds, int tid, int nthr) {
+  const FwdLayout L = fwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
+  id_rows_load<R, ST>(scr0, st0, 2 * M.ndof, M.magic_n2, L.oQ, nworlds, tid, nthr);  // oV = oQ + n
+  id_rows_load<R, ST>(scr0, nv0, M.ndof, M.magic_n, L.oAct, nworlds, tid, nthr);
+}
+template <class R, int ST>
+NB2_HD void id_store(const Nb2ModelDev<R>& M, const R* scr0, R* tau0, int nworlds, int tid, int nthr) {
+  const FwdLayout L = fwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
+  id_rows_store<R, ST>(scr0, tau0, M.ndof, M.magic_n, L.oAct, nworlds, tid, nthr);
+}
+
+// ---- backward (VJP) with lambda = g_tau.  Scratch: bwd_layout (what bwd_B3 reads and writes: oSt, oLam, W at body word 1..6, oQb, oVb)
+// followed by 6 words per accumulator slot for the M lambda pass (B3's slots still hold its own sums when that pass runs).
+// Outputs:  g_q = (dID/dq)^T lambda + K lambda ;  g_qdot = (dID/dqdot)^T lambda + (D + dt K) lambda - M lambda / dt ;  g_v' = M lambda / dt
+NB2_HD int id_bwd_words(int nb, int n, int nslots, int nfree) { return bwd_layout(nb, n, nslots, nfree).total + 6 * nslots; }
+// parent <- child transform of body i from the saved stream (as bwd_B3 forms it)
+template <class R, int ST>
+NB2_HD Xf<R> id_saved_xf(const Nb2ModelDev<R>& M, const R* bt, int i, const R* scr, const BwdLayout& L, const R* sv, size_t B) {
+  const int jt = M.jtype[i];
+  const R* s = sv + (size_t)(i * 21) * B;
+  if (jt == NB2_JT_REV) return xf_rev(M, bt, i, s[19 * B], s[20 * B]);
+  if (jt == NB2_JT_PRIS) return xf_pris(M, bt, i, scr[(size_t)(L.oSt + M.dof_off[i]) * ST]);
+  R t12[12];
+  for (int k = 0; k < 12; k++) t12[k] = sv[(size_t)(M.nb * 21 + M.free_idx[i] * 33 + 21 + k) * B];
+  return ldXf<R, 1>(t12);
+}
+// root -> leaf: the field W_i = X^-1 W_p + S lambda_i that seeds bwd_B3 (it replaces B1 / B2 of the step)
+template <class R, int ST>
+NB2_HD void id_bwd_field(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, int lo, int hi, const R* bt) {
+  const BwdLayout L = bwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
+  for (int i = lo; i < hi; i++) {
+    const int jt = M.jtype[i], p = M.parent[i], o = M.dof_off[i];
+    V6<R> W = (p >= 0) ? AdInvT(id_saved_xf<R, ST>(M, bt, i, scr, L, sv, B), ld6<R, ST>(scr + (size_t)(L.oBody + 7 * p + 1) * ST)) : zero6<R>();
+    if (jt != NB2_JT_FREE) W = W + S_times<R>(jt, scr[(size_t)(L.oLam + o) * ST]);
+    else W = W + ld6<R, ST>(scr + (size_t)(L.oLam + o) * ST);
+    st6<R, ST>(scr + (size_t)(L.oBody + 7 * i + 1) * ST, W);
+  }
+}
+// leaf -> root, after bwd_B3 of the same bodies: M lambda = S^T sum_subtree X* G W, the assembly above, and (gI != nullptr)
+// dL/d(m, h, Ibar) of body i = d(W^T (G A + V x* G V))/d(theta) = t(W, A) - t(ad(V, W), V) in the arithmetic type (gI: fp64 [10*nb][gIB])
+template <class R, int ST>
+NB2_HD void id_bwd_mass(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, int lo, int hi, const R* bt, const double* wi, size_t wiB,
+                        double* gI, size_t gIB) {
+  const BwdLayout L = bwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
+  const int oS = L.total;
+  const R dt = M.dt, rdt = R(1) / M.dt;
+  V6<R> hA = zero6<R>();
+  bool hvalid = false;
+  for (int i = hi - 1; i >= lo; i--) {
+    const int jt = M.jtype[i], p = M.parent[i], o = M.dof_off[i], fl = M.flags[i];
+    R m; V3<R> h; S3<R> Ib; inertia_of(M, bt, wi, wiB, i, &m, &h, &Ib);
+    const V6<R> W = ld6<R, ST>(scr + (size_t)(L.oBody + 7 * i + 1) * ST);
+    V6<R> Ab = mulG(m, h, Ib, W);
+    if (hvalid) Ab = Ab + hA;
+    if (fl & NB2_F_HAS_SLOT)
+      for (int k = 0; k < M.slot_count[i]; k++) Ab = Ab + ld6<R, ST>(scr + (size_t)(oS + 6 * (M.slot_self[i] + k)) * ST);
+    if (gI) {
+      const R* s = sv + (size_t)(i * 21) * B;
+      const V6<R> V = sv_ld6<R>(s, B, 0), A = sv_ld6<R>(s, B, 6);
+      V6<R> Y2;
+      Y2.a = cross_rn(V.a, W.a);
+      Y2.l = cross_rn(V.a, W.l) + cross_rn(V.l, W.a);
+      R t[10], t2[10];
+      inertia_param_form(W, A, t);
+      inertia_param_form(Y2, V, t2);
+      for (int k = 0; k < 10; k++) gI[(size_t)(10 * i + k) * gIB] = (double)(t[k] - t2[k]);
+    }
+    const int nd = (jt == NB2_JT_FREE) ? 6 : 1;
+    for (int k = 0; k < nd; k++) {
+      const int d = o + k;
+      const R ml = ((jt == NB2_JT_FREE) ? comp6(Ab, k) : S_dot(jt, Ab)) * rdt, lam = scr[(size_t)(L.oLam + d) * ST];
+      scr[(size_t)(L.oQb + d) * ST] += M.spring[d] * lam;
+      scr[(size_t)(L.oVb + d) * ST] += (M.damping[d] + dt * M.spring[d]) * lam - ml;
+      scr[(size_t)(L.oGQ + d) * ST] = ml;
+    }
+    hvalid = false;
+    if (p >= 0) {
+      const V6<R> cA = dAdInvT(id_saved_xf<R, ST>(M, bt, i, scr, L, sv, B), Ab);
+      if (fl & NB2_F_HANDOFF) { hA = cA; hvalid = true; }
+      else st6<R, ST>(scr + (size_t)(oS + 6 * M.slot_parent[i]) * ST, cA);
+    }
+  }
+}
+// Stages of the inverse-dynamics backward:
+//   0 group load of [q; qdot] and g_tau | barrier
+//   1 W trunk (lane 0) | barrier      2 W limbs   3 B3 limbs   4 M lambda + assembly limbs | barrier
+//   5 B3 trunk   6 M lambda + assembly trunk (lane 0) | barrier      7 group store of g_state, g_v'
+#define NB2_ID_BWD_STAGES 8
+#define NB2_ID_BWD_SYNC_MASK 0x53u        /* after stages 0, 1, 4, 6 */
+#define NB2_ID_BWD_SYNC_MASK_1LANE 0x41u  /* lanes == 1: after the group load and before the group store */
+template <class R, int ST>
+NB2_HD void id_backward_stage(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, int lane, int stage, const R* bt,
+                              const double* wi, size_t wiB, double* gI, size_t gIB) {
+  const bool trunk = (stage == 1) | (stage == 5) | (stage == 6);
+  if (trunk && lane != 0) return;
+  BwdContactData<ST> cd; cd.active = 0; cd.error = 0; cd.inj_of_body = nullptr;
+  const int nr = trunk ? M.trunk_n : M.limb_n[lane];
+  for (int rr = 0; rr < nr; rr++) {
+    const int r = (stage >= 3) ? nr - 1 - rr : rr;
+    const int lo = trunk ? M.trunk_lo[r] : M.limb_lo[lane][r], hi = trunk ? M.trunk_hi[r] : M.limb_hi[lane][r];
+    if (stage <= 2) id_bwd_field<R, ST>(M, scr, sv, B, lo, hi, bt);
+    else if (stage == 3 || stage == 5) bwd_B3<R, ST, false>(M, scr, nullptr, sv, B, cd, lo, hi, nullptr, bt, B, wi, wiB, nullptr);
+    else id_bwd_mass<R, ST>(M, scr, sv, B, lo, hi, bt, wi, wiB, gI, gIB);
+  }
+}
+template <class R, int ST>
+NB2_HD void id_bwd_load(const Nb2ModelDev<R>& M, R* scr0, const R* st0, const R* gtau0, int nworlds, int tid, int nthr) {
+  const BwdLayout L = bwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
+  id_rows_load<R, ST>(scr0, st0, 2 * M.ndof, M.magic_n2, L.oSt, nworlds, tid, nthr);
+  id_rows_load<R, ST>(scr0, gtau0, M.ndof, M.magic_n, L.oLam, nworlds, tid, nthr);
+}
+template <class R, int ST>
+NB2_HD void id_bwd_store(const Nb2ModelDev<R>& M, const R* scr0, R* gstate0, R* gnext0, int nworlds, int tid, int nthr) {
+  const BwdLayout L = bwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
+  id_rows_store<R, ST>(scr0, gstate0, 2 * M.ndof, M.magic_n2, L.oQb, nworlds, tid, nthr);  // oVb = oQb + n
+  id_rows_store<R, ST>(scr0, gnext0, M.ndof, M.magic_n, L.oGQ, nworlds, tid, nthr);
+}
+
 }  // namespace nb2

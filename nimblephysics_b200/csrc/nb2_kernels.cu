@@ -219,6 +219,62 @@ k_step_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
   }
 }
 
+// ---- inverse dynamics (nb2_inverse_dynamics / _backward): the warp shape of the step kernels (K lanes per world, [word][slot]
+// scratch in shared memory), I/O rows in the arithmetic type R.  Per-world inertia is a run-time pointer test here: it costs these
+// kernels no spill (-Xptxas -v), unlike the step kernels (see k_step_fwd).
+template <class R, int K>
+__global__ void __launch_bounds__(128)
+k_id_fwd(const __grid_constant__ Nb2ModelDev<R> M, int B, const R* __restrict__ state, const R* __restrict__ next_vel, R* __restrict__ tau,
+         R* __restrict__ saved, int words, const double* __restrict__ winertia) {
+  extern __shared__ __align__(16) unsigned char nb2_smem[];
+  constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
+  const int li = threadIdx.x & 31, slot = li / K, lane = li % K;
+  const int g0 = (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * WPW;
+  const int nworlds = min(WPW, B - g0);  // <= 0: idle warp (grid tail)
+  const bool valid = slot < nworlds;
+  const size_t wg = nworlds > 0 ? g0 : 0, w = wg + (valid ? slot : 0);
+  const R* bt = stage_body_table<R, K>(M, reinterpret_cast<R*>(nb2_smem));
+  R* scr0 = reinterpret_cast<R*>(nb2_smem) + body_table_words<K>(M.nb) + (size_t)(threadIdx.x >> 5) * words * ST;
+  R* scr = scr0 + slot;
+  R* sv = saved ? saved + w : nullptr;
+  const double* wi = winertia ? winertia + w : nullptr;
+  constexpr unsigned sync_mask = (K > 1) ? NB2_ID_FWD_SYNC_MASK : NB2_ID_FWD_SYNC_MASK_1LANE;
+#pragma unroll 1
+  for (int sg = 0; sg < NB2_ID_FWD_STAGES; sg++) {
+    if (sg == 0) { if (nworlds > 0) nb2::id_load<R, ST>(M, scr0, state + wg * 2 * M.ndof, next_vel + wg * M.ndof, nworlds, li, 32); }
+    else if (sg == NB2_ID_FWD_STAGES - 1) { if (nworlds > 0) nb2::id_store<R, ST>(M, scr0, tau + wg * M.ndof, nworlds, li, 32); }
+    else if (valid) nb2::id_forward_stage<R, ST>(M, scr, sv, (size_t)B, saved != nullptr, lane, sg, bt, wi, (size_t)B);
+    if ((sync_mask >> sg) & 1u) __syncwarp();
+  }
+}
+
+template <class R, int K>
+__global__ void __launch_bounds__(128)
+k_id_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, const R* __restrict__ state, const R* __restrict__ saved, const R* __restrict__ gtau,
+         R* __restrict__ gstate, R* __restrict__ gnext, double* __restrict__ ginertia, int words, const double* __restrict__ winertia) {
+  extern __shared__ __align__(16) unsigned char nb2_smem[];
+  constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
+  const int li = threadIdx.x & 31, slot = li / K, lane = li % K;
+  const int g0 = (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * WPW;
+  const int nworlds = min(WPW, B - g0);
+  const bool valid = slot < nworlds;
+  const size_t wg = nworlds > 0 ? g0 : 0, w = wg + (valid ? slot : 0);
+  const R* bt = stage_body_table<R, K>(M, reinterpret_cast<R*>(nb2_smem));
+  R* scr0 = reinterpret_cast<R*>(nb2_smem) + body_table_words<K>(M.nb) + (size_t)(threadIdx.x >> 5) * words * ST;
+  R* scr = scr0 + slot;
+  const double* wi = winertia ? winertia + w : nullptr;
+  double* gI = ginertia ? ginertia + w : nullptr;
+  constexpr unsigned sync_mask = (K > 1) ? NB2_ID_BWD_SYNC_MASK : NB2_ID_BWD_SYNC_MASK_1LANE;
+#pragma unroll 1
+  for (int sg = 0; sg < NB2_ID_BWD_STAGES; sg++) {
+    if (sg == 0) { if (nworlds > 0) nb2::id_bwd_load<R, ST>(M, scr0, state + wg * 2 * M.ndof, gtau + wg * M.ndof, nworlds, li, 32); }
+    else if (sg == NB2_ID_BWD_STAGES - 1) {
+      if (nworlds > 0) nb2::id_bwd_store<R, ST>(M, scr0, gstate + wg * 2 * M.ndof, gnext + wg * M.ndof, nworlds, li, 32);
+    } else if (valid) nb2::id_backward_stage<R, ST>(M, scr, saved + w, (size_t)B, lane, sg, bt, wi, (size_t)B, gI, (size_t)B);
+    if ((sync_mask >> sg) & 1u) __syncwarp();
+  }
+}
+
 // ---- fused step kernels of worlds WITH a contact stage (fp64): ONE WARP PER WORLD.
 // Forward: group load -> the three ABA sweeps on the first M.lanes lanes (trunk / limb schedule) -> the warp-cooperative contact /
 // boxed-LCP stage on all 32 lanes (nb2_cw.cuh) -> store.  Everything a world needs — ABA scratch, contact list, LCP matrix and its
@@ -697,10 +753,12 @@ struct LaunchShape { int warps_per_block = 0; int resident_warps = 0; };  // fil
 struct nb2_variant {
   Nb2ModelDev<float> mf;
   Nb2ModelDev<double> md;
-  int fwd_words, bwd_words;
+  int fwd_words, bwd_words, id_bwd_words;
   int depth;                 // bodies on the sequential path of one sweep: |trunk| + longest lane
-  LaunchShape shape[2][2];   // [forward/backward][fp32/fp64]
+  LaunchShape shape[4][2];   // [launch family: LF_*][fp32/fp64]
 };
+// launch families of the contact-free kernels (one LaunchShape each per variant and precision)
+enum { LF_STEP_FWD = 0, LF_STEP_BWD = 1, LF_ID_FWD = 2, LF_ID_BWD = 3 };
 
 struct nb2_model {
   Nb2ModelDev<float> mf;   // the schedule given to nb2_model_create (also what the contact kernels use)
@@ -734,6 +792,7 @@ template <> const Nb2ModelDev<double>& model_of<double>(const nb2_variant& v) { 
 static void init_variant(nb2_variant& v) {
   v.fwd_words = nb2::fwd_layout(v.mf.nb, v.mf.ndof, v.mf.nslots, v.mf.nfree).total;
   v.bwd_words = nb2::bwd_layout(v.mf.nb, v.mf.ndof, v.mf.nslots, v.mf.nfree).total;
+  v.id_bwd_words = nb2::id_bwd_words(v.mf.nb, v.mf.ndof, v.mf.nslots, v.mf.nfree);
   int trunk = 0, longest = 0;
   for (int r = 0; r < v.mf.trunk_n; r++) trunk += v.mf.trunk_hi[r] - v.mf.trunk_lo[r];
   for (int l = 0; l < v.mf.lanes; l++) {
@@ -772,12 +831,15 @@ static int block_warps(int total_warps, int sm_count, const LaunchShape& sh, siz
 }
 
 template <class R, int K>
-static int prepare_k(nb2_variant& v, int dir) {  // dir 0 forward, 1 backward
+static int prepare_k(nb2_variant& v, int dir) {  // dir: LF_*
   constexpr int ST = CoopShape<K>::ST;
   LaunchShape& sh = v.shape[dir][sizeof(R) == 8];
-  // the occupancy query sizes a warp with its scratch AND its input-staging buffer, in both directions
-  const size_t scratch_and_staging = (size_t)(dir ? v.bwd_words : v.fwd_words) * ST * sizeof(R) +
-                                     (dir ? staging_bytes<K>(4 * v.mf.ndof + v.mf.na) : staging_bytes<K>(2 * v.mf.ndof + v.mf.na));
+  // the occupancy query sizes a step warp with its scratch AND its input-staging buffer, in both directions (the inverse-dynamics
+  // kernels stage nothing)
+  const size_t scratch_and_staging =
+      dir == LF_ID_FWD ? (size_t)v.fwd_words * ST * sizeof(R) : dir == LF_ID_BWD ? (size_t)v.id_bwd_words * ST * sizeof(R) :
+      (size_t)(dir ? v.bwd_words : v.fwd_words) * ST * sizeof(R) +
+          (dir ? staging_bytes<K>(4 * v.mf.ndof + v.mf.na) : staging_bytes<K>(2 * v.mf.ndof + v.mf.na));
   const size_t per_block = (size_t)body_table_words<K>(v.mf.nb) * sizeof(R) + 16;
   if (scratch_and_staging + per_block > (size_t)kMaxSmem) {
     g_err = "model needs " + std::to_string(scratch_and_staging) + " B of shared memory per warp (> 227 KB)"; return NB2_ERR_UNSUPPORTED;
@@ -786,9 +848,15 @@ static int prepare_k(nb2_variant& v, int dir) {  // dir 0 forward, 1 backward
   if (dir == 0) {  // the per-world-inertia variant launches with the shape of the shared-table kernel
     if ((rc = allow_max_smem<k_step_fwd<R, K, false>>()) || (rc = allow_max_smem<k_step_fwd<R, K, true>>())) return rc;
     if (!sh.warps_per_block) sh = occupancy_shape(k_step_fwd<R, K, false>, scratch_and_staging, per_block);
-  } else {
+  } else if (dir == LF_STEP_BWD) {
     if ((rc = allow_max_smem<k_step_bwd<R, K, false>>()) || (rc = allow_max_smem<k_step_bwd<R, K, true>>())) return rc;
     if (!sh.warps_per_block) sh = occupancy_shape(k_step_bwd<R, K, false>, scratch_and_staging, per_block);
+  } else if (dir == LF_ID_FWD) {
+    if ((rc = allow_max_smem<k_id_fwd<R, K>>())) return rc;
+    if (!sh.warps_per_block) sh = occupancy_shape(k_id_fwd<R, K>, scratch_and_staging, per_block);
+  } else {
+    if ((rc = allow_max_smem<k_id_bwd<R, K>>())) return rc;
+    if (!sh.warps_per_block) sh = occupancy_shape(k_id_bwd<R, K>, scratch_and_staging, per_block);
   }
   if (!sh.warps_per_block) { g_err = "no launch shape fits this model"; return NB2_ERR_UNSUPPORTED; }
   return NB2_OK;
@@ -890,6 +958,34 @@ static int launch_bwd(nb2_model* m, int B, const float* state, const float* acti
   if (rc) return rc;
   return with_lanes(pv->mf.lanes, [&](auto k) {
     return launch_bwd_k<R, decltype(k)::value>(*pv, m->sm_count, Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia, st, accumulate, wi, gIa);
+  });
+}
+
+// ---- inverse dynamics: the launch family of the step kernels (variant pick, lane schedules, block shape), dir LF_ID_FWD or LF_ID_BWD
+template <class R, int K>
+static int launch_id_k(const nb2_variant& v, int sm_count, int B, int dir, const R* state, const R* next_vel, R* tau, R* saved, const R* gtau,
+                       R* gstate, R* gnext, double* gI, const double* wi, cudaStream_t st) {
+  constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
+  const int words = dir == LF_ID_FWD ? v.fwd_words : v.id_bwd_words;
+  const size_t per_warp = (size_t)words * ST * sizeof(R);
+  const int total_warps = (B + WPW - 1) / WPW;
+  const int warps = block_warps(total_warps, sm_count, v.shape[dir][sizeof(R) == 8], per_warp);
+  const int blocks = (total_warps + warps - 1) / warps;
+  const size_t smem = per_warp * warps + (size_t)body_table_words<K>(v.mf.nb) * sizeof(R);
+  if (dir == LF_ID_FWD) k_id_fwd<R, K><<<blocks, warps * 32, smem, st>>>(model_of<R>(v), B, state, next_vel, tau, saved, words, wi);
+  else k_id_bwd<R, K><<<blocks, warps * 32, smem, st>>>(model_of<R>(v), B, state, saved, gtau, gstate, gnext, gI, words, wi);
+  g_launches++;
+  NB2_CUDA(cudaGetLastError());
+  return NB2_OK;
+}
+template <class R>
+static int launch_id(nb2_model* m, int B, int dir, const R* state, const R* next_vel, R* tau, R* saved, const R* gtau, R* gstate, R* gnext,
+                     double* gI, const double* wi, cudaStream_t st) {
+  nb2_variant* pv = nullptr;
+  int rc = pick_variant<R>(m, B, dir, &pv);
+  if (rc) return rc;
+  return with_lanes(pv->mf.lanes, [&](auto k) {
+    return launch_id_k<R, decltype(k)::value>(*pv, m->sm_count, B, dir, state, next_vel, tau, saved, gtau, gstate, gnext, gI, wi, st);
   });
 }
 
@@ -1400,6 +1496,31 @@ int nb2_lcp_solve_batch(int B, int mcap, int mode, int early_termination, double
   g_launches++;
   NB2_CUDA(cudaGetLastError());
   return NB2_OK;
+}
+int nb2_inverse_dynamics(const nb2_model* cm, int B, const void* state, const void* next_vel, const double* world_inertia, void* tau, void* saved,
+                         int precision, void* stream) {
+  nb2_model* m = const_cast<nb2_model*>(cm);
+  if (!m || B < 0 || !state || !next_vel || !tau) { g_err = "nb2_inverse_dynamics: bad argument"; return NB2_ERR_INVALID; }
+  if (B == 0) return NB2_OK;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    return launch_id<R>(m, B, LF_ID_FWD, (const R*)state, (const R*)next_vel, (R*)tau, (R*)saved, nullptr, nullptr, nullptr, nullptr, world_inertia,
+                        (cudaStream_t)stream);
+  });
+}
+int nb2_inverse_dynamics_backward(const nb2_model* cm, int B, const void* state, const void* next_vel, const double* world_inertia, const void* saved,
+                                  const void* grad_tau, void* grad_state, void* grad_next_vel, double* grad_inertia, int precision, void* stream) {
+  nb2_model* m = const_cast<nb2_model*>(cm);
+  (void)next_vel;  // the saved stream holds the accelerations it implies
+  if (!m || B < 0 || !state || !saved || !grad_tau || !grad_state || !grad_next_vel) {
+    g_err = "nb2_inverse_dynamics_backward: bad argument"; return NB2_ERR_INVALID;
+  }
+  if (B == 0) return NB2_OK;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    return launch_id<R>(m, B, LF_ID_BWD, (const R*)state, nullptr, nullptr, (R*)saved, (const R*)grad_tau, (R*)grad_state, (R*)grad_next_vel,
+                        grad_inertia, world_inertia, (cudaStream_t)stream);
+  });
 }
 int nb2_model_ndof(const nb2_model* m) { return m ? m->mf.ndof : -1; }
 int nb2_model_na(const nb2_model* m) { return m ? m->mf.na : -1; }

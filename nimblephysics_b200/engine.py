@@ -147,6 +147,16 @@ class DeviceModel:
                                                          torch.cuda.current_stream().cuda_stream))
         return acc
 
+    def inverse_dynamics_device(self, B, state_ptr, next_vel_ptr, tau_ptr, saved_ptr, stream, precision=FP32, wi_ptr=None):
+        """Contact-free inverse dynamics (include/nb2.h nb2_inverse_dynamics): rows in the arithmetic type of `precision`."""
+        _cabi.check(_cabi.lib().nb2_inverse_dynamics(self.handle, B, state_ptr, next_vel_ptr, wi_ptr, tau_ptr, saved_ptr, precision, stream))
+
+    def inverse_dynamics_backward_device(self, B, state_ptr, saved_ptr, gtau_ptr, gstate_ptr, gnext_ptr, stream, precision=FP32,
+                                         ginertia_ptr=None, wi_ptr=None):
+        """VJP of inverse_dynamics_device; ginertia_ptr: optional [10*nb, B] float64 buffer receiving dL/d(inertia parameters)."""
+        _cabi.check(_cabi.lib().nb2_inverse_dynamics_backward(self.handle, B, state_ptr, None, wi_ptr, saved_ptr, gtau_ptr, gstate_ptr,
+                                                              gnext_ptr, ginertia_ptr, precision, stream))
+
     def contact_workspace_bytes(self, B):
         return int(_cabi.lib().nb2_contact_workspace_bytes(self.handle, B))
 

@@ -40,6 +40,31 @@ def _inertia_grad(gi, like):
     return gi.t().to(torch.float64).reshape(like.shape).to(device=like.device, dtype=like.dtype)
 
 
+def set_shared_masses(world, mass: torch.Tensor, who: str = "timestep()"):
+    """A 1-D mass vector [getMassDims()] shared by every world of a batch: world.setMasses(mass), which stays set, and the device model
+    that follows it.  The device -> host copy (a sync) is skipped when this very tensor, unchanged since the last call, is already what
+    the world holds."""
+    if mass.dim() != 1 or mass.numel() != world.getMassDims():
+        raise ValueError(f"{who}: mass has shape {tuple(mass.shape)}, expected [{world.getMassDims()}] (= getMassDims(); "
+                         "register parameters with world.tuneMass)")
+    from .world import edit_epoch
+
+    mkey = (mass.data_ptr(), mass._version, tuple(mass.shape), str(mass.device), edit_epoch())
+    if getattr(world, "_mass_key", None) != mkey:
+        world.setMasses(mass.detach().cpu().numpy().astype(np.float64))
+        device_model_for(world)   # setMasses edited the model: the device model follows (inertia refresh)
+        world._mass_key = mkey
+        world._mass_P = None
+    return device_model_for(world)
+
+
+def shared_mass_jacobian(world, dm, dev) -> torch.Tensor:
+    """d(canonical inertia)/d(mass vector) [mass_dims, 10*nb] fp64 on `dev`, cached on the world with the mass key."""
+    if getattr(world, "_mass_P", None) is None or world._mass_P.device != dev:
+        world._mass_P = torch.from_numpy(dm.inertia_param_jacobian(world)).to(dev)
+    return world._mass_P
+
+
 class TimestepLayer(torch.autograd.Function):
     """world_inertia (optional): per-world canonical inertia [B, nb, 10] (modelspec.mass_to_inertia); it replaces the model's table for
     world w only, and its gradient is the kernels' per-world dL/d(inertia).  Exclusive with the 1-D `mass` argument."""
@@ -52,18 +77,7 @@ class TimestepLayer(torch.autograd.Function):
         if mass is not None:
             # reference: world.setMasses(mass) before the step (timestep.py:33-35); the masses stay set afterwards.
             # One mass vector per call: every world of the batch shares the model (the gradient sums over the batch).
-            if mass.dim() != 1 or mass.numel() != world.getMassDims():
-                raise ValueError(f"timestep(): mass has shape {tuple(mass.shape)}, expected [{world.getMassDims()}] (= getMassDims(); "
-                                 "register parameters with world.tuneMass)")
-            # (a device -> host copy, i.e. a sync: skipped when this very tensor, unchanged since the last call, is already what the world holds)
-            from .world import edit_epoch
-
-            mkey = (mass.data_ptr(), mass._version, tuple(mass.shape), str(mass.device), edit_epoch())
-            if getattr(world, "_mass_key", None) != mkey:
-                world.setMasses(mass.detach().cpu().numpy().astype(np.float64))
-                dm = device_model_for(world)   # setMasses edited the model: the device model follows (inertia refresh)
-                world._mass_key = mkey
-                world._mass_P = None
+            dm = set_shared_masses(world, mass)
         n2, na = 2 * dm.ndof, dm.na
         legacy = state.dim() == 1
         if legacy and (state.numel() != n2 or action.numel() != na):
@@ -91,9 +105,7 @@ class TimestepLayer(torch.autograd.Function):
         ctx.wi_like = world_inertia
         ctx.mass_grad = mass is not None and ctx.needs_input_grad[3]
         if ctx.mass_grad:
-            if getattr(world, "_mass_P", None) is None or world._mass_P.device != dev:
-                world._mass_P = torch.from_numpy(dm.inertia_param_jacobian(world)).to(dev)  # [mass_dims, 10*nb], fp64; cached with the mass key
-            ctx.mass_P = world._mass_P
+            ctx.mass_P = shared_mass_jacobian(world, dm, dev)
             ctx.mass_like = mass
         need_grad = any(ctx.needs_input_grad[1:5])
         ctx.contact = dm.has_contacts
@@ -234,14 +246,14 @@ def reset_contact_cache(world):
     world._lcp_cache = None
 
 
-def per_world_inertia(world, state: torch.Tensor, mass: torch.Tensor) -> torch.Tensor:
+def per_world_inertia(world, state: torch.Tensor, mass: torch.Tensor, who: str = "timestep()") -> torch.Tensor:
     """Checks a 2-D mass argument against a batch of states and maps it to the per-world inertia table the kernels read."""
     from .modelspec import mass_to_inertia
 
     if state.dim() != 2:
-        raise ValueError(f"timestep(): a per-world mass [B, getMassDims()] needs a batched state [B, 2n], got state of shape {tuple(state.shape)}")
+        raise ValueError(f"{who}: a per-world mass [B, getMassDims()] needs a batched state [B, 2n], got state of shape {tuple(state.shape)}")
     if mass.shape[0] != state.shape[0]:
-        raise ValueError(f"timestep(): mass has {mass.shape[0]} rows for a batch of {state.shape[0]} worlds")
+        raise ValueError(f"{who}: mass has {mass.shape[0]} rows for a batch of {state.shape[0]} worlds")
     return mass_to_inertia(world, mass)
 
 

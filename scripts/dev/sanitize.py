@@ -1,5 +1,5 @@
 """Small end-to-end run for compute-sanitizer (memcheck): contact-free fwd+bwd (device + pinned-host paths, partial groups),
-contact fwd+bwd, fused rollout."""
+contact fwd+bwd, fused rollout, inverse dynamics fwd+bwd (both precisions, per-world masses, partial groups)."""
 import sys
 import numpy as np, torch
 sys.path.insert(0, ".")
@@ -25,5 +25,14 @@ for name, B in (("half_cheetah", 40), ("atlas_ground", 24)):
     cs, ca = contact_inputs(craw, name, B, seed=3)
     st = torch.tensor(cs, device="cuda", requires_grad=True); at = torch.tensor(ca, device="cuda", requires_grad=True)
     out = nb.timestep(cw, st, at); out.sum().backward()
+for B in (7, 203):
+    s, _, _ = sample_inputs(raw, B, seed=B)
+    for dt in (torch.float32, torch.float64):
+        st = torch.tensor(s, device="cuda", dtype=dt, requires_grad=True)
+        vn = (st.detach()[:, raw.ndof:] + 1e-3).requires_grad_()
+        mass = torch.tensor(np.ones((B, 1)), device="cuda", requires_grad=True)
+        mw = nb.World.from_raw(raw); mw._contacts_disabled = True
+        mw.tuneMass(mw.skeletons[0]._ordered_bodies()[0], 0)
+        nb.inverse_dynamics(mw, st, vn, mass * torch.tensor(mw.getMasses(), device="cuda")).sum().backward()
 torch.cuda.synchronize()
 print("sanitize run finished")

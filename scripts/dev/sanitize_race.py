@@ -1,4 +1,4 @@
-"""Shared-memory hazard check (compute-sanitizer --tool racecheck) of the cooperative-lane step kernels."""
+"""Shared-memory hazard check (compute-sanitizer --tool racecheck) of the cooperative-lane step and inverse-dynamics kernels, every lane schedule."""
 import sys
 import numpy as np, torch
 sys.path.insert(0, ".")
@@ -11,5 +11,12 @@ for name in ("atlas", "half_cheetah"):
         s, a, g = sample_inputs(raw, B, seed=B)
         st = torch.tensor(s, device="cuda", requires_grad=True); at = torch.tensor(a, device="cuda", requires_grad=True)
         nb.timestep(w, st, at).backward(torch.tensor(g, device="cuda"))
+        dm = nb.device_model_for(w)
+        for c in dm.schedules:
+            dm.set_lanes(c.lanes)
+            sr = st.detach().clone().requires_grad_()
+            vn = (sr.detach()[:, raw.ndof:] + 1e-3).requires_grad_()
+            nb.inverse_dynamics(w, sr, vn).sum().backward()
+        dm.set_lanes(0)
 torch.cuda.synchronize()
 print("racecheck run finished")
