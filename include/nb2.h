@@ -220,6 +220,25 @@ int nb2_inverse_dynamics(const nb2_model* m, int B, const void* state, const voi
 int nb2_inverse_dynamics_backward(const nb2_model* m, int B, const void* state, const void* next_vel, const double* world_inertia, const void* saved,
                                   const void* grad_tau, void* grad_state, void* grad_next_vel, double* grad_inertia, int precision, void* stream);
 
+/* Contact inverse dynamics of B worlds with one contact body: tau_ID of nb2_inverse_dynamics split into the contact wrench [B, 6] and the
+ * joint torques tau [B, ndof] that remain:
+ *     tau + J_c(q)^T wrench = tau_ID        on every dof,        tau = 0 on the six dofs of the contact body's free root,
+ * where J_c maps qdot to the spatial velocity [omega; v_origin] of contact_body in world axes about the world origin, and wrench is
+ * [torque; force] in the same axes about the same point.  The root's six tau_ID entries are its joint-frame force F_r (the step's free-joint
+ * convention), so wrench = X*(root -> world) F_r, and tau differs from tau_ID only on the dofs of the joints between contact_body and the
+ * root: tau_j = tau_ID,j - S_j^T F_j with F_j = F_r expressed in frame j.  Every other dof is tau_ID exactly.  The wrench is the same for
+ * every body of the tree.  contact_body: canonical body index (modelspec body_owner); it must lie under a FREE root (NB2_ERR_INVALID
+ * otherwise).  Rows, world_inertia and saved are those of nb2_inverse_dynamics (arithmetic type); tau, wrench: device, one row per world. */
+int nb2_contact_inverse_dynamics(const nb2_model* m, int B, int contact_body, const void* state, const void* next_vel, const double* world_inertia,
+                                 void* tau, void* wrench, void* saved, int precision, void* stream);
+/* Vector-Jacobian product of the same call, with the SAME state, world_inertia, saved stream and the forward's wrench (next_vel is not
+ * read).  grad_tau [B, ndof], grad_wrench [B, 6] -> grad_state, grad_next_vel, grad_inertia as in nb2_inverse_dynamics_backward.  seed:
+ * caller-owned workspace [B, ndof] in the arithmetic type (the g_tau_ID handed to the inverse-dynamics backward); the call allocates nothing. */
+int nb2_contact_inverse_dynamics_backward(const nb2_model* m, int B, int contact_body, const void* state, const void* next_vel,
+                                          const double* world_inertia, const void* saved, const void* wrench, const void* grad_tau,
+                                          const void* grad_wrench, void* seed, void* grad_state, void* grad_next_vel, double* grad_inertia,
+                                          int precision, void* stream);
+
 /* Batched boxed-LCP solves on the device: B independent problems, one warp each — the reference's pointer-style lower boundary
  * BoxedLcpSolver::solve(n, A, x, b, nub, lo, hi, findex, earlyTermination) (dart/constraint/BoxedLcpSolver.hpp:125-135) and the
  * solve chain of BoxedLcpConstraintSolver::solveLcp (BoxedLcpConstraintSolver.cpp:352-789).  Device pointers; problem w has dimension

@@ -1150,4 +1150,96 @@ NB2_HD void id_bwd_store(const Nb2ModelDev<R>& M, const R* scr0, R* gstate0, R* 
   id_rows_store<R, ST>(scr0, gnext0, M.ndof, M.magic_n, L.oGQ, nworlds, tid, nthr);
 }
 
+// =====================================================================================================
+// contact inverse dynamics (DESIGN.md §6f): the inverse-dynamics force tau_ID split into a contact wrench on one body and the joint
+// torques that remain, tau + J_c^T wrench = tau_ID with tau = 0 on the free root of the contact body's tree.  J_c maps qdot to the
+// contact body's spatial velocity in world axes about the world origin, and the wrench is [torque; force] in the same axes.  The free
+// root's six tau_ID entries are its 6-D joint-frame force F_r (id_pass_force writes comp6(f, k)), so wrench = X*(root -> world) F_r and
+// on the chain below the root tau_j = tau_ID,j - S_j^T F_j with F_j = F_r in frame j.  Dofs off the chain keep tau_ID.  One thread walks
+// one world's chain from its own rows (stride 1, the arithmetic type R); the chain is at most one limb deep.
+// =====================================================================================================
+struct CidChain {
+  int n;                            // bodies on the chain
+  int16_t body[NB2_MAX_BODIES];     // the free root first, the contact body last
+};
+// the chain from the free root down to `body`; returns its length, or -1 if `body` is out of range or its tree's root is not FREE
+template <class R> NB2_HD int cid_chain(const Nb2ModelDev<R>& M, int body, CidChain* c) {
+  if (body < 0 || body >= M.nb) return -1;
+  int k = 0;
+  for (int i = body; i >= 0; i = M.parent[i]) k++;
+  c->n = k;
+  for (int i = body; i >= 0; i = M.parent[i]) c->body[--k] = (int16_t)i;
+  return M.jtype[c->body[0]] == NB2_JT_FREE ? c->n : -1;
+}
+// parent <- child transform of body i at the positions q (a state row; the same arithmetic as fwd_pass1)
+template <class R> NB2_HD Xf<R> cid_xf(const Nb2ModelDev<R>& M, int i, const R* q) {
+  const int jt = M.jtype[i], o = M.dof_off[i];
+  if (jt == NB2_JT_REV) { R s, c; nb2_sincos(q[o], &s, &c); return xf_rev(M, i, s, c); }
+  if (jt == NB2_JT_PRIS) return xf_pris(M, i, q[o]);
+  const Xf<R> X = xtree(M, i);
+  Xf<R> T;
+  T.R_ = mul(X.R_, expmap(mk3<R>(q[o], q[o + 1], q[o + 2])));
+  T.p = mul(X.R_, mk3<R>(q[o + 3], q[o + 4], q[o + 5])) + X.p;
+  return T;
+}
+template <class R> NB2_HD V6<R> row6(const R* p) { V6<R> v; v.a = mk3<R>(p[0], p[1], p[2]); v.l = mk3<R>(p[3], p[4], p[5]); return v; }
+template <class R> NB2_HD void put6(R* p, const V6<R>& v) { p[0] = v.a.x; p[1] = v.a.y; p[2] = v.a.z; p[3] = v.l.x; p[4] = v.l.y; p[5] = v.l.z; }
+// the joint's S^T f, subtracted from its tau entries
+template <class R> NB2_HD void cid_sub_joint_force(const Nb2ModelDev<R>& M, int i, const V6<R>& F, R* tau) {
+  const int jt = M.jtype[i], o = M.dof_off[i];
+  if (jt == NB2_JT_FREE) { for (int k = 0; k < 6; k++) tau[o + k] -= comp6(F, k); }
+  else tau[o] -= S_dot(jt, F);
+}
+// dL/dq of a free joint [exp(phi), p] from c, the dual of its body-frame twist: the twist of (d phi, d p) is (Jr(phi) d phi, R^T d p)
+template <class R> NB2_HD void cid_free_q_grad(const R* q, int o, const V6<R>& c, R* gq) {
+  const V3<R> phi = mk3<R>(q[o], q[o + 1], q[o + 2]);
+  const V3<R> ga = mulT(so3_Jr(phi), c.a), gl = mul(expmap(phi), c.l);
+  gq[o] += ga.x; gq[o + 1] += ga.y; gq[o + 2] += ga.z; gq[o + 3] += gl.x; gq[o + 4] += gl.y; gq[o + 5] += gl.z;
+}
+
+// forward: tau holds tau_ID on entry and tau on return (in place); wrench [6]
+template <class R> NB2_HD void cid_forward(const Nb2ModelDev<R>& M, const CidChain& c, const R* q, R* tau, R* wrench) {
+  const int r = c.body[0], o = M.dof_off[r];
+  V6<R> F = row6(tau + o);
+  put6(wrench, dAdInvT(cid_xf(M, r, q), F));
+  for (int k = 0; k < 6; k++) tau[o + k] = R(0);
+  for (int k = 1; k < c.n; k++) {
+    const int i = c.body[k];
+    F = dAdT(cid_xf(M, i, q), F);
+    cid_sub_joint_force(M, i, F, tau);
+  }
+}
+// VJP.  With the chain's forces F_j (F_r recomputed from the forward's wrench) and lambda_j = dL/dF_j, accumulated leaf -> root:
+//   seed (may be nullptr): the g_tau_ID that the inverse-dynamics backward takes: g_tau off the root, and on the root rows
+//     g_F_r = X*(root -> world)^T g_wrench + X*(j <- root)^T sums of -S_j g_tau_j  (the incoming g_tau of the root rows is dropped)
+//   gq (may be nullptr): ADDS the direct q-derivative of the chain and root transforms:  d/dq_j = xi_j . (lambda_j x* F_j) on the chain,
+//     -xi_r . (mu x* F_r) with mu = X*(root -> world)^T g_wrench on the root (xi: the joint's body-frame twist per unit dq)
+template <class R> NB2_HD void cid_vjp(const Nb2ModelDev<R>& M, const CidChain& c, const R* q, const R* wrench, const R* gtau, const R* gw, R* seed,
+                                       R* gq) {
+  const int r = c.body[0];
+  const Xf<R> Tr = cid_xf(M, r, q);
+  const V6<R> Fr = dAdT(Tr, row6(wrench));
+  V6<R> F = Fr, lam = zero6<R>();
+  for (int k = 1; k < c.n; k++) F = dAdT(cid_xf(M, c.body[k], q), F);
+  for (int k = c.n - 1; k >= 1; k--) {
+    const int i = c.body[k], jt = M.jtype[i], o = M.dof_off[i];
+    if (jt == NB2_JT_FREE) lam = lam - row6(gtau + o);
+    else lam = lam - S_times<R>(jt, gtau[o]);
+    if (gq) {
+      const V6<R> cg = crf(lam, F);
+      if (jt == NB2_JT_FREE) cid_free_q_grad(q, o, cg, gq);
+      else gq[o] += S_dot(jt, cg);
+    }
+    const Xf<R> T = cid_xf(M, i, q);
+    F = dAdInvT(T, F);
+    lam = AdT(T, lam);
+  }
+  const V6<R> mu = AdInvT(Tr, row6(gw));
+  if (seed) {
+    for (int d = 0; d < M.ndof; d++) seed[d] = gtau[d];
+    put6(seed + M.dof_off[r], lam + mu);
+  }
+  if (gq) cid_free_q_grad(q, M.dof_off[r], zero6<R>() - crf(mu, Fr), gq);
+}
+
 }  // namespace nb2

@@ -275,6 +275,28 @@ k_id_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, const R* __restrict__ 
   }
 }
 
+// ---- contact inverse dynamics (nb2_contact_inverse_dynamics / _backward): the chain walk that follows (forward) or brackets (backward)
+// the inverse-dynamics kernels.  One thread per world on its own rows, 1-D grid, the last block partial.
+template <class R>
+__global__ void __launch_bounds__(128)
+k_cid_fwd(const __grid_constant__ Nb2ModelDev<R> M, const __grid_constant__ nb2::CidChain c, int B, const R* __restrict__ state,
+          R* __restrict__ tau, R* __restrict__ wrench) {
+  const int w = blockIdx.x * blockDim.x + threadIdx.x;
+  if (w >= B) return;
+  nb2::cid_forward<R>(M, c, state + (size_t)w * 2 * M.ndof, tau + (size_t)w * M.ndof, wrench + (size_t)w * 6);
+}
+// seed != nullptr: write the inverse-dynamics backward's seed; else add the chain's direct q-term to gstate
+template <class R>
+__global__ void __launch_bounds__(128)
+k_cid_bwd(const __grid_constant__ Nb2ModelDev<R> M, const __grid_constant__ nb2::CidChain c, int B, const R* __restrict__ state,
+          const R* __restrict__ wrench, const R* __restrict__ gtau, const R* __restrict__ gwrench, R* __restrict__ seed, R* __restrict__ gstate) {
+  const int w = blockIdx.x * blockDim.x + threadIdx.x;
+  if (w >= B) return;
+  const size_t n = M.ndof;
+  nb2::cid_vjp<R>(M, c, state + w * 2 * n, wrench + (size_t)w * 6, gtau + w * n, gwrench + (size_t)w * 6, seed ? seed + w * n : nullptr,
+                  seed ? nullptr : gstate + w * 2 * n);
+}
+
 // ---- fused step kernels of worlds WITH a contact stage (fp64): ONE WARP PER WORLD.
 // Forward: group load -> the three ABA sweeps on the first M.lanes lanes (trunk / limb schedule) -> the warp-cooperative contact /
 // boxed-LCP stage on all 32 lanes (nb2_cw.cuh) -> store.  Everything a world needs — ABA scratch, contact list, LCP matrix and its
@@ -989,6 +1011,25 @@ static int launch_id(nb2_model* m, int B, int dir, const R* state, const R* next
   });
 }
 
+// ---- contact inverse dynamics: the chain of the contact body, checked (in range, under a free root), and the chain kernels' launch
+static int cid_chain_of(const nb2_model* m, int body, nb2::CidChain* c, const char* who) {
+  if (nb2::cid_chain(m->mf, body, c) < 0) {
+    g_err = std::string(who) + ": contact body " + std::to_string(body) + " is not a canonical body of the model under a free root";
+    return NB2_ERR_INVALID;
+  }
+  return NB2_OK;
+}
+template <class R>
+static int launch_cid(const nb2_model* m, const nb2::CidChain& c, int B, bool fwd, const R* state, R* tau, const R* wrench_in, R* wrench_out,
+                      const R* gtau, const R* gwrench, R* seed, R* gstate, cudaStream_t st) {
+  const int threads = 128, blocks = (B + threads - 1) / threads;
+  if (fwd) k_cid_fwd<R><<<blocks, threads, 0, st>>>(model_of<R>(m->variants[0]), c, B, state, tau, wrench_out);
+  else k_cid_bwd<R><<<blocks, threads, 0, st>>>(model_of<R>(m->variants[0]), c, B, state, wrench_in, gtau, gwrench, seed, gstate);
+  g_launches++;
+  NB2_CUDA(cudaGetLastError());
+  return NB2_OK;
+}
+
 // The host entry points take host buffers.  When every buffer of a call is page-locked memory visible to the device
 // (cudaHostAlloc / cudaHostRegister, e.g. torch pin_memory()), the kernels read and write it DIRECTLY: the group load /
 // store of every warp is a coalesced, deeply pipelined stream over PCIe, so the transfer overlaps the sweeps warp by warp
@@ -1520,6 +1561,45 @@ int nb2_inverse_dynamics_backward(const nb2_model* cm, int B, const void* state,
     using R = decltype(r);
     return launch_id<R>(m, B, LF_ID_BWD, (const R*)state, nullptr, nullptr, (R*)saved, (const R*)grad_tau, (R*)grad_state, (R*)grad_next_vel,
                         grad_inertia, world_inertia, (cudaStream_t)stream);
+  });
+}
+int nb2_contact_inverse_dynamics(const nb2_model* cm, int B, int contact_body, const void* state, const void* next_vel, const double* world_inertia,
+                                 void* tau, void* wrench, void* saved, int precision, void* stream) {
+  nb2_model* m = const_cast<nb2_model*>(cm);
+  if (!m || B < 0 || !state || !next_vel || !tau || !wrench) { g_err = "nb2_contact_inverse_dynamics: bad argument"; return NB2_ERR_INVALID; }
+  nb2::CidChain c;
+  if (int rc = cid_chain_of(m, contact_body, &c, "nb2_contact_inverse_dynamics")) return rc;
+  if (B == 0) return NB2_OK;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc = launch_id<R>(m, B, LF_ID_FWD, (const R*)state, (const R*)next_vel, (R*)tau, (R*)saved, nullptr, nullptr, nullptr, nullptr, world_inertia, st);
+    if (rc) return rc;
+    return launch_cid<R>(m, c, B, true, (const R*)state, (R*)tau, nullptr, (R*)wrench, nullptr, nullptr, nullptr, nullptr, st);
+  });
+}
+int nb2_contact_inverse_dynamics_backward(const nb2_model* cm, int B, int contact_body, const void* state, const void* next_vel,
+                                          const double* world_inertia, const void* saved, const void* wrench, const void* grad_tau,
+                                          const void* grad_wrench, void* seed, void* grad_state, void* grad_next_vel, double* grad_inertia,
+                                          int precision, void* stream) {
+  nb2_model* m = const_cast<nb2_model*>(cm);
+  (void)next_vel;
+  if (!m || B < 0 || !state || !saved || !wrench || !grad_tau || !grad_wrench || !seed || !grad_state || !grad_next_vel) {
+    g_err = "nb2_contact_inverse_dynamics_backward: bad argument"; return NB2_ERR_INVALID;
+  }
+  nb2::CidChain c;
+  if (int rc = cid_chain_of(m, contact_body, &c, "nb2_contact_inverse_dynamics_backward")) return rc;
+  if (B == 0) return NB2_OK;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc = launch_cid<R>(m, c, B, false, (const R*)state, nullptr, (const R*)wrench, nullptr, (const R*)grad_tau, (const R*)grad_wrench, (R*)seed,
+                           nullptr, st);
+    if (!rc) rc = launch_id<R>(m, B, LF_ID_BWD, (const R*)state, nullptr, nullptr, (R*)saved, (const R*)seed, (R*)grad_state, (R*)grad_next_vel,
+                               grad_inertia, world_inertia, st);
+    if (!rc) rc = launch_cid<R>(m, c, B, false, (const R*)state, nullptr, (const R*)wrench, nullptr, (const R*)grad_tau, (const R*)grad_wrench,
+                                nullptr, (R*)grad_state, st);
+    return rc;
   });
 }
 int nb2_model_ndof(const nb2_model* m) { return m ? m->mf.ndof : -1; }

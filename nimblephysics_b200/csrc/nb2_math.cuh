@@ -164,6 +164,12 @@ template <class R> NB2_HD V6<R> AdInvT(const Xf<R>& T, const V6<R>& V) {  // mot
 template <class R> NB2_HD V6<R> dAdInvT(const Xf<R>& T, const V6<R>& F) {  // force: child frame -> parent frame
   V6<R> r; r.l = mul(T.R_, F.l); r.a = mul(T.R_, F.a) + cross(T.p, r.l); return r;
 }
+template <class R> NB2_HD V6<R> AdT(const Xf<R>& T, const V6<R>& V) {  // motion: child frame -> parent frame (inverse of AdInvT)
+  V6<R> r; r.a = mul(T.R_, V.a); r.l = mul(T.R_, V.l) + cross(T.p, r.a); return r;
+}
+template <class R> NB2_HD V6<R> dAdT(const Xf<R>& T, const V6<R>& F) {  // force: parent frame -> child frame (inverse of dAdInvT)
+  V6<R> r; r.l = mulT(T.R_, F.l); r.a = mulT(T.R_, F.a - cross(T.p, F.l)); return r;
+}
 template <class R> NB2_HD V6<R> ad(const V6<R>& X, const V6<R>& Y) {  // motion cross motion (:1470-1483)
   V6<R> r; r.a = cross(X.a, Y.a); r.l = cross(X.a, Y.l) + cross(X.l, Y.a); return r;
 }

@@ -157,6 +157,19 @@ class DeviceModel:
         _cabi.check(_cabi.lib().nb2_inverse_dynamics_backward(self.handle, B, state_ptr, None, wi_ptr, saved_ptr, gtau_ptr, gstate_ptr,
                                                               gnext_ptr, ginertia_ptr, precision, stream))
 
+    def contact_inverse_dynamics_device(self, B, body, state_ptr, next_vel_ptr, tau_ptr, wrench_ptr, saved_ptr, stream, precision=FP32,
+                                        wi_ptr=None):
+        """Contact inverse dynamics (include/nb2.h nb2_contact_inverse_dynamics); body: canonical index of the contact body."""
+        _cabi.check(_cabi.lib().nb2_contact_inverse_dynamics(self.handle, B, body, state_ptr, next_vel_ptr, wi_ptr, tau_ptr, wrench_ptr,
+                                                             saved_ptr, precision, stream))
+
+    def contact_inverse_dynamics_backward_device(self, B, body, state_ptr, saved_ptr, wrench_ptr, gtau_ptr, gwrench_ptr, seed_ptr, gstate_ptr,
+                                                 gnext_ptr, stream, precision=FP32, ginertia_ptr=None, wi_ptr=None):
+        """VJP of contact_inverse_dynamics_device; seed_ptr: caller-owned [B, ndof] workspace in the arithmetic type."""
+        _cabi.check(_cabi.lib().nb2_contact_inverse_dynamics_backward(self.handle, B, body, state_ptr, None, wi_ptr, saved_ptr, wrench_ptr,
+                                                                      gtau_ptr, gwrench_ptr, seed_ptr, gstate_ptr, gnext_ptr, ginertia_ptr,
+                                                                      precision, stream))
+
     def contact_workspace_bytes(self, B):
         return int(_cabi.lib().nb2_contact_workspace_bytes(self.handle, B))
 

@@ -1,5 +1,6 @@
 """Small end-to-end run for compute-sanitizer (memcheck): contact-free fwd+bwd (device + pinned-host paths, partial groups),
-contact fwd+bwd, fused rollout, inverse dynamics fwd+bwd (both precisions, per-world masses, partial groups)."""
+contact fwd+bwd, fused rollout, inverse dynamics and contact inverse dynamics fwd+bwd (both precisions, per-world masses, partial
+groups and partial blocks)."""
 import sys
 import numpy as np, torch
 sys.path.insert(0, ".")
@@ -34,5 +35,7 @@ for B in (7, 203):
         mw = nb.World.from_raw(raw); mw._contacts_disabled = True
         mw.tuneMass(mw.skeletons[0]._ordered_bodies()[0], 0)
         nb.inverse_dynamics(mw, st, vn, mass * torch.tensor(mw.getMasses(), device="cuda")).sum().backward()
+        tau, wr = nb.contact_inverse_dynamics(mw, st, vn, mw.skeletons[0]._ordered_bodies()[27], mass * torch.tensor(mw.getMasses(), device="cuda"))
+        (tau.sum() + wr.sum()).backward()
 torch.cuda.synchronize()
 print("sanitize run finished")
