@@ -239,6 +239,31 @@ int nb2_contact_inverse_dynamics_backward(const nb2_model* m, int B, int contact
                                           const void* grad_wrench, void* seed, void* grad_state, void* grad_next_vel, double* grad_inertia,
                                           int precision, void* stream);
 
+/* Multiple-contact inverse dynamics of B worlds: tau_ID of nb2_inverse_dynamics split over k = ncontact contact bodies of one tree, into
+ * wrenches w_i [B, k, 6] and the joint torques tau [B, ndof] that remain:
+ *     tau + sum_i J_i(q)^T w_i = tau_ID   on every dof,   tau = 0 on the six dofs of the bodies' free root,
+ *     minimise sum_i | Gamma(p_i)^-1 (w_i - g_i) |^2,
+ * J_i and the wrench convention ([torque; force], world axes, about the world origin) as nb2_contact_inverse_dynamics; p_i the world
+ * position of contact point i, Gamma(p) = [[I, [p]x], [0, I]] (a wrench about p -> about the origin), so the deviation is measured as
+ * [torque about p_i; force]; g_i the guesses.  The constraint is sum_i w_i = W (the one-body wrench) and
+ *     lambda = H^-1 (W - sum_j g_j),  w_i = g_i + Gamma_i Gamma_i^T lambda,  H = sum_i Gamma_i Gamma_i^T.
+ * contact_body [k]: canonical body indices (host); contact_point [k][3] (host): each point in its body's canonical frame.  1 <= k <=
+ * NB2_MAX_CONTACT_BODIES; every body in range and under the same FREE root (NB2_ERR_INVALID otherwise).  guess [B, k, 6] or NULL (0).  With
+ * k = 1 the result is nb2_contact_inverse_dynamics's (the guess is not read).  Rows, world_inertia and saved as nb2_inverse_dynamics. */
+#define NB2_MAX_CONTACT_BODIES 4
+int nb2_multiple_contact_inverse_dynamics(const nb2_model* m, int B, int ncontact, const int32_t* contact_body, const double* contact_point,
+                                          const void* state, const void* next_vel, const double* world_inertia, const void* guess, void* tau,
+                                          void* wrenches, void* saved, int precision, void* stream);
+/* Vector-Jacobian product of the same call, with the SAME bodies, points, state, world_inertia, saved stream and guess, and the forward's
+ * wrenches (next_vel is not read).  grad_tau [B, ndof], grad_wrenches [B, k, 6] -> grad_state, grad_next_vel, grad_inertia (may be NULL)
+ * as nb2_inverse_dynamics_backward, and grad_guess [B, k, 6] (may be NULL).  seed: caller-owned workspace [B, ndof] in the arithmetic type;
+ * the call allocates nothing. */
+int nb2_multiple_contact_inverse_dynamics_backward(const nb2_model* m, int B, int ncontact, const int32_t* contact_body, const double* contact_point,
+                                                   const void* state, const void* next_vel, const double* world_inertia, const void* saved,
+                                                   const void* wrenches, const void* guess, const void* grad_tau, const void* grad_wrenches,
+                                                   void* seed, void* grad_state, void* grad_next_vel, double* grad_inertia, void* grad_guess,
+                                                   int precision, void* stream);
+
 /* Batched boxed-LCP solves on the device: B independent problems, one warp each — the reference's pointer-style lower boundary
  * BoxedLcpSolver::solve(n, A, x, b, nub, lo, hi, findex, earlyTermination) (dart/constraint/BoxedLcpSolver.hpp:125-135) and the
  * solve chain of BoxedLcpConstraintSolver::solveLcp (BoxedLcpConstraintSolver.cpp:352-789).  Device pointers; problem w has dimension

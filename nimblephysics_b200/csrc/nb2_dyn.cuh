@@ -18,6 +18,7 @@
 
 #include "nb2_math.cuh"
 #include "nb2_model.h"
+#include "../../include/nb2.h"  // NB2_MAX_CONTACT_BODIES
 
 namespace nb2 {
 
@@ -1197,28 +1198,31 @@ template <class R> NB2_HD void cid_free_q_grad(const R* q, int o, const V6<R>& c
   gq[o] += ga.x; gq[o + 1] += ga.y; gq[o + 2] += ga.z; gq[o + 3] += gl.x; gq[o + 4] += gl.y; gq[o + 5] += gl.z;
 }
 
-// forward: tau holds tau_ID on entry and tau on return (in place); wrench [6]
-template <class R> NB2_HD void cid_forward(const Nb2ModelDev<R>& M, const CidChain& c, const R* q, R* tau, R* wrench) {
-  const int r = c.body[0], o = M.dof_off[r];
-  V6<R> F = row6(tau + o);
-  put6(wrench, dAdInvT(cid_xf(M, r, q), F));
-  for (int k = 0; k < 6; k++) tau[o + k] = R(0);
+// the chain walk below the root: F (root frame) carried down, F_j = X*(p -> j) F_p, and op(j, F_j) on every joint below the root
+template <class R, class Op> NB2_HD void cid_walk(const Nb2ModelDev<R>& M, const CidChain& c, const R* q, V6<R> F, Op op) {
   for (int k = 1; k < c.n; k++) {
     const int i = c.body[k];
     F = dAdT(cid_xf(M, i, q), F);
-    cid_sub_joint_force(M, i, F, tau);
+    op(i, F);
   }
 }
-// VJP.  With the chain's forces F_j (F_r recomputed from the forward's wrench) and lambda_j = dL/dF_j, accumulated leaf -> root:
-//   seed (may be nullptr): the g_tau_ID that the inverse-dynamics backward takes: g_tau off the root, and on the root rows
-//     g_F_r = X*(root -> world)^T g_wrench + X*(j <- root)^T sums of -S_j g_tau_j  (the incoming g_tau of the root rows is dropped)
-//   gq (may be nullptr): ADDS the direct q-derivative of the chain and root transforms:  d/dq_j = xi_j . (lambda_j x* F_j) on the chain,
-//     -xi_r . (mu x* F_r) with mu = X*(root -> world)^T g_wrench on the root (xi: the joint's body-frame twist per unit dq)
-template <class R> NB2_HD void cid_vjp(const Nb2ModelDev<R>& M, const CidChain& c, const R* q, const R* wrench, const R* gtau, const R* gw, R* seed,
-                                       R* gq) {
-  const int r = c.body[0];
-  const Xf<R> Tr = cid_xf(M, r, q);
-  const V6<R> Fr = dAdT(Tr, row6(wrench));
+// tau_j -= S_j^T F_j down the chain, F_r the root-frame force
+template <class R> NB2_HD void cid_walk_tau(const Nb2ModelDev<R>& M, const CidChain& c, const R* q, const V6<R>& Fr, R* tau) {
+  cid_walk(M, c, q, Fr, [&](int i, const V6<R>& F) { cid_sub_joint_force(M, i, F, tau); });
+}
+
+// forward: tau holds tau_ID on entry and tau on return (in place); wrench [6]
+template <class R> NB2_HD void cid_forward(const Nb2ModelDev<R>& M, const CidChain& c, const R* q, R* tau, R* wrench) {
+  const int r = c.body[0], o = M.dof_off[r];
+  const V6<R> F = row6(tau + o);
+  put6(wrench, dAdInvT(cid_xf(M, r, q), F));
+  for (int k = 0; k < 6; k++) tau[o + k] = R(0);
+  cid_walk_tau(M, c, q, F, tau);
+}
+// the chain loop of the VJP: with the chain's forces F_j (from the root-frame force Fr) and lambda_j = dL/dF_j of the rows
+// tau_j -= S_j^T F_j, accumulated leaf -> root; returns lambda at the root (dL/dFr).  gq (may be nullptr): ADDS the direct q-derivative
+// of the chain's transforms, xi_j . (lambda_j x* F_j) on every joint below the root
+template <class R> NB2_HD V6<R> cid_chain_vjp(const Nb2ModelDev<R>& M, const CidChain& c, const R* q, const V6<R>& Fr, const R* gtau, R* gq) {
   V6<R> F = Fr, lam = zero6<R>();
   for (int k = 1; k < c.n; k++) F = dAdT(cid_xf(M, c.body[k], q), F);
   for (int k = c.n - 1; k >= 1; k--) {
@@ -1234,12 +1238,170 @@ template <class R> NB2_HD void cid_vjp(const Nb2ModelDev<R>& M, const CidChain& 
     F = dAdInvT(T, F);
     lam = AdT(T, lam);
   }
+  return lam;
+}
+// VJP.  With the chain's forces F_j (F_r recomputed from the forward's wrench) and lambda_j = dL/dF_j, accumulated leaf -> root:
+//   seed (may be nullptr): the g_tau_ID that the inverse-dynamics backward takes: g_tau off the root, and on the root rows
+//     g_F_r = X*(root -> world)^T g_wrench + X*(j <- root)^T sums of -S_j g_tau_j  (the incoming g_tau of the root rows is dropped)
+//   gq (may be nullptr): ADDS the direct q-derivative of the chain and root transforms:  d/dq_j = xi_j . (lambda_j x* F_j) on the chain,
+//     -xi_r . (mu x* F_r) with mu = X*(root -> world)^T g_wrench on the root (xi: the joint's body-frame twist per unit dq)
+template <class R> NB2_HD void cid_vjp(const Nb2ModelDev<R>& M, const CidChain& c, const R* q, const R* wrench, const R* gtau, const R* gw, R* seed,
+                                       R* gq) {
+  const int r = c.body[0];
+  const Xf<R> Tr = cid_xf(M, r, q);
+  const V6<R> Fr = dAdT(Tr, row6(wrench));
+  const V6<R> lam = cid_chain_vjp(M, c, q, Fr, gtau, gq);
   const V6<R> mu = AdInvT(Tr, row6(gw));
   if (seed) {
     for (int d = 0; d < M.ndof; d++) seed[d] = gtau[d];
     put6(seed + M.dof_off[r], lam + mu);
   }
   if (gq) cid_free_q_grad(q, M.dof_off[r], zero6<R>() - crf(mu, Fr), gq);
+}
+
+// =====================================================================================================
+// multiple-contact inverse dynamics (DESIGN.md §6g): tau_ID split into wrenches w_1..w_k on k bodies of one free-rooted tree and the joint
+// torques that remain, tau + sum_i J_i^T w_i = tau_ID with tau = 0 on the root, the w_i as close as possible to guesses g_i:
+//   minimise sum_i |Gamma(p_i)^-1 (w_i - g_i)|^2   subject to   sum_i w_i = W   (W: the §6f wrench),
+// p_i the world position of body i's own origin, Gamma(p) = [[I, [p]x], [0, I]] (a wrench about p -> the same wrench about the origin).
+// With H = sum_i Gamma_i Gamma_i^T:  lambda = H^-1 (W - sum_j g_j),  w_i = g_i + Gamma_i Gamma_i^T lambda.  The system is solved about the
+// mean point pbar (d_i = p_i - pbar, Gbar = Gamma(pbar)): H = Gbar Hd Gbar^T with Hd = diag(S, k I), S = k I + sum_i (|d_i|^2 I - d_i d_i^T),
+// one 3x3 SPD solve (S >= k I) whose conditioning does not depend on how far the tree is from the origin.  Each w_i then walks its
+// body's chain as in §6f, from the root-frame force X*(world -> root) w_i; chains that share bodies add.
+// =====================================================================================================
+template <class R> struct McidBodies {
+  int k;                                  // contact bodies, 1..NB2_MAX_CONTACT_BODIES (the entry points hand k = 1 to §6f)
+  CidChain c[NB2_MAX_CONTACT_BODIES];     // from the shared free root down to the body's canonical owner
+  R r[NB2_MAX_CONTACT_BODIES][3];         // the body's own origin in its owner's canonical frame
+};
+// the k chains and points; returns k, or -1 if k is out of range, a body is out of range or not under a FREE root, or the bodies lie
+// under different roots
+template <class RM, class R> NB2_HD int mcid_bodies(const Nb2ModelDev<RM>& M, int k, const int32_t* body, const double* point, McidBodies<R>* b) {
+  if (k < 1 || k > NB2_MAX_CONTACT_BODIES) return -1;
+  b->k = k;
+  for (int i = 0; i < k; i++) {
+    if (cid_chain(M, body[i], &b->c[i]) < 0 || b->c[i].body[0] != b->c[0].body[0]) return -1;
+    for (int a = 0; a < 3; a++) b->r[i][a] = R(point[3 * i + a]);
+  }
+  return k;
+}
+// Gamma(p) w, Gamma(p)^-1 w (wrenches) and Gamma(p)^T m (a motion vector about the origin -> about p)
+template <class R> NB2_HD V6<R> gam(const V3<R>& p, const V6<R>& w) { V6<R> r; r.a = w.a + cross(p, w.l); r.l = w.l; return r; }
+template <class R> NB2_HD V6<R> gam_inv(const V3<R>& p, const V6<R>& w) { V6<R> r; r.a = w.a - cross(p, w.l); r.l = w.l; return r; }
+template <class R> NB2_HD V6<R> gam_T(const V3<R>& p, const V6<R>& m) { V6<R> r; r.a = m.a; r.l = m.l - cross(p, m.a); return r; }
+
+template <class R> struct McidSys {
+  V3<R> pbar, d[NB2_MAX_CONTACT_BODIES];  // the mean point and p_i - pbar
+  S3<R> Si;                               // S^-1
+  R rk;                                   // 1 / k
+};
+// world position of body i's origin: its owner's chain transforms applied to r_i
+template <class R> NB2_HD V3<R> mcid_point(const Nb2ModelDev<R>& M, const McidBodies<R>& b, int i, const R* q) {
+  V3<R> p = mk3<R>(b.r[i][0], b.r[i][1], b.r[i][2]);
+  for (int k = b.c[i].n - 1; k >= 0; k--) {
+    const Xf<R> T = cid_xf(M, b.c[i].body[k], q);
+    p = mul(T.R_, p) + T.p;
+  }
+  return p;
+}
+template <class R> NB2_HD McidSys<R> mcid_system(const Nb2ModelDev<R>& M, const McidBodies<R>& b, const R* q) {
+  McidSys<R> s;
+  s.pbar = zero3<R>();
+  for (int i = 0; i < b.k; i++) { s.d[i] = mcid_point(M, b, i, q); s.pbar = s.pbar + s.d[i]; }
+  s.rk = R(1) / R(b.k);
+  s.pbar = s.pbar * s.rk;
+  S3<R> S;
+  S.xx = S.yy = S.zz = R(b.k);
+  S.xy = S.xz = S.yz = R(0);
+  for (int i = 0; i < b.k; i++) {
+    const V3<R> d = s.d[i] - s.pbar;
+    const R dd = dot(d, d);
+    s.d[i] = d;
+    S.xx += dd - d.x * d.x; S.yy += dd - d.y * d.y; S.zz += dd - d.z * d.z;
+    S.xy -= d.x * d.y; S.xz -= d.x * d.z; S.yz -= d.y * d.z;
+  }
+  S3<R> A;  // adjugate; det(S) >= k^3
+  A.xx = S.yy * S.zz - S.yz * S.yz; A.yy = S.xx * S.zz - S.xz * S.xz; A.zz = S.xx * S.yy - S.xy * S.xy;
+  A.xy = S.xz * S.yz - S.xy * S.zz; A.xz = S.xy * S.yz - S.xz * S.yy; A.yz = S.xy * S.xz - S.xx * S.yz;
+  const R id = R(1) / (S.xx * A.xx + S.xy * A.xy + S.xz * A.xz);
+  A.xx *= id; A.yy *= id; A.zz *= id; A.xy *= id; A.xz *= id; A.yz *= id;
+  s.Si = A;
+  return s;
+}
+// Hd^-1 x for a wrench x about pbar
+template <class R> NB2_HD V6<R> mcid_hd_solve(const McidSys<R>& s, const V6<R>& x) { V6<R> l; l.a = mul(s.Si, x.a); l.l = x.l * s.rk; return l; }
+// lambda' = Gbar^T lambda = Hd^-1 Gbar^-1 (sum_i w_i - sum_i g_i): in the forward sum_i w_i is W; the backward recomputes it from the
+// forward's wrenches.  Gamma_i^T lambda = Gamma(d_i)^T lambda'.
+template <class R> NB2_HD V6<R> mcid_lambda(const McidBodies<R>& b, const McidSys<R>& s, V6<R> x, const R* guess) {
+  if (guess) for (int i = 0; i < b.k; i++) x = x - row6(guess + 6 * i);
+  return mcid_hd_solve(s, gam_inv(s.pbar, x));
+}
+
+// forward: tau holds tau_ID on entry and tau on return (in place); guess [k][6] (may be nullptr: 0); wrench [k][6]
+template <class R> NB2_HD void mcid_forward(const Nb2ModelDev<R>& M, const McidBodies<R>& b, const R* q, const R* guess, R* tau, R* wrench) {
+  const int r = b.c[0].body[0], o = M.dof_off[r];
+  const Xf<R> Tr = cid_xf(M, r, q);
+  const McidSys<R> s = mcid_system(M, b, q);
+  const V6<R> lam = mcid_lambda(b, s, dAdInvT(Tr, row6(tau + o)), guess);
+  for (int k = 0; k < 6; k++) tau[o + k] = R(0);
+  for (int i = 0; i < b.k; i++) {
+    V6<R> w = gam(s.pbar + s.d[i], gam_T(s.d[i], lam));
+    if (guess) w = w + row6(guess + 6 * i);
+    put6(wrench + 6 * i, w);
+    cid_walk_tau(M, b.c[i], q, dAdT(Tr, w), tau);
+  }
+}
+// VJP, from q, the forward's wrenches and the guesses (p_i, H and lambda recomputed).  With F_i = X*(world -> root) w_i and l_i = dL/dF_i
+// of body i's chain rows (cid_chain_vjp), wbar_i = g_w_i + X*(world -> root)^T l_i, and then
+//   lbar = sum_i Gamma_i Gamma_i^T wbar_i,  E = H^-1 lbar,  dL/dg_i = wbar_i - E,  dL/dW = E,  dL/dp_i = y_i x u_i.a + z_i x lambda.a
+// (u_i = wbar_i - E, y_i / z_i: the linear parts of Gamma_i^T lambda / Gamma_i^T u_i).
+//   seed (may be nullptr): the g_tau_ID of the inverse-dynamics backward: g_tau off the root, mu = X*(root -> world)^T E on the root rows
+//   gguess (may be nullptr, written with seed): dL/dg_i [k][6]
+//   gq (may be nullptr): ADDS the direct q-derivative: the chains' transforms (cid_chain_vjp), the root transform in W (-mu x* F_r) and in
+//     every F_i (l_i x* F_i), and the points p_i through J_i^T [p_i x dL/dp_i; dL/dp_i], free joints through Jr(phi)
+template <class R> NB2_HD void mcid_vjp(const Nb2ModelDev<R>& M, const McidBodies<R>& b, const R* q, const R* wrench, const R* guess, const R* gtau,
+                                        const R* gw, R* seed, R* gguess, R* gq) {
+  const int r = b.c[0].body[0], o = M.dof_off[r];
+  const Xf<R> Tr = cid_xf(M, r, q);
+  const McidSys<R> s = mcid_system(M, b, q);
+  V6<R> W = zero6<R>(), lbar = zero6<R>(), cr = zero6<R>();
+  V6<R> wb[NB2_MAX_CONTACT_BODIES];
+  for (int i = 0; i < b.k; i++) {
+    const V6<R> F = dAdT(Tr, row6(wrench + 6 * i));
+    const V6<R> l = cid_chain_vjp(M, b.c[i], q, F, gtau, gq);
+    if (gq) cr = cr + crf(l, F);
+    W = W + row6(wrench + 6 * i);
+    wb[i] = row6(gw + 6 * i) + AdT(Tr, l);
+    lbar = lbar + gam(s.d[i], gam_T(s.pbar + s.d[i], wb[i]));  // Gbar^-1 lbar
+  }
+  const V6<R> Eb = mcid_hd_solve(s, lbar);  // Gbar^T E
+  const V6<R> E = gam_T(zero3<R>() - s.pbar, Eb);
+  const V6<R> mu = AdInvT(Tr, E);
+  if (seed) {
+    for (int d = 0; d < M.ndof; d++) seed[d] = gtau[d];
+    put6(seed + o, mu);
+    if (gguess) for (int i = 0; i < b.k; i++) put6(gguess + 6 * i, wb[i] - E);
+  }
+  if (!gq) return;
+  const V6<R> lam = mcid_lambda(b, s, W, guess);
+  cr = cr - crf(mu, dAdT(Tr, W));
+  for (int i = 0; i < b.k; i++) {
+    const V3<R> p = s.pbar + s.d[i];
+    const V6<R> u = wb[i] - E;
+    const V3<R> z = (gam_T(p, wb[i]) - gam_T(s.d[i], Eb)).l;  // Gamma_i^T u_i
+    const V3<R> gp = cross(gam_T(s.d[i], lam).l, u.a) + cross(z, lam.a);
+    V6<R> f;
+    f.l = gp;
+    f.a = cross(p, gp);
+    const V6<R> fr = dAdT(Tr, f);
+    cr = cr + fr;
+    cid_walk(M, b.c[i], q, fr, [&](int j, const V6<R>& Fj) {
+      const int jt = M.jtype[j], oj = M.dof_off[j];
+      if (jt == NB2_JT_FREE) cid_free_q_grad(q, oj, Fj, gq);
+      else gq[oj] += S_dot(jt, Fj);
+    });
+  }
+  cid_free_q_grad(q, o, cr, gq);
 }
 
 }  // namespace nb2

@@ -297,6 +297,29 @@ k_cid_bwd(const __grid_constant__ Nb2ModelDev<R> M, const __grid_constant__ nb2:
                   seed ? nullptr : gstate + w * 2 * n);
 }
 
+// ---- multiple-contact inverse dynamics (nb2_multiple_contact_inverse_dynamics / _backward): the k chains' walk, placed as k_cid_*.
+template <class R>
+__global__ void __launch_bounds__(128)
+k_mcid_fwd(const __grid_constant__ Nb2ModelDev<R> M, const __grid_constant__ nb2::McidBodies<R> b, int B, const R* __restrict__ state,
+           const R* __restrict__ guess, R* __restrict__ tau, R* __restrict__ wrench) {
+  const int w = blockIdx.x * blockDim.x + threadIdx.x;
+  if (w >= B) return;
+  const size_t kw = (size_t)w * 6 * b.k;
+  nb2::mcid_forward<R>(M, b, state + (size_t)w * 2 * M.ndof, guess ? guess + kw : nullptr, tau + (size_t)w * M.ndof, wrench + kw);
+}
+// seed != nullptr: write the inverse-dynamics backward's seed and the guess gradient (gguess may be nullptr); else add the direct q-term
+template <class R>
+__global__ void __launch_bounds__(128)
+k_mcid_bwd(const __grid_constant__ Nb2ModelDev<R> M, const __grid_constant__ nb2::McidBodies<R> b, int B, const R* __restrict__ state,
+           const R* __restrict__ wrench, const R* __restrict__ guess, const R* __restrict__ gtau, const R* __restrict__ gwrench,
+           R* __restrict__ seed, R* __restrict__ gguess, R* __restrict__ gstate) {
+  const int w = blockIdx.x * blockDim.x + threadIdx.x;
+  if (w >= B) return;
+  const size_t n = M.ndof, kw = (size_t)w * 6 * b.k;
+  nb2::mcid_vjp<R>(M, b, state + w * 2 * n, wrench + kw, guess ? guess + kw : nullptr, gtau + w * n, gwrench + kw, seed ? seed + w * n : nullptr,
+                   seed && gguess ? gguess + kw : nullptr, seed ? nullptr : gstate + w * 2 * n);
+}
+
 // ---- fused step kernels of worlds WITH a contact stage (fp64): ONE WARP PER WORLD.
 // Forward: group load -> the three ABA sweeps on the first M.lanes lanes (trunk / limb schedule) -> the warp-cooperative contact /
 // boxed-LCP stage on all 32 lanes (nb2_cw.cuh) -> store.  Everything a world needs — ABA scratch, contact list, LCP matrix and its
@@ -1030,6 +1053,31 @@ static int launch_cid(const nb2_model* m, const nb2::CidChain& c, int B, bool fw
   return NB2_OK;
 }
 
+// ---- multiple-contact inverse dynamics: the k chains and points, checked (1 <= k <= NB2_MAX_CONTACT_BODIES, bodies in range under one free
+// root), and the chain kernels' launch
+template <class R>
+static int mcid_bodies_of(const nb2_model* m, int k, const int32_t* body, const double* point, nb2::McidBodies<R>* b, const char* who) {
+  if (k < 1 || k > NB2_MAX_CONTACT_BODIES) {
+    g_err = std::string(who) + ": " + std::to_string(k) + " contact bodies, expected 1.." + std::to_string(NB2_MAX_CONTACT_BODIES);
+    return NB2_ERR_INVALID;
+  }
+  if (nb2::mcid_bodies(m->mf, k, body, point, b) < 0) {
+    g_err = std::string(who) + ": the contact bodies are not canonical bodies of the model under one free root";
+    return NB2_ERR_INVALID;
+  }
+  return NB2_OK;
+}
+template <class R>
+static int launch_mcid(const nb2_model* m, const nb2::McidBodies<R>& b, int B, bool fwd, const R* state, const R* guess, R* tau,
+                       const R* wrench_in, R* wrench_out, const R* gtau, const R* gwrench, R* seed, R* gguess, R* gstate, cudaStream_t st) {
+  const int threads = 128, blocks = (B + threads - 1) / threads;
+  if (fwd) k_mcid_fwd<R><<<blocks, threads, 0, st>>>(model_of<R>(m->variants[0]), b, B, state, guess, tau, wrench_out);
+  else k_mcid_bwd<R><<<blocks, threads, 0, st>>>(model_of<R>(m->variants[0]), b, B, state, wrench_in, guess, gtau, gwrench, seed, gguess, gstate);
+  g_launches++;
+  NB2_CUDA(cudaGetLastError());
+  return NB2_OK;
+}
+
 // The host entry points take host buffers.  When every buffer of a call is page-locked memory visible to the device
 // (cudaHostAlloc / cudaHostRegister, e.g. torch pin_memory()), the kernels read and write it DIRECTLY: the group load /
 // store of every warp is a coalesced, deeply pipelined stream over PCIe, so the transfer overlaps the sweeps warp by warp
@@ -1600,6 +1648,58 @@ int nb2_contact_inverse_dynamics_backward(const nb2_model* cm, int B, int contac
     if (!rc) rc = launch_cid<R>(m, c, B, false, (const R*)state, nullptr, (const R*)wrench, nullptr, (const R*)grad_tau, (const R*)grad_wrench,
                                 nullptr, (R*)grad_state, st);
     return rc;
+  });
+}
+// One contact body is §6f exactly (w_1 = W whatever the guess, dL/dg_1 = 0): the §6f kernels run and the solve is skipped.
+int nb2_multiple_contact_inverse_dynamics(const nb2_model* cm, int B, int ncontact, const int32_t* contact_body, const double* contact_point,
+                                          const void* state, const void* next_vel, const double* world_inertia, const void* guess, void* tau,
+                                          void* wrenches, void* saved, int precision, void* stream) {
+  static const char* who = "nb2_multiple_contact_inverse_dynamics";
+  nb2_model* m = const_cast<nb2_model*>(cm);
+  if (!m || B < 0 || !contact_body || !contact_point || !state || !next_vel || !tau || !wrenches) { g_err = std::string(who) + ": bad argument"; return NB2_ERR_INVALID; }
+  return with_precision(precision, [&](auto r) -> int {
+    using R = decltype(r);
+    nb2::McidBodies<R> b;
+    if (int rc = mcid_bodies_of(m, ncontact, contact_body, contact_point, &b, who)) return rc;
+    if (B == 0) return NB2_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc = launch_id<R>(m, B, LF_ID_FWD, (const R*)state, (const R*)next_vel, (R*)tau, (R*)saved, nullptr, nullptr, nullptr, nullptr, world_inertia, st);
+    if (rc) return rc;
+    if (b.k == 1) return launch_cid<R>(m, b.c[0], B, true, (const R*)state, (R*)tau, nullptr, (R*)wrenches, nullptr, nullptr, nullptr, nullptr, st);
+    return launch_mcid<R>(m, b, B, true, (const R*)state, (const R*)guess, (R*)tau, nullptr, (R*)wrenches, nullptr, nullptr, nullptr, nullptr, nullptr, st);
+  });
+}
+int nb2_multiple_contact_inverse_dynamics_backward(const nb2_model* cm, int B, int ncontact, const int32_t* contact_body, const double* contact_point,
+                                                   const void* state, const void* next_vel, const double* world_inertia, const void* saved,
+                                                   const void* wrenches, const void* guess, const void* grad_tau, const void* grad_wrenches,
+                                                   void* seed, void* grad_state, void* grad_next_vel, double* grad_inertia, void* grad_guess,
+                                                   int precision, void* stream) {
+  static const char* who = "nb2_multiple_contact_inverse_dynamics_backward";
+  nb2_model* m = const_cast<nb2_model*>(cm);
+  (void)next_vel;
+  if (!m || B < 0 || !contact_body || !contact_point || !state || !saved || !wrenches || !grad_tau || !grad_wrenches || !seed || !grad_state ||
+      !grad_next_vel) {
+    g_err = std::string(who) + ": bad argument"; return NB2_ERR_INVALID;
+  }
+  return with_precision(precision, [&](auto r) -> int {
+    using R = decltype(r);
+    nb2::McidBodies<R> b;
+    if (int rc = mcid_bodies_of(m, ncontact, contact_body, contact_point, &b, who)) return rc;
+    if (B == 0) return NB2_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    const R *S = (const R*)state, *Wr = (const R*)wrenches, *G = (const R*)guess, *Gt = (const R*)grad_tau, *Gw = (const R*)grad_wrenches;
+    int rc;
+    if (b.k == 1) {
+      rc = launch_cid<R>(m, b.c[0], B, false, S, nullptr, Wr, nullptr, Gt, Gw, (R*)seed, nullptr, st);
+      if (!rc && grad_guess) NB2_CUDA(cudaMemsetAsync(grad_guess, 0, (size_t)B * 6 * sizeof(R), st));
+    } else {
+      rc = launch_mcid<R>(m, b, B, false, S, G, nullptr, Wr, nullptr, Gt, Gw, (R*)seed, (R*)grad_guess, nullptr, st);
+    }
+    if (!rc) rc = launch_id<R>(m, B, LF_ID_BWD, S, nullptr, nullptr, (R*)saved, (const R*)seed, (R*)grad_state, (R*)grad_next_vel, grad_inertia,
+                               world_inertia, st);
+    if (rc) return rc;
+    if (b.k == 1) return launch_cid<R>(m, b.c[0], B, false, S, nullptr, Wr, nullptr, Gt, Gw, nullptr, (R*)grad_state, st);
+    return launch_mcid<R>(m, b, B, false, S, G, nullptr, Wr, nullptr, Gt, Gw, nullptr, nullptr, (R*)grad_state, st);
   });
 }
 int nb2_model_ndof(const nb2_model* m) { return m ? m->mf.ndof : -1; }

@@ -170,6 +170,31 @@ class DeviceModel:
                                                                       gtau_ptr, gwrench_ptr, seed_ptr, gstate_ptr, gnext_ptr, ginertia_ptr,
                                                                       precision, stream))
 
+    @staticmethod
+    def _contact_set(bodies, points):
+        b = np.ascontiguousarray(bodies, np.int32).reshape(-1)
+        p = np.ascontiguousarray(points, np.float64).reshape(len(b), 3)
+        return len(b), b, p
+
+    def multiple_contact_inverse_dynamics_device(self, B, bodies, points, state_ptr, next_vel_ptr, guess_ptr, tau_ptr, wrench_ptr, saved_ptr,
+                                                 stream, precision=FP32, wi_ptr=None):
+        """Multiple-contact inverse dynamics (include/nb2.h nb2_multiple_contact_inverse_dynamics); bodies [k]: canonical indices, points
+        [k, 3]: each body's own origin in its canonical frame; guess_ptr: [B, k, 6] or None; wrench_ptr: [B, k, 6]."""
+        k, b, p = self._contact_set(bodies, points)
+        _cabi.check(_cabi.lib().nb2_multiple_contact_inverse_dynamics(self.handle, B, k, b.ctypes.data, p.ctypes.data, state_ptr, next_vel_ptr,
+                                                                      wi_ptr, guess_ptr, tau_ptr, wrench_ptr, saved_ptr, precision, stream))
+
+    def multiple_contact_inverse_dynamics_backward_device(self, B, bodies, points, state_ptr, saved_ptr, wrench_ptr, guess_ptr, gtau_ptr,
+                                                          gwrench_ptr, seed_ptr, gstate_ptr, gnext_ptr, stream, precision=FP32, ginertia_ptr=None,
+                                                          gguess_ptr=None, wi_ptr=None):
+        """VJP of multiple_contact_inverse_dynamics_device; seed_ptr: caller-owned [B, ndof] workspace in the arithmetic type; gguess_ptr:
+        optional [B, k, 6] buffer receiving dL/d(guess)."""
+        k, b, p = self._contact_set(bodies, points)
+        _cabi.check(_cabi.lib().nb2_multiple_contact_inverse_dynamics_backward(self.handle, B, k, b.ctypes.data, p.ctypes.data, state_ptr, None,
+                                                                               wi_ptr, saved_ptr, wrench_ptr, guess_ptr, gtau_ptr, gwrench_ptr,
+                                                                               seed_ptr, gstate_ptr, gnext_ptr, ginertia_ptr, gguess_ptr,
+                                                                               precision, stream))
+
     def contact_workspace_bytes(self, B):
         return int(_cabi.lib().nb2_contact_workspace_bytes(self.handle, B))
 

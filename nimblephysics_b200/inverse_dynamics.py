@@ -1,5 +1,6 @@
-"""``inverse_dynamics(world, state, next_vel, mass=None)`` — contact-free inverse dynamics, batched and differentiable — and
-``contact_inverse_dynamics(world, state, next_vel, contact_body, mass=None)``, the same force split into a contact wrench and joint torques.
+"""``inverse_dynamics(world, state, next_vel, mass=None)`` — contact-free inverse dynamics, batched and differentiable —,
+``contact_inverse_dynamics(world, state, next_vel, contact_body, mass=None)``, the same force split into a contact wrench and joint torques,
+and ``multiple_contact_inverse_dynamics(world, state, next_vel, contact_bodies, mass=None, wrench_guesses=None)``, split over several bodies.
 
 It answers the reverse question of ``timestep``: which generalised force takes each world from ``state = [q; qdot]`` to the
 velocity ``next_vel`` in one contact-free step?
@@ -22,14 +23,23 @@ total external wrench the motion needs, the ground reaction of a robot standing 
 skeleton is named.  tau differs from tau_ID only on the joints between the contact body and the root; every other dof, other skeletons
 included, is tau_ID bit for bit.  The frame in which the reference reports its ``contactWrench`` is not checked here.
 
+Multiple-contact inverse dynamics (the reference's ``Skeleton::getMultipleContactInverseDynamics(nextVel, bodies, bodyWrenchGuesses)``):
+with k contact bodies c_1..c_k of one skeleton, J_i their Jacobians as above, p_i the world position of c_i's own origin and g_i guesses,
+
+    tau + sum_i J_i(q)^T w_i = tau_ID   on every dof ,     tau = 0 on the free root ,
+    minimise  sum_i | Gamma(p_i)^-1 (w_i - g_i) |^2 ,      Gamma(p) = [[I, [p]x], [0, I]] ,
+
+so the deviation from each guess is measured as [torque about p_i; force], independently of where the world origin is.  The w_i sum to the
+one-body wrench; the objective and the wrench frame are this package's, the reference's could not be checked.
+
 Precision follows the state's dtype: float64 tensors run the fp64 kernels with fp64 rows, anything else the fp32 ones.
 Gradients flow to ``state``, ``next_vel`` and ``mass`` (1-D: ``setMasses``, shared by the batch, gradient summed; 2-D ``[B, m]``:
 per world, the World is left untouched).  The work is done by libnb2.so (include/nb2.h ``nb2_inverse_dynamics``,
-``nb2_contact_inverse_dynamics``).
+``nb2_contact_inverse_dynamics``, ``nb2_multiple_contact_inverse_dynamics``).
 """
 from __future__ import annotations
 
-from typing import Optional
+from typing import Optional, Sequence
 
 import torch
 
@@ -39,6 +49,8 @@ from .world import FREE
 
 _WHO = "inverse_dynamics()"
 _WHO_CONTACT = "contact_inverse_dynamics()"
+_WHO_MULTI = "multiple_contact_inverse_dynamics()"
+MAX_CONTACT_BODIES = 4  # include/nb2.h NB2_MAX_CONTACT_BODIES
 
 
 def _check_rows(world, state, next_vel, who):
@@ -192,6 +204,68 @@ class ContactInverseDynamicsLayer(torch.autograd.Function):
         return (None,) + _input_grads(ctx, gs, gn, gi) + (None,)
 
 
+def contact_body_indices(world, bodies, who: str = _WHO_MULTI) -> list:
+    """The raw indices of `bodies`, 1..MAX_CONTACT_BODIES distinct BodyNodes of one skeleton of `world`, each as contact_body_index
+    requires.  ValueError before any device work otherwise."""
+    bodies = list(bodies)
+    if not 1 <= len(bodies) <= MAX_CONTACT_BODIES:
+        raise ValueError(f"{who}: {len(bodies)} contact bodies, expected 1 to {MAX_CONTACT_BODIES}")
+    if len({id(b) for b in bodies}) != len(bodies):
+        raise ValueError(f"{who}: a contact body appears twice")
+    raw = [contact_body_index(world, b, who) for b in bodies]
+    if any(b.skeleton is not bodies[0].skeleton for b in bodies):
+        raise ValueError(f"{who}: the contact bodies belong to different skeletons")
+    return raw
+
+
+class MultipleContactInverseDynamicsLayer(torch.autograd.Function):
+    """Multiple-contact inverse dynamics of the raw bodies `raw_bodies` (see contact_body_indices); guesses: [B, k, 6] / [k, 6] or None;
+    world_inertia as for InverseDynamicsLayer.  Returns (tau, wrenches)."""
+
+    @staticmethod
+    def forward(ctx, world, state, next_vel, mass, world_inertia, guesses, raw_bodies):
+        dm, sd, vd, wi, need_grad = _prepare(ctx, world, state, next_vel, mass, world_inertia, _WHO_MULTI)
+        need_grad = need_grad or ctx.needs_input_grad[5]
+        k, cm = len(raw_bodies), dm.cm
+        ctx.bodies = [int(cm.body_owner[r]) for r in raw_bodies]
+        ctx.points = [cm.body_T[r][:3, 3].astype(float) for r in raw_bodies]  # each body's own origin in its owner's canonical frame
+        B, dev = ctx.B, sd.device
+        gd = guesses.detach().reshape(B, k, 6).to(device=dev, dtype=sd.dtype).contiguous() if guesses is not None else None
+        with torch.cuda.device(dev):
+            tau = torch.empty((B, dm.ndof), dtype=sd.dtype, device=dev)
+            wrenches = torch.empty((B, k, 6), dtype=sd.dtype, device=dev)
+            saved = torch.empty((dm.saved_words, B), dtype=sd.dtype, device=dev) if need_grad else None
+            dm.multiple_contact_inverse_dynamics_device(B, ctx.bodies, ctx.points, sd.data_ptr(), vd.data_ptr(), _ptr(gd), tau.data_ptr(),
+                                                        wrenches.data_ptr(), _ptr(saved), torch.cuda.current_stream().cuda_stream, ctx.prec,
+                                                        wi_ptr=_ptr(wi))
+        ctx.guess_grad = ctx.needs_input_grad[5]
+        ctx.guess_like = guesses
+        if need_grad:
+            ctx.save_for_backward(sd, saved, wi, wrenches, gd)
+        if ctx.single:
+            tau, wrenches = tau[0], wrenches[0]
+        return tau.to(device=state.device, dtype=state.dtype), wrenches.to(device=state.device, dtype=state.dtype)
+
+    @staticmethod
+    def backward(ctx, grad_tau, grad_wrenches):
+        dm, B = ctx.dm, ctx.B
+        sd, saved, wi, wrenches, gd = ctx.saved_tensors
+        dev, k = sd.device, wrenches.shape[1]
+        g = grad_tau.detach().reshape(B, dm.ndof).to(device=dev, dtype=sd.dtype).contiguous()
+        gw = grad_wrenches.detach().reshape(B, k, 6).to(device=dev, dtype=sd.dtype).contiguous()
+        with torch.cuda.device(dev):
+            gs, gn, gi = _backward_buffers(ctx, dev, sd.dtype)
+            seed = torch.empty((B, dm.ndof), dtype=sd.dtype, device=dev)
+            gg = torch.empty((B, k, 6), dtype=sd.dtype, device=dev) if ctx.guess_grad else None
+            dm.multiple_contact_inverse_dynamics_backward_device(B, ctx.bodies, ctx.points, sd.data_ptr(), saved.data_ptr(), wrenches.data_ptr(),
+                                                                 _ptr(gd), g.data_ptr(), gw.data_ptr(), seed.data_ptr(), gs.data_ptr(),
+                                                                 gn.data_ptr(), torch.cuda.current_stream().cuda_stream, ctx.prec,
+                                                                 ginertia_ptr=_ptr(gi), gguess_ptr=_ptr(gg), wi_ptr=_ptr(wi))
+        if gg is not None:
+            gg = gg.reshape(ctx.guess_like.shape).to(device=ctx.guess_like.device, dtype=ctx.guess_like.dtype)
+        return (None,) + _input_grads(ctx, gs, gn, gi) + (gg, None)
+
+
 def inverse_dynamics(world, state: torch.Tensor, next_vel: torch.Tensor, mass: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Generalised force [B, n] (or [n] for a 1-D state) that takes every world from `state` [B, 2n] to `next_vel` [B, n] in one
     contact-free step (see the module docstring).  mass: None, a 1-D vector [getMassDims()] (world.setMasses(mass) first, shared by the
@@ -212,3 +286,27 @@ def contact_inverse_dynamics(world, state: torch.Tensor, next_vel: torch.Tensor,
     if mass is not None and mass.dim() == 2:
         return ContactInverseDynamicsLayer.apply(world, state, next_vel, None, per_world_inertia(world, state, mass, _WHO_CONTACT), raw_body)
     return ContactInverseDynamicsLayer.apply(world, state, next_vel, mass, None, raw_body)
+
+
+def multiple_contact_inverse_dynamics(world, state: torch.Tensor, next_vel: torch.Tensor, contact_bodies: Sequence, mass: Optional[torch.Tensor] = None,
+                                      wrench_guesses: Optional[torch.Tensor] = None):
+    """(tau, wrenches): tau [B, n] (or [n]) and wrenches [B, k, 6] (or [k, 6]) with tau + sum_i J_i^T w_i =
+    inverse_dynamics(world, state, next_vel, mass), tau = 0 on the free root, and the w_i as close as possible to `wrench_guesses` (see
+    the module docstring).  contact_bodies: 1 to 4 distinct BodyNodes of one mobile skeleton of `world` with a FreeJoint root; each wrench
+    is [torque; force] in world axes about the world origin, on that body's own origin.  wrench_guesses: [B, k, 6] ([k, 6] for a 1-D
+    state) in the same convention, or None (0).  ValueError for any of these, before any device work.
+
+    The motion fixes only the total wrench.  Without guesses the split is the minimum-norm one, not a prediction of how the load is
+    actually shared; with measured per-body wrenches (force plates) as guesses it is the dynamically consistent set closest to them, with
+    the matching joint torques.  With one body the result is contact_inverse_dynamics's.  Gradients of both outputs reach state, next_vel,
+    mass and the guesses."""
+    raw_bodies = contact_body_indices(world, contact_bodies)
+    _check_rows(world, state, next_vel, _WHO_MULTI)
+    if wrench_guesses is not None:
+        want = tuple(state.shape[:-1]) + (len(raw_bodies), 6)
+        if tuple(wrench_guesses.shape) != want:
+            raise ValueError(f"{_WHO_MULTI}: wrench_guesses has shape {tuple(wrench_guesses.shape)}, expected {list(want)}")
+    if mass is not None and mass.dim() == 2:
+        return MultipleContactInverseDynamicsLayer.apply(world, state, next_vel, None, per_world_inertia(world, state, mass, _WHO_MULTI),
+                                                         wrench_guesses, raw_bodies)
+    return MultipleContactInverseDynamicsLayer.apply(world, state, next_vel, mass, None, wrench_guesses, raw_bodies)

@@ -1,5 +1,5 @@
 """Small end-to-end run for compute-sanitizer (memcheck): contact-free fwd+bwd (device + pinned-host paths, partial groups),
-contact fwd+bwd, fused rollout, inverse dynamics and contact inverse dynamics fwd+bwd (both precisions, per-world masses, partial
+contact fwd+bwd, fused rollout, inverse dynamics, contact and multiple-contact inverse dynamics fwd+bwd (both precisions, per-world masses, partial
 groups and partial blocks)."""
 import sys
 import numpy as np, torch
@@ -36,6 +36,10 @@ for B in (7, 203):
         mw.tuneMass(mw.skeletons[0]._ordered_bodies()[0], 0)
         nb.inverse_dynamics(mw, st, vn, mass * torch.tensor(mw.getMasses(), device="cuda")).sum().backward()
         tau, wr = nb.contact_inverse_dynamics(mw, st, vn, mw.skeletons[0]._ordered_bodies()[27], mass * torch.tensor(mw.getMasses(), device="cuda"))
+        (tau.sum() + wr.sum()).backward()
+        bodies = [b for b in mw.skeletons[0]._ordered_bodies() if b.name in ("l_foot", "r_foot", "l_hand", "r_hand")]
+        guess = torch.zeros((B, 4, 6), device="cuda", dtype=dt, requires_grad=True)
+        tau, wr = nb.multiple_contact_inverse_dynamics(mw, st, vn, bodies, mass * torch.tensor(mw.getMasses(), device="cuda"), guess)
         (tau.sum() + wr.sum()).backward()
 torch.cuda.synchronize()
 print("sanitize run finished")
