@@ -264,6 +264,21 @@ int nb2_multiple_contact_inverse_dynamics_backward(const nb2_model* m, int B, in
                                                    void* seed, void* grad_state, void* grad_next_vel, double* grad_inertia, void* grad_guess,
                                                    int precision, void* stream);
 
+/* Joint-space mass matrix M(q) [B, ndof, ndof] (row-major) of B worlds at the positions pos [B, ndof]: the matrix the step inverts, in its
+ * velocity coordinates (free joints: body twist, S = I6), block-diagonal over trees; contacts, limits, springs and damping are not part of
+ * it.  Rows in the arithmetic type of `precision` (NB2_FP64: double, else float); world_inertia as nb2_step_forward_pw (NULL: the model's).
+ * Composite-rigid-body algorithm, one warp per world.  The result is exactly symmetric.  NB2_ERR_INVALID for a model without dofs. */
+int nb2_mass_matrix(const nb2_model* m, int B, const void* pos, const double* world_inertia, void* M, int precision, void* stream);
+/* M(q)^-1 [B, ndof, ndof]: the step's articulated inertias and one bias-free unit-force sweep pair per column (not a factorisation of M). */
+int nb2_inverse_mass_matrix(const nb2_model* m, int B, const void* pos, const double* world_inertia, void* Minv, int precision, void* stream);
+/* Vector-Jacobian products, L = <grad, out>.  grad_pos [B, ndof] (written; a free root's six entries are exactly 0), grad_inertia
+ * [10 * nb][B] fp64 or NULL (written, as nb2_inverse_dynamics_backward).  The inverse's backward takes the forward's Minv and a caller-owned
+ * workspace [B, ndof, ndof] in the arithmetic type; neither call allocates. */
+int nb2_mass_matrix_backward(const nb2_model* m, int B, const void* pos, const double* world_inertia, const void* grad_M, void* grad_pos,
+                             double* grad_inertia, int precision, void* stream);
+int nb2_inverse_mass_matrix_backward(const nb2_model* m, int B, const void* pos, const double* world_inertia, const void* Minv, const void* grad_Minv,
+                                     void* workspace, void* grad_pos, double* grad_inertia, int precision, void* stream);
+
 /* Batched boxed-LCP solves on the device: B independent problems, one warp each — the reference's pointer-style lower boundary
  * BoxedLcpSolver::solve(n, A, x, b, nub, lo, hi, findex, earlyTermination) (dart/constraint/BoxedLcpSolver.hpp:125-135) and the
  * solve chain of BoxedLcpConstraintSolver::solveLcp (BoxedLcpConstraintSolver.cpp:352-789).  Device pointers; problem w has dimension

@@ -17,6 +17,7 @@
 
 #include "../../include/nb2.h"
 #include "nb2_dyn.cuh"
+#include "nb2_mm.cuh"
 #include "nb2_cw.cuh"
 #include "nb2_host_model.h"
 
@@ -318,6 +319,86 @@ k_mcid_bwd(const __grid_constant__ Nb2ModelDev<R> M, const __grid_constant__ nb2
   const size_t n = M.ndof, kw = (size_t)w * 6 * b.k;
   nb2::mcid_vjp<R>(M, b, state + w * 2 * n, wrench + kw, guess ? guess + kw : nullptr, gtau + w * n, gwrench + kw, seed ? seed + w * n : nullptr,
                    seed && gguess ? gguess + kw : nullptr, seed ? nullptr : gstate + w * 2 * n);
+}
+
+// ---- mass matrix and its inverse (nb2_mass_matrix / nb2_inverse_mass_matrix / _backward, nb2_mm.cuh): ONE WARP PER WORLD, one world per
+// block, the world's working set and its n x n result in the block's dynamic shared memory.  The result leaves as one contiguous block.
+// row-major n*n block of one world: 16-byte stores when the world's block is aligned (lanes take consecutive vectors), words otherwise
+template <class R>
+__device__ __forceinline__ void mm_store_block(R* __restrict__ dst, const R* src, int words, int lane) {
+  if (((reinterpret_cast<size_t>(dst) | (size_t)words * sizeof(R)) & 15) == 0) {
+    const int nv = (int)((size_t)words * sizeof(R) / 16);
+    for (int k = lane; k < nv; k += 32) reinterpret_cast<uint4*>(dst)[k] = reinterpret_cast<const uint4*>(src)[k];
+  } else {
+    for (int k = lane; k < words; k += 32) dst[k] = src[k];
+  }
+}
+template <class R>
+__global__ void __launch_bounds__(32)
+k_mm_fwd(const __grid_constant__ Nb2ModelDev<R> M, int B, const R* __restrict__ pos, const double* __restrict__ winertia, R* __restrict__ out) {
+  extern __shared__ __align__(16) unsigned char nb2_smem[];
+  R* ws = reinterpret_cast<R*>(nb2_smem);
+  const int lane = threadIdx.x;
+  const size_t w = blockIdx.x, n = M.ndof;
+  nb2::crba_init<R>(M, pos + w * n, winertia ? winertia + w : nullptr, (size_t)B, ws, lane, 32);
+  __syncwarp();
+  nb2::crba_composite<R>(M, ws, lane);
+  __syncwarp();
+  nb2::crba_columns<R>(M, ws, lane, 32);
+  __syncwarp();
+  mm_store_block<R>(out + w * n * n, ws + nb2::mm_layout(M.nb, M.ndof).oMat, M.ndof * M.ndof, lane);
+}
+template <class R>
+__global__ void __launch_bounds__(32)
+k_minv_fwd(const __grid_constant__ Nb2ModelDev<R> M, int B, const R* __restrict__ pos, const double* __restrict__ winertia, R* __restrict__ out) {
+  extern __shared__ __align__(16) unsigned char nb2_smem[];
+  R* ws = reinterpret_cast<R*>(nb2_smem);
+  const int lane = threadIdx.x;
+  const size_t w = blockIdx.x, n = M.ndof;
+  nb2::minv_init<R>(M, pos + w * n, ws, lane, 32);
+  __syncwarp();
+  nb2::minv_articulated<R>(M, ws, winertia ? winertia + w : nullptr, (size_t)B, lane, 32);
+  __syncwarp();
+  nb2::minv_columns<R>(M, ws, lane, 32);
+  __syncwarp();
+  mm_store_block<R>(out + w * n * n, ws + nb2::minv_layout(M.nb, M.ndof, M.nslots, M.nfree, 32).oMat, M.ndof * M.ndof, lane);
+}
+// minv == nullptr: the M backward of grad; else the M^-1 backward (G_M = -Minv Gs Minv first, `tmp` a caller-owned [B, n, n] workspace)
+template <class R>
+__global__ void __launch_bounds__(32)
+k_mm_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, const R* __restrict__ pos, const double* __restrict__ winertia, const R* __restrict__ grad,
+         const R* __restrict__ minv, R* __restrict__ tmp, R* __restrict__ gpos, double* __restrict__ ginertia) {
+  extern __shared__ __align__(16) unsigned char nb2_smem[];
+  R* ws = reinterpret_cast<R*>(nb2_smem);
+  const int lane = threadIdx.x;
+  const size_t w = blockIdx.x, n = M.ndof;
+  const R* q = pos + w * n;
+  const double* wi = winertia ? winertia + w : nullptr;
+  if (minv) {
+    nb2::mminvb_load<R>(M, minv + w * n * n, grad + w * n * n, ws, lane, 32);
+    __syncwarp();
+    nb2::mminvb_left<R>(M, ws, tmp + w * n * n, lane, 32);
+    __syncwarp();
+    nb2::mminvb_right<R>(M, ws, tmp + w * n * n, lane, 32);
+  }
+  nb2::mmb_init<R>(M, q, minv ? nullptr : grad + w * n * n, ws, lane, 32);
+  __syncwarp();
+  nb2::mmb_root_frames<R>(M, ws, lane, 32);
+  __syncwarp();
+#pragma unroll 1
+  for (int b = 0; b < M.nb; b++) {
+    nb2::mmb_body_chain<R>(M, ws, b, lane, 32);
+    __syncwarp();
+    nb2::mmb_body_columns<R>(M, ws, b, lane, 32);
+    __syncwarp();
+    nb2::mmb_body_forces<R>(M, ws, b, wi, (size_t)B, lane, 32);
+    __syncwarp();
+    nb2::mmb_body_reduce<R>(M, ws, b, ginertia ? ginertia + w : nullptr, (size_t)B, lane, 32);
+    __syncwarp();
+  }
+  nb2::mmb_free_q<R>(M, q, ws, lane, 32);
+  __syncwarp();
+  nb2::mmb_store_row<R>(M, ws, gpos + w * n, lane, 32);
 }
 
 // ---- fused step kernels of worlds WITH a contact stage (fp64): ONE WARP PER WORLD.
@@ -1700,6 +1781,83 @@ int nb2_multiple_contact_inverse_dynamics_backward(const nb2_model* cm, int B, i
     if (rc) return rc;
     if (b.k == 1) return launch_cid<R>(m, b.c[0], B, false, S, nullptr, Wr, nullptr, Gt, Gw, nullptr, (R*)grad_state, st);
     return launch_mcid<R>(m, b, B, false, S, G, nullptr, Wr, nullptr, Gt, Gw, nullptr, nullptr, (R*)grad_state, st);
+  });
+}
+}  // extern "C"
+
+// ---- mass matrix and its inverse: one warp per world, one world per block, the shared memory sized from the model
+enum { MM_FWD = 0, MM_INV = 1, MM_BWD = 2, MM_INV_BWD = 3 };
+static size_t mm_smem_words(const Nb2ModelDev<float>& M, int which) {
+  if (which == MM_FWD) return nb2::mm_layout(M.nb, M.ndof).total;
+  if (which == MM_INV) return nb2::minv_layout(M.nb, M.ndof, M.nslots, M.nfree, 32).total;
+  if (which == MM_BWD) return nb2::mmb_layout(M.nb, M.ndof, 32).total;
+  return nb2::mminvb_words(M.nb, M.ndof, 32);
+}
+template <class R>
+static int launch_mm(const nb2_model* m, int which, int B, const R* pos, const double* wi, R* out, const R* grad, const R* minv, R* tmp,
+                     R* gpos, double* gI, cudaStream_t st, const char* who) {
+  const nb2_variant& v = m->variants[0];
+  const size_t smem = mm_smem_words(v.mf, which) * sizeof(R);
+  if (smem > (size_t)kMaxSmem) { g_err = std::string(who) + ": the model's working set does not fit in shared memory"; return NB2_ERR_INVALID; }
+  int rc;
+  if (which == MM_FWD) {
+    if ((rc = allow_max_smem<k_mm_fwd<R>>())) return rc;
+    k_mm_fwd<R><<<B, 32, smem, st>>>(model_of<R>(v), B, pos, wi, out);
+  } else if (which == MM_INV) {
+    if ((rc = allow_max_smem<k_minv_fwd<R>>())) return rc;
+    k_minv_fwd<R><<<B, 32, smem, st>>>(model_of<R>(v), B, pos, wi, out);
+  } else {
+    if ((rc = allow_max_smem<k_mm_bwd<R>>())) return rc;
+    k_mm_bwd<R><<<B, 32, smem, st>>>(model_of<R>(v), B, pos, wi, grad, minv, tmp, gpos, gI);
+  }
+  g_launches++;
+  NB2_CUDA(cudaGetLastError());
+  return NB2_OK;
+}
+static int mm_args_ok(const nb2_model* m, int B, bool ok, const char* who) {
+  if (!m || B < 0 || !ok) { g_err = std::string(who) + ": bad argument"; return NB2_ERR_INVALID; }
+  if (m->mf.ndof == 0) { g_err = std::string(who) + ": the model has no dofs"; return NB2_ERR_INVALID; }
+  return NB2_OK;
+}
+extern "C" {
+int nb2_mass_matrix(const nb2_model* m, int B, const void* pos, const double* world_inertia, void* M, int precision, void* stream) {
+  static const char* who = "nb2_mass_matrix";
+  if (int rc = mm_args_ok(m, B, pos && M, who)) return rc;
+  if (B == 0) return NB2_OK;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    return launch_mm<R>(m, MM_FWD, B, (const R*)pos, world_inertia, (R*)M, nullptr, nullptr, nullptr, nullptr, nullptr, (cudaStream_t)stream, who);
+  });
+}
+int nb2_inverse_mass_matrix(const nb2_model* m, int B, const void* pos, const double* world_inertia, void* Minv, int precision, void* stream) {
+  static const char* who = "nb2_inverse_mass_matrix";
+  if (int rc = mm_args_ok(m, B, pos && Minv, who)) return rc;
+  if (B == 0) return NB2_OK;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    return launch_mm<R>(m, MM_INV, B, (const R*)pos, world_inertia, (R*)Minv, nullptr, nullptr, nullptr, nullptr, nullptr, (cudaStream_t)stream, who);
+  });
+}
+int nb2_mass_matrix_backward(const nb2_model* m, int B, const void* pos, const double* world_inertia, const void* grad_M, void* grad_pos,
+                             double* grad_inertia, int precision, void* stream) {
+  static const char* who = "nb2_mass_matrix_backward";
+  if (int rc = mm_args_ok(m, B, pos && grad_M && grad_pos, who)) return rc;
+  if (B == 0) return NB2_OK;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    return launch_mm<R>(m, MM_BWD, B, (const R*)pos, world_inertia, nullptr, (const R*)grad_M, nullptr, nullptr, (R*)grad_pos, grad_inertia,
+                        (cudaStream_t)stream, who);
+  });
+}
+int nb2_inverse_mass_matrix_backward(const nb2_model* m, int B, const void* pos, const double* world_inertia, const void* Minv, const void* grad_Minv,
+                                     void* workspace, void* grad_pos, double* grad_inertia, int precision, void* stream) {
+  static const char* who = "nb2_inverse_mass_matrix_backward";
+  if (int rc = mm_args_ok(m, B, pos && Minv && grad_Minv && workspace && grad_pos, who)) return rc;
+  if (B == 0) return NB2_OK;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    return launch_mm<R>(m, MM_INV_BWD, B, (const R*)pos, world_inertia, nullptr, (const R*)grad_Minv, (const R*)Minv, (R*)workspace, (R*)grad_pos,
+                        grad_inertia, (cudaStream_t)stream, who);
   });
 }
 int nb2_model_ndof(const nb2_model* m) { return m ? m->mf.ndof : -1; }

@@ -195,6 +195,24 @@ class DeviceModel:
                                                                                seed_ptr, gstate_ptr, gnext_ptr, ginertia_ptr, gguess_ptr,
                                                                                precision, stream))
 
+    def mass_matrix_device(self, B, pos_ptr, out_ptr, stream, precision=FP32, wi_ptr=None):
+        """M(q) [B, n, n] (include/nb2.h nb2_mass_matrix): rows in the arithmetic type of `precision`."""
+        _cabi.check(_cabi.lib().nb2_mass_matrix(self.handle, B, pos_ptr, wi_ptr, out_ptr, precision, stream))
+
+    def inverse_mass_matrix_device(self, B, pos_ptr, out_ptr, stream, precision=FP32, wi_ptr=None):
+        """M(q)^-1 [B, n, n] (include/nb2.h nb2_inverse_mass_matrix)."""
+        _cabi.check(_cabi.lib().nb2_inverse_mass_matrix(self.handle, B, pos_ptr, wi_ptr, out_ptr, precision, stream))
+
+    def mass_matrix_backward_device(self, B, pos_ptr, gM_ptr, gpos_ptr, stream, precision=FP32, ginertia_ptr=None, wi_ptr=None):
+        """VJP of mass_matrix_device; ginertia_ptr: optional [10*nb, B] float64 buffer receiving dL/d(inertia parameters)."""
+        _cabi.check(_cabi.lib().nb2_mass_matrix_backward(self.handle, B, pos_ptr, wi_ptr, gM_ptr, gpos_ptr, ginertia_ptr, precision, stream))
+
+    def inverse_mass_matrix_backward_device(self, B, pos_ptr, minv_ptr, gMinv_ptr, ws_ptr, gpos_ptr, stream, precision=FP32, ginertia_ptr=None,
+                                            wi_ptr=None):
+        """VJP of inverse_mass_matrix_device from its output minv_ptr; ws_ptr: caller-owned [B, n, n] workspace in the arithmetic type."""
+        _cabi.check(_cabi.lib().nb2_inverse_mass_matrix_backward(self.handle, B, pos_ptr, wi_ptr, minv_ptr, gMinv_ptr, ws_ptr, gpos_ptr,
+                                                                 ginertia_ptr, precision, stream))
+
     def contact_workspace_bytes(self, B):
         return int(_cabi.lib().nb2_contact_workspace_bytes(self.handle, B))
 

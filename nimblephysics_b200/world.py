@@ -411,6 +411,22 @@ class Skeleton:
             return w._state[off:off + self.getNumDofs()].copy()
         return np.array([j.init_pos[k] for j, k in self._dof_slots()])
 
+    def _mass_matrix_block(self, inverse):
+        w, off = self._dof_offset_in_world()
+        if w is None:
+            raise ValueError("Skeleton.getMassMatrix(): the skeleton is not part of a World")
+        n = self.getNumDofs()
+        return w._mass_matrix(inverse)[off:off + n, off:off + n].copy()
+
+    def getMassMatrix(self):
+        """Skeleton::getMassMatrix: this skeleton's block of its World's mass matrix at the current positions (numpy fp64; fp64 kernels,
+        nimblephysics_b200.mass_matrix)."""
+        return self._mass_matrix_block(False)
+
+    def getInvMassMatrix(self):
+        """Skeleton::getInvMassMatrix: this skeleton's block of M^-1 (M is block-diagonal over skeletons)."""
+        return self._mass_matrix_block(True)
+
     def setVelocity(self, i, v):
         w, off = self._dof_offset_in_world()
         if w is None:
@@ -831,6 +847,19 @@ class World:
 
     def getPositions(self):
         return self.getState()[: self.getNumDofs()]
+
+    def _mass_matrix(self, inverse):
+        from .mass_matrix import _single_world
+
+        return _single_world(self, "World.getInvMassMatrix()" if inverse else "World.getMassMatrix()", inverse)
+
+    def getMassMatrix(self):
+        """The world's mass matrix [n, n] at the current positions (numpy fp64, computed by the fp64 kernels at B = 1)."""
+        return self._mass_matrix(False)
+
+    def getInvMassMatrix(self):
+        """M^-1 [n, n] at the current positions (numpy fp64, fp64 kernels)."""
+        return self._mass_matrix(True)
 
     def getVelocities(self):
         return self.getState()[self.getNumDofs():]

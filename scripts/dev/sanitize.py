@@ -1,6 +1,6 @@
 """Small end-to-end run for compute-sanitizer (memcheck): contact-free fwd+bwd (device + pinned-host paths, partial groups),
-contact fwd+bwd, fused rollout, inverse dynamics, contact and multiple-contact inverse dynamics fwd+bwd (both precisions, per-world masses, partial
-groups and partial blocks)."""
+contact fwd+bwd, fused rollout, inverse dynamics, contact and multiple-contact inverse dynamics fwd+bwd, the mass matrix and its inverse fwd+bwd (both precisions, per-world masses,
+partial groups and partial blocks)."""
 import sys
 import numpy as np, torch
 sys.path.insert(0, ".")
@@ -41,5 +41,8 @@ for B in (7, 203):
         guess = torch.zeros((B, 4, 6), device="cuda", dtype=dt, requires_grad=True)
         tau, wr = nb.multiple_contact_inverse_dynamics(mw, st, vn, bodies, mass * torch.tensor(mw.getMasses(), device="cuda"), guess)
         (tau.sum() + wr.sum()).backward()
+        q = st.detach()[:, :raw.ndof].clone().requires_grad_()
+        for f in (nb.mass_matrix, nb.inverse_mass_matrix):
+            f(mw, q, mass * torch.tensor(mw.getMasses(), device="cuda")).sum().backward()
 torch.cuda.synchronize()
 print("sanitize run finished")
