@@ -50,9 +50,20 @@ template <class R, int K>
 __device__ __forceinline__ const R* stage_body_table(const Nb2ModelDev<R>& M, R* tab) {
   if constexpr (K == 1) return nullptr;
   else {
-  for (int k = threadIdx.x; k < M.nb * NB2_BT_WORDS; k += blockDim.x) {
-    const int i = k / NB2_BT_WORDS, j = k - i * NB2_BT_WORDS;
-    tab[k] = (j < 12) ? M.Xtree[i][j] : M.inertia[i][j - 12];
+  // copied in 8-byte units: these loads have lane-varying addresses too, and the constant bank replays a load once per
+  // distinct address, so fp32 tables take half the replays of a word-by-word copy.  The 8-byte loads need M itself 8-byte
+  // aligned in the parameter space: every kernel that calls this takes M as its FIRST parameter (the parameter space starts
+  // aligned), keep it there.  The member offsets are checked below; an alignas(8) on Nb2ModelDev would also guarantee it, but it
+  // changes the code generated for most kernels that read the model (inverse dynamics, mass matrix, the one-lane step kernels).
+  using U = std::conditional_t<sizeof(R) == 4, float2, double>;
+  constexpr int XU = 12 * sizeof(R) / sizeof(U), IU = 10 * sizeof(R) / sizeof(U), BU = XU + IU;  // units per Xtree / inertia row
+  static_assert(offsetof(Nb2ModelDev<R>, Xtree) % sizeof(U) == 0 && offsetof(Nb2ModelDev<R>, inertia) % sizeof(U) == 0, "unaligned body tables");
+  const U* xs = reinterpret_cast<const U*>(&M.Xtree[0][0]);
+  const U* is = reinterpret_cast<const U*>(&M.inertia[0][0]);
+  U* t = reinterpret_cast<U*>(tab);
+  for (int k = threadIdx.x; k < M.nb * BU; k += blockDim.x) {
+    const int i = k / BU, j = k - i * BU;
+    t[k] = (j < XU) ? xs[i * XU + j] : is[i * IU + j - XU];
   }
   __syncthreads();
   return tab;
@@ -91,6 +102,23 @@ template <int K> __host__ __device__ constexpr size_t staging_bytes(int floats_p
   return (((size_t)floats_per_world * CoopShape<K>::WPW * sizeof(float) + 15) & ~(size_t)15) + 16;
 }
 
+// ---- optional stage clocks of the contact-free step kernels (-DNB2_STEP_CLOCKS; dev builds only, scripts/dev/stage_clocks.py):
+// thread 0 of every NB2_CLK_EVERY-th warp of the grid (up to NB2_CLK_WARPS of them) records clock64() at kernel entry, after the
+// body-table and input staging, and after every stage including its barrier.  Default builds compile none of it.
+#ifdef NB2_STEP_CLOCKS
+#define NB2_CLK_WARPS 8
+#define NB2_CLK_EVERY 64
+#define NB2_CLK_SLOTS 16
+__device__ long long nb2_step_clk[2][NB2_CLK_WARPS][NB2_CLK_SLOTS];  // [forward, backward][sampled warp][entry, staged, stage 0, 1, ...]
+#define NB2_CLK(dir, k)                                                                                                   \
+  do {                                                                                                                    \
+    const int w_ = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);                                                   \
+    if ((threadIdx.x & 31) == 0 && w_ % NB2_CLK_EVERY == 0 && w_ / NB2_CLK_EVERY < NB2_CLK_WARPS) nb2_step_clk[dir][w_ / NB2_CLK_EVERY][k] = clock64(); \
+  } while (0)
+#else
+#define NB2_CLK(dir, k)
+#endif
+
 // PW: the variant with a per-world inertia table (nb2_step_forward_pw).  A compile-time switch: as a run-time pointer test it cost the
 // shared-table kernels registers (fp32) and spills (fp64).
 template <class R, int K, bool PW>
@@ -100,39 +128,46 @@ k_step_fwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
            float* __restrict__ state_copy, float* __restrict__ action_copy, const double* __restrict__ winertia) {
   // worlds [w0, w0 + count) of a batch of B (B is the stride of the saved stream and of the per-world inertia; the host entry points launch chunks)
   extern __shared__ __align__(16) unsigned char nb2_smem[];
+  NB2_CLK(0, 0);
   constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
   const int li = threadIdx.x & 31, slot = li / K, lane = li % K;
   const int g0 = (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * WPW;  // first world of this warp's group
   const int nworlds = min(WPW, count - g0);                                      // <= 0: idle warp (grid tail)
   const bool valid = slot < nworlds;
   const size_t wg = (size_t)w0 + (nworlds > 0 ? g0 : 0);
-  const R* bt = stage_body_table<R, K>(M, reinterpret_cast<R*>(nb2_smem));
   R* scr0 = reinterpret_cast<R*>(nb2_smem) + body_table_words<K>(M.nb) + (size_t)(threadIdx.x >> 5) * words * ST;
   R* scr = scr0 + slot;
   R* sv = saved ? saved + wg + (valid ? slot : 0) : nullptr;
   const double* wi = PW ? winertia + wg + (valid ? slot : 0) : nullptr;
   constexpr unsigned sync_mask = (K > 1) ? NB2_FWD_SYNC_MASK : NB2_FWD_SYNC_MASK_1LANE;
-  // input rows of the group: through the bulk-copy staging buffer when they qualify, else read in place
+  // input rows of the group: through the bulk-copy staging buffer when they qualify, else read in place.  The copy is in
+  // flight while the block stages the body table: the table's constant-bank loads (one replay per distinct address) and
+  // the DRAM round trip of the rows overlap instead of adding up.
   const float* st_src = state + wg * 2 * M.ndof;
   const float* act_src = action + wg * M.na;
+  unsigned long long* bar = nullptr;
   if (nworlds > 0) {
     const size_t sb = (size_t)nworlds * 2 * M.ndof * sizeof(float), ab = (size_t)nworlds * M.na * sizeof(float);
     if (bulk_ok(st_src, sb) && bulk_ok(act_src, ab)) {
       unsigned char* stg = nb2_smem + (((size_t)body_table_words<K>(M.nb) + (size_t)(blockDim.x >> 5) * words * ST) * sizeof(R) + 15 & ~(size_t)15) +
                            (size_t)(threadIdx.x >> 5) * staging_bytes<K>(2 * M.ndof + M.na);
-      unsigned long long* bar = reinterpret_cast<unsigned long long*>(stg + staging_bytes<K>(2 * M.ndof + M.na) - 16);
+      bar = reinterpret_cast<unsigned long long*>(stg + staging_bytes<K>(2 * M.ndof + M.na) - 16);
       if (li == 0) {
         mbar_init(bar);
         mbar_expect_tx(bar, (unsigned)(sb + ab));
         bulk_g2s(stg, st_src, (unsigned)sb, bar);
         bulk_g2s(stg + sb, act_src, (unsigned)ab, bar);
       }
-      __syncwarp();
-      mbar_wait(bar, 0);
       st_src = reinterpret_cast<const float*>(stg);
       act_src = reinterpret_cast<const float*>(stg + sb);
     }
   }
+  const R* bt = stage_body_table<R, K>(M, reinterpret_cast<R*>(nb2_smem));
+  if (bar) {
+    __syncwarp();
+    mbar_wait(bar, 0);
+  }
+  NB2_CLK(0, 1);
 #pragma unroll 1
   for (int sg = 0; sg < NB2_FWD_STAGES; sg++) {
     if (sg == 0) {
@@ -142,6 +177,7 @@ k_step_fwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
     else if (sg == NB2_FWD_STAGES - 1) { if (nworlds > 0) nb2::fwd_store<R, ST>(M, scr0, next + wg * 2 * M.ndof, nworlds, li, 32); }
     else if (valid) nb2::world_forward_stage<R, ST>(M, scr, sv, (size_t)B, saved != nullptr, lane, sg, bt, nullptr, wi, (size_t)B);
     if ((sync_mask >> sg) & 1u) __syncwarp();
+    NB2_CLK(0, 2 + sg);
   }
 }
 
@@ -152,6 +188,7 @@ k_step_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
            float* __restrict__ gstate, float* __restrict__ gaction, float* __restrict__ ginertia, int words,
            int stage_saved, int accumulate_state, unsigned in_stage_off, const double* __restrict__ winertia, double* __restrict__ ginertia_acc) {
   extern __shared__ __align__(16) unsigned char nb2_smem[];
+  NB2_CLK(1, 0);
   constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
   const int li = threadIdx.x & 31, slot = li / K, lane = li % K;
   const int g0 = (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * WPW;
@@ -159,9 +196,31 @@ k_step_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
   const bool valid = slot < nworlds;
   const size_t wg = (size_t)w0 + (nworlds > 0 ? g0 : 0);
   const size_t w = wg + (valid ? slot : 0);
-  const R* bt = stage_body_table<R, K>(M, reinterpret_cast<R*>(nb2_smem));
   R* scr0 = reinterpret_cast<R*>(nb2_smem) + body_table_words<K>(M.nb) + (size_t)(threadIdx.x >> 5) * words * ST;
   R* scr = scr0 + slot;
+  // input rows (dL/dx', x, u) of the group through the bulk-copy staging buffer when they qualify; in flight, like the
+  // saved-stream burst below, while the block stages the body table (see k_step_fwd)
+  const float* g_src = gnext + wg * 2 * M.ndof;
+  const float* st_src = state + wg * 2 * M.ndof;
+  const float* act_src = action + wg * M.na;
+  unsigned long long* bar = nullptr;
+  if (nworlds > 0 && in_stage_off) {
+    const size_t sb = (size_t)nworlds * 2 * M.ndof * sizeof(float), ab = (size_t)nworlds * M.na * sizeof(float);
+    if (bulk_ok(g_src, sb) && bulk_ok(st_src, sb) && bulk_ok(act_src, ab)) {
+      unsigned char* stg = nb2_smem + in_stage_off + (size_t)(threadIdx.x >> 5) * staging_bytes<K>(4 * M.ndof + M.na);
+      bar = reinterpret_cast<unsigned long long*>(stg + staging_bytes<K>(4 * M.ndof + M.na) - 16);
+      if (li == 0) {
+        mbar_init(bar);
+        mbar_expect_tx(bar, (unsigned)(2 * sb + ab));
+        bulk_g2s(stg, g_src, (unsigned)sb, bar);
+        bulk_g2s(stg + sb, st_src, (unsigned)sb, bar);
+        bulk_g2s(stg + 2 * sb, act_src, (unsigned)ab, bar);
+      }
+      g_src = reinterpret_cast<const float*>(stg);
+      st_src = reinterpret_cast<const float*>(stg + sb);
+      act_src = reinterpret_cast<const float*>(stg + 2 * sb);
+    }
+  }
   // The sweeps walk the saved stream body by body, every access a dependent DRAM round trip.  When the launch leaves room
   // (small batches: the regime where latency is all that matters) each warp first pulls its group's rows of the stream
   // into shared memory with one burst of asynchronous 16-byte copies ([word][B] layout: the group's worlds are adjacent),
@@ -185,29 +244,12 @@ k_step_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
     svB = WPW;
   }
   constexpr unsigned sync_mask = (K > 1) ? NB2_BWD_SYNC_MASK : NB2_BWD_SYNC_MASK_1LANE;
-  // input rows (dL/dx', x, u) of the group through the bulk-copy staging buffer when they qualify (see k_step_fwd)
-  const float* g_src = gnext + wg * 2 * M.ndof;
-  const float* st_src = state + wg * 2 * M.ndof;
-  const float* act_src = action + wg * M.na;
-  if (nworlds > 0 && in_stage_off) {
-    const size_t sb = (size_t)nworlds * 2 * M.ndof * sizeof(float), ab = (size_t)nworlds * M.na * sizeof(float);
-    if (bulk_ok(g_src, sb) && bulk_ok(st_src, sb) && bulk_ok(act_src, ab)) {
-      unsigned char* stg = nb2_smem + in_stage_off + (size_t)(threadIdx.x >> 5) * staging_bytes<K>(4 * M.ndof + M.na);
-      unsigned long long* bar = reinterpret_cast<unsigned long long*>(stg + staging_bytes<K>(4 * M.ndof + M.na) - 16);
-      if (li == 0) {
-        mbar_init(bar);
-        mbar_expect_tx(bar, (unsigned)(2 * sb + ab));
-        bulk_g2s(stg, g_src, (unsigned)sb, bar);
-        bulk_g2s(stg + sb, st_src, (unsigned)sb, bar);
-        bulk_g2s(stg + 2 * sb, act_src, (unsigned)ab, bar);
-      }
-      __syncwarp();
-      mbar_wait(bar, 0);
-      g_src = reinterpret_cast<const float*>(stg);
-      st_src = reinterpret_cast<const float*>(stg + sb);
-      act_src = reinterpret_cast<const float*>(stg + 2 * sb);
-    }
+  const R* bt = stage_body_table<R, K>(M, reinterpret_cast<R*>(nb2_smem));
+  if (bar) {
+    __syncwarp();
+    mbar_wait(bar, 0);
   }
+  NB2_CLK(1, 1);
 #pragma unroll 1
   for (int sg = 0; sg < NB2_BWD_STAGES; sg++) {
     if (sg == 0) { if (nworlds > 0) nb2::bwd_load<R, ST, false>(M, scr0, st_src, act_src, g_src, nworlds, li, 32); }
@@ -217,6 +259,7 @@ k_step_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
                                                        (PW && winertia) ? winertia + w : nullptr, (size_t)B, (PW && ginertia_acc) ? ginertia_acc + w : nullptr);
     if (sg == 0 && stage_saved) asm volatile("cp.async.wait_group 0;" ::: "memory");
     if (((sync_mask >> sg) & 1u) || (sg == 0 && stage_saved)) __syncwarp();
+    NB2_CLK(1, 2 + sg);
   }
 }
 
@@ -1582,6 +1625,17 @@ int nb2_model_set_contact_capacity(nb2_model* m, int max_contacts_in_shared_memo
   return NB2_OK;
 }
 int nb2_model_contact_capacity(const nb2_model* m) { return (m && m->has_contacts) ? m->contact_mc : 0; }
+/* dev builds (-DNB2_STEP_CLOCKS): the stage clocks of the last k_step_fwd / k_step_bwd launches, [2][8][16] clock64() values
+   (see NB2_CLK); returns 0 when not compiled in */
+int nb2_step_clocks_read(long long* out64, int reset) {
+#ifdef NB2_STEP_CLOCKS
+  if (out64 && cudaMemcpyFromSymbol(out64, nb2_step_clk, sizeof(nb2_step_clk)) != cudaSuccess) return 0;
+  if (reset) { static const long long z[2 * NB2_CLK_WARPS * NB2_CLK_SLOTS] = {}; cudaMemcpyToSymbol(nb2_step_clk, z, sizeof(z)); }
+  return 1;
+#else
+  (void)out64; (void)reset; return 0;
+#endif
+}
 /* dev builds (-DNB2_CW_PROFILE): per-phase cycle counters of the fused contact kernels; returns 0 when not compiled in */
 int nb2_cw_profile_read(unsigned long long* out64, int reset) {
 #ifdef NB2_CW_PROFILE
