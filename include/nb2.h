@@ -279,6 +279,28 @@ int nb2_mass_matrix_backward(const nb2_model* m, int B, const void* pos, const d
 int nb2_inverse_mass_matrix_backward(const nb2_model* m, int B, const void* pos, const double* world_inertia, const void* Minv, const void* grad_Minv,
                                      void* workspace, void* grad_pos, double* grad_inertia, int precision, void* stream);
 
+/* World Jacobians of body points [B, k, 6, ndof] (row-major per (world, node)) at the positions pos [B, ndof]: columns in the step's
+ * velocity coordinates (free joints: body twist), J_e qdot = [omega_b ; d/dt p_e] in world axes for the point p_e = W_b T_e o_e of
+ * canonical body b = body[e] (-1: static, an all-zero block).  T_owner_from_node [12k] (host, fp64: R row-major, p) places each node on
+ * its body; offsets (device, arithmetic type): NULL (the nodes' origins), [k, 3] shared by the batch or [B, k, 3] (offsets_per_world = 1),
+ * in each node's frame.  Rows in the arithmetic type of `precision`; world_inertia and mass play no part.  One warp per (world, node).
+ * NB2_ERR_INVALID for k outside 1..NB2_MAX_JACOBIAN_NODES (32), a body outside -1..nb-1 or a model without dofs. */
+#define NB2_MAX_JACOBIAN_NODES 32
+int nb2_world_jacobian(const nb2_model* m, int B, const void* pos, int k, const int32_t* body, const double* T_owner_from_node, const void* offsets,
+                       int offsets_per_world, void* J, int precision, void* stream);
+/* VJP, L = <grad_J, J>: grad_pos [B, ndof] (written); grad_offsets NULL or [B, k, 3] (written, one row per world also for shared offsets:
+ * their gradient is the sum over the batch, left to the caller so that it stays deterministic).  One warp per world owns its rows. */
+int nb2_world_jacobian_backward(const nb2_model* m, int B, const void* pos, int k, const int32_t* body, const double* T_owner_from_node,
+                                const void* offsets, int offsets_per_world, const void* grad_J, void* grad_pos, void* grad_offsets, int precision,
+                                void* stream);
+/* Centre-of-mass Jacobian [B, 3, ndof] of the tree rooted at canonical body root_body (Skeleton::getCOMLinearJacobian; columns of other
+ * trees' dofs are 0); world_inertia as nb2_step_forward_pw (NULL: the model's).  Its VJP writes grad_pos [B, ndof] and, if not NULL,
+ * grad_inertia [10 * nb][B] fp64 (as nb2_inverse_dynamics_backward; zero for bodies of other trees).  One warp per world.
+ * NB2_ERR_INVALID for a root_body that is not a tree root or a model without dofs. */
+int nb2_com_jacobian(const nb2_model* m, int B, const void* pos, int root_body, const double* world_inertia, void* J, int precision, void* stream);
+int nb2_com_jacobian_backward(const nb2_model* m, int B, const void* pos, int root_body, const double* world_inertia, const void* grad_J,
+                              void* grad_pos, double* grad_inertia, int precision, void* stream);
+
 /* Batched boxed-LCP solves on the device: B independent problems, one warp each — the reference's pointer-style lower boundary
  * BoxedLcpSolver::solve(n, A, x, b, nub, lo, hi, findex, earlyTermination) (dart/constraint/BoxedLcpSolver.hpp:125-135) and the
  * solve chain of BoxedLcpConstraintSolver::solveLcp (BoxedLcpConstraintSolver.cpp:352-789).  Device pointers; problem w has dimension

@@ -18,6 +18,7 @@
 #include "../../include/nb2.h"
 #include "nb2_dyn.cuh"
 #include "nb2_mm.cuh"
+#include "nb2_jac.cuh"
 #include "nb2_cw.cuh"
 #include "nb2_host_model.h"
 
@@ -442,6 +443,96 @@ k_mm_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, const R* __restrict__ 
   nb2::mmb_free_q<R>(M, q, ws, lane, 32);
   __syncwarp();
   nb2::mmb_store_row<R>(M, ws, gpos + w * n, lane, 32);
+}
+
+// ---- world Jacobians (nb2_world_jacobian / nb2_com_jacobian / _backward, nb2_jac.cuh): ONE WARP PER ITEM, JAC_WPB items per block, each
+// warp's working set in its slice of the block's dynamic shared memory.  Forward items are (world, node) pairs for body points and
+// worlds for the COM; each item's block is staged whole, zeros included, and leaves in contiguous stores.  Backward items are worlds:
+// the warp owns the world's gradient row (deterministic sums, no atomics).  The node records are a second __grid_constant__ parameter.
+constexpr int JAC_WPB = 4;
+template <class R>
+__global__ void __launch_bounds__(32 * JAC_WPB)
+k_jac_point_fwd(const __grid_constant__ Nb2ModelDev<R> M, const __grid_constant__ nb2::JacNodes<R> N, int B, const R* __restrict__ pos,
+                const R* __restrict__ off, int off_pw, R* __restrict__ out) {
+  extern __shared__ __align__(16) unsigned char nb2_smem[];
+  const int lane = threadIdx.x & 31, n = M.ndof, words = nb2::jp_layout(n).total;
+  const size_t item = (size_t)blockIdx.x * JAC_WPB + (threadIdx.x >> 5);
+  if (item >= (size_t)B * N.k) return;
+  R* ws = reinterpret_cast<R*>(nb2_smem) + (threadIdx.x >> 5) * words;
+  const size_t w = item / N.k;
+  const int e = (int)(item - w * N.k), b = N.body[e];
+  const R* o = off ? off + ((off_pw ? w * N.k : 0) + e) * 3 : nullptr;
+  nb2::jp_zero<R>(M, ws, lane, 32);
+  __syncwarp();
+  nb2::jp_walk<R>(M, pos + w * n, b, N.T[e], o, ws, lane);
+  __syncwarp();
+  nb2::jp_columns<R>(M, b, ws, lane, 32);
+  __syncwarp();
+  mm_store_block<R>(out + item * 6 * n, ws, 6 * n, lane);
+}
+template <class R>
+__global__ void __launch_bounds__(32 * JAC_WPB)
+k_jac_point_bwd(const __grid_constant__ Nb2ModelDev<R> M, const __grid_constant__ nb2::JacNodes<R> N, int B, const R* __restrict__ pos,
+                const R* __restrict__ off, int off_pw, const R* __restrict__ grad, R* __restrict__ gpos, R* __restrict__ goff) {
+  extern __shared__ __align__(16) unsigned char nb2_smem[];
+  const int lane = threadIdx.x & 31, n = M.ndof;
+  const size_t w = (size_t)blockIdx.x * JAC_WPB + (threadIdx.x >> 5);
+  if (w >= (size_t)B) return;
+  R* ws = reinterpret_cast<R*>(nb2_smem) + (threadIdx.x >> 5) * ((nb2::jpb_layout(M.nb, n).total + 3) & ~3);
+  const R* q = pos + w * n;
+  nb2::jpb_init<R>(M, ws, lane, 32);
+#pragma unroll 1
+  for (int e = 0; e < N.k; e++) {
+    const int b = N.body[e];
+    __syncwarp();
+    nb2::jpb_walk<R>(M, q, b, N.T[e], off ? off + ((off_pw ? w * N.k : 0) + e) * 3 : nullptr, ws, lane);
+    __syncwarp();
+    nb2::jpb_terms<R>(M, b, grad + (w * N.k + e) * 6 * n, ws, lane, 32);
+    __syncwarp();
+    nb2::jpb_reduce<R>(M, q, b, ws, goff ? goff + (w * N.k + e) * 3 : nullptr, lane);
+  }
+  __syncwarp();
+  nb2::jpb_store_row<R>(M, ws, gpos + w * n, lane, 32);
+}
+template <class R>
+__global__ void __launch_bounds__(32 * JAC_WPB)
+k_jac_com_fwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int root, const R* __restrict__ pos, const double* __restrict__ winertia,
+              R* __restrict__ out) {
+  extern __shared__ __align__(16) unsigned char nb2_smem[];
+  const int lane = threadIdx.x & 31, n = M.ndof;
+  const nb2::JcLayout L = nb2::jc_layout(M.nb, n, false);
+  const size_t w = (size_t)blockIdx.x * JAC_WPB + (threadIdx.x >> 5);
+  if (w >= (size_t)B) return;
+  R* ws = reinterpret_cast<R*>(nb2_smem) + (threadIdx.x >> 5) * L.total;
+  nb2::jc_init<R>(M, pos + w * n, root, false, ws, lane, 32);
+  __syncwarp();
+  nb2::jc_moments<R>(M, root, winertia ? winertia + w : nullptr, (size_t)B, ws, lane, 32);
+  __syncwarp();
+  nb2::jc_columns<R>(M, root, ws, lane, 32);
+  __syncwarp();
+  mm_store_block<R>(out + w * 3 * n, ws + L.oCol, 3 * n, lane);
+}
+template <class R>
+__global__ void __launch_bounds__(32 * JAC_WPB)
+k_jac_com_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int root, const R* __restrict__ pos, const double* __restrict__ winertia,
+              const R* __restrict__ grad, R* __restrict__ gpos, double* __restrict__ ginertia) {
+  extern __shared__ __align__(16) unsigned char nb2_smem[];
+  const int lane = threadIdx.x & 31, n = M.ndof;
+  const size_t w = (size_t)blockIdx.x * JAC_WPB + (threadIdx.x >> 5);
+  if (w >= (size_t)B) return;
+  R* ws = reinterpret_cast<R*>(nb2_smem) + (threadIdx.x >> 5) * nb2::jc_layout(M.nb, n, true).total;
+  const R* q = pos + w * n;
+  nb2::jc_init<R>(M, q, root, true, ws, lane, 32);
+  __syncwarp();
+  nb2::jc_moments<R>(M, root, winertia ? winertia + w : nullptr, (size_t)B, ws, lane, 32);
+  __syncwarp();
+  nb2::jcb_terms<R>(M, root, grad + w * 3 * n, ws, lane, 32);
+  __syncwarp();
+  nb2::jcb_sums<R>(M, root, ws, lane);
+  __syncwarp();
+  nb2::jcb_grads<R>(M, q, root, ws, ginertia ? ginertia + w : nullptr, (size_t)B, lane, 32);
+  __syncwarp();
+  nb2::jcb_store_row<R>(M, ws, gpos + w * n, lane, 32);
 }
 
 // ---- fused step kernels of worlds WITH a contact stage (fp64): ONE WARP PER WORLD.
@@ -1912,6 +2003,114 @@ int nb2_inverse_mass_matrix_backward(const nb2_model* m, int B, const void* pos,
     using R = decltype(r);
     return launch_mm<R>(m, MM_INV_BWD, B, (const R*)pos, world_inertia, nullptr, (const R*)grad_Minv, (const R*)Minv, (R*)workspace, (R*)grad_pos,
                         grad_inertia, (cudaStream_t)stream, who);
+  });
+}
+}  // extern "C"
+
+// ---- world Jacobians: JAC_WPB warps per block, the shared memory sized from the model.  The node table is a kernel parameter next to
+// the model: the kernel-parameter space holds 32 764 bytes (CUDA 12.1+, sm_70+), Nb2ModelDev<double> takes about 17.5 kB of it, so
+// NB2_MAX_JACOBIAN_NODES = 32 nodes (3.2 kB in fp64) leave room for both without reaching the limit.
+static_assert(sizeof(Nb2ModelDev<double>) + sizeof(nb2::JacNodes<double>) + 64 <= 32764, "the node table does not fit the kernel parameters");
+template <class R>
+static int jac_nodes(const nb2_model* m, int k, const int32_t* body, const double* T, nb2::JacNodes<R>* N, const char* who) {
+  if (k < 1 || k > NB2_MAX_JACOBIAN_NODES || !body || !T) {
+    g_err = std::string(who) + ": k = " + std::to_string(k) + " is outside 1.." + std::to_string(NB2_MAX_JACOBIAN_NODES) + " (or no node arrays)";
+    return NB2_ERR_INVALID;
+  }
+  N->k = k;
+  for (int e = 0; e < k; e++) {
+    if (body[e] < -1 || body[e] >= m->mf.nb) { g_err = std::string(who) + ": node " + std::to_string(e) + " names body " + std::to_string(body[e]); return NB2_ERR_INVALID; }
+    N->body[e] = body[e];
+    for (int c = 0; c < 12; c++) N->T[e][c] = (R)T[12 * e + c];
+  }
+  for (int e = k; e < NB2_MAX_JACOBIAN_NODES; e++) { N->body[e] = -1; for (int c = 0; c < 12; c++) N->T[e][c] = R(0); }
+  return NB2_OK;
+}
+template <auto Kern> static int jac_launch_prep(size_t smem, const char* who) {
+  if (smem > (size_t)kMaxSmem) { g_err = std::string(who) + ": the model's working set does not fit in shared memory"; return NB2_ERR_INVALID; }
+  return smem > 48 * 1024 ? allow_max_smem<Kern>() : NB2_OK;
+}
+static unsigned jac_blocks(size_t items) { return (unsigned)((items + JAC_WPB - 1) / JAC_WPB); }
+template <class R>
+static int launch_jac_point(const nb2_model* m, int B, const R* pos, int k, const int32_t* body, const double* T, const R* off, int off_pw, R* J,
+                            const R* gJ, R* gpos, R* goff, cudaStream_t st, const char* who) {
+  nb2::JacNodes<R> N;
+  if (int rc = jac_nodes<R>(m, k, body, T, &N, who)) return rc;
+  const nb2_variant& v = m->variants[0];
+  int rc;
+  if (J) {
+    const size_t smem = (size_t)JAC_WPB * nb2::jp_layout(v.mf.ndof).total * sizeof(R);
+    if ((rc = jac_launch_prep<k_jac_point_fwd<R>>(smem, who))) return rc;
+    k_jac_point_fwd<R><<<jac_blocks((size_t)B * k), 32 * JAC_WPB, smem, st>>>(model_of<R>(v), N, B, pos, off, off_pw, J);
+  } else {
+    const size_t smem = (size_t)JAC_WPB * ((nb2::jpb_layout(v.mf.nb, v.mf.ndof).total + 3) & ~3) * sizeof(R);
+    if ((rc = jac_launch_prep<k_jac_point_bwd<R>>(smem, who))) return rc;
+    k_jac_point_bwd<R><<<jac_blocks((size_t)B), 32 * JAC_WPB, smem, st>>>(model_of<R>(v), N, B, pos, off, off_pw, gJ, gpos, goff);
+  }
+  g_launches++;
+  NB2_CUDA(cudaGetLastError());
+  return NB2_OK;
+}
+template <class R>
+static int launch_jac_com(const nb2_model* m, int B, const R* pos, int root, const double* wi, R* J, const R* gJ, R* gpos, double* gI, cudaStream_t st,
+                          const char* who) {
+  const nb2_variant& v = m->variants[0];
+  if (root < 0 || root >= v.mf.nb || v.mf.parent[root] >= 0) { g_err = std::string(who) + ": root_body " + std::to_string(root) + " is not a tree root"; return NB2_ERR_INVALID; }
+  const size_t smem = (size_t)JAC_WPB * nb2::jc_layout(v.mf.nb, v.mf.ndof, J == nullptr).total * sizeof(R);
+  int rc;
+  if (J) {
+    if ((rc = jac_launch_prep<k_jac_com_fwd<R>>(smem, who))) return rc;
+    k_jac_com_fwd<R><<<jac_blocks((size_t)B), 32 * JAC_WPB, smem, st>>>(model_of<R>(v), B, root, pos, wi, J);
+  } else {
+    if ((rc = jac_launch_prep<k_jac_com_bwd<R>>(smem, who))) return rc;
+    k_jac_com_bwd<R><<<jac_blocks((size_t)B), 32 * JAC_WPB, smem, st>>>(model_of<R>(v), B, root, pos, wi, gJ, gpos, gI);
+  }
+  g_launches++;
+  NB2_CUDA(cudaGetLastError());
+  return NB2_OK;
+}
+extern "C" {
+int nb2_world_jacobian(const nb2_model* m, int B, const void* pos, int k, const int32_t* body, const double* T_owner_from_node, const void* offsets,
+                       int offsets_per_world, void* J, int precision, void* stream) {
+  static const char* who = "nb2_world_jacobian";
+  if (int rc = mm_args_ok(m, B, pos && J, who)) return rc;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    if (B == 0) { nb2::JacNodes<R> N; return jac_nodes<R>(m, k, body, T_owner_from_node, &N, who); }
+    return launch_jac_point<R>(m, B, (const R*)pos, k, body, T_owner_from_node, (const R*)offsets, offsets_per_world, (R*)J, nullptr, nullptr, nullptr,
+                               (cudaStream_t)stream, who);
+  });
+}
+int nb2_world_jacobian_backward(const nb2_model* m, int B, const void* pos, int k, const int32_t* body, const double* T_owner_from_node,
+                                const void* offsets, int offsets_per_world, const void* grad_J, void* grad_pos, void* grad_offsets, int precision,
+                                void* stream) {
+  static const char* who = "nb2_world_jacobian_backward";
+  if (int rc = mm_args_ok(m, B, pos && grad_J && grad_pos, who)) return rc;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    if (B == 0) { nb2::JacNodes<R> N; return jac_nodes<R>(m, k, body, T_owner_from_node, &N, who); }
+    return launch_jac_point<R>(m, B, (const R*)pos, k, body, T_owner_from_node, (const R*)offsets, offsets_per_world, nullptr, (const R*)grad_J,
+                               (R*)grad_pos, (R*)grad_offsets, (cudaStream_t)stream, who);
+  });
+}
+int nb2_com_jacobian(const nb2_model* m, int B, const void* pos, int root_body, const double* world_inertia, void* J, int precision, void* stream) {
+  static const char* who = "nb2_com_jacobian";
+  if (int rc = mm_args_ok(m, B, pos && J, who)) return rc;
+  if (B == 0) return NB2_OK;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    return launch_jac_com<R>(m, B, (const R*)pos, root_body, world_inertia, (R*)J, nullptr, nullptr, nullptr, (cudaStream_t)stream, who);
+  });
+}
+int nb2_com_jacobian_backward(const nb2_model* m, int B, const void* pos, int root_body, const double* world_inertia, const void* grad_J,
+                              void* grad_pos, double* grad_inertia, int precision, void* stream) {
+  static const char* who = "nb2_com_jacobian_backward";
+  if (int rc = mm_args_ok(m, B, pos && grad_J && grad_pos, who)) return rc;
+  if (B == 0) return NB2_OK;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    return launch_jac_com<R>(m, B, (const R*)pos, root_body, world_inertia, nullptr, (const R*)grad_J, (R*)grad_pos, grad_inertia, (cudaStream_t)stream,
+                             who);
   });
 }
 int nb2_model_ndof(const nb2_model* m) { return m ? m->mf.ndof : -1; }

@@ -213,6 +213,29 @@ class DeviceModel:
         _cabi.check(_cabi.lib().nb2_inverse_mass_matrix_backward(self.handle, B, pos_ptr, wi_ptr, minv_ptr, gMinv_ptr, ws_ptr, gpos_ptr,
                                                                  ginertia_ptr, precision, stream))
 
+    def world_jacobian_device(self, B, pos_ptr, bodies, T12, off_ptr, off_per_world, out_ptr, stream, precision=FP32):
+        """J [B, k, 6, n] of body points (include/nb2.h nb2_world_jacobian); bodies [k] int32 and T12 [k, 12] fp64 are host arrays."""
+        b = np.ascontiguousarray(bodies, np.int32)
+        T = np.ascontiguousarray(T12, np.float64)
+        _cabi.check(_cabi.lib().nb2_world_jacobian(self.handle, B, pos_ptr, len(b), b.ctypes.data, T.ctypes.data, off_ptr, int(off_per_world),
+                                                   out_ptr, precision, stream))
+
+    def world_jacobian_backward_device(self, B, pos_ptr, bodies, T12, off_ptr, off_per_world, gJ_ptr, gpos_ptr, goff_ptr, stream, precision=FP32):
+        """VJP of world_jacobian_device; goff_ptr: optional [B, k, 3] buffer (one row per world, also for shared offsets)."""
+        b = np.ascontiguousarray(bodies, np.int32)
+        T = np.ascontiguousarray(T12, np.float64)
+        _cabi.check(_cabi.lib().nb2_world_jacobian_backward(self.handle, B, pos_ptr, len(b), b.ctypes.data, T.ctypes.data, off_ptr,
+                                                            int(off_per_world), gJ_ptr, gpos_ptr, goff_ptr, precision, stream))
+
+    def com_jacobian_device(self, B, pos_ptr, root, out_ptr, stream, precision=FP32, wi_ptr=None):
+        """J_com [B, 3, n] of the tree rooted at canonical body `root` (include/nb2.h nb2_com_jacobian)."""
+        _cabi.check(_cabi.lib().nb2_com_jacobian(self.handle, B, pos_ptr, int(root), wi_ptr, out_ptr, precision, stream))
+
+    def com_jacobian_backward_device(self, B, pos_ptr, root, gJ_ptr, gpos_ptr, stream, precision=FP32, ginertia_ptr=None, wi_ptr=None):
+        """VJP of com_jacobian_device; ginertia_ptr: optional [10*nb, B] float64 buffer receiving dL/d(inertia parameters)."""
+        _cabi.check(_cabi.lib().nb2_com_jacobian_backward(self.handle, B, pos_ptr, int(root), wi_ptr, gJ_ptr, gpos_ptr, ginertia_ptr, precision,
+                                                          stream))
+
     def contact_workspace_bytes(self, B):
         return int(_cabi.lib().nb2_contact_workspace_bytes(self.handle, B))
 

@@ -427,6 +427,32 @@ class Skeleton:
         """Skeleton::getInvMassMatrix: this skeleton's block of M^-1 (M is block-diagonal over skeletons)."""
         return self._mass_matrix_block(True)
 
+    def _jacobian_columns(self, who, node=None, offset=None):
+        from .world_jacobian import _single_world_com, _single_world_point
+
+        w, off = self._dof_offset_in_world()
+        if w is None:
+            raise ValueError(f"Skeleton.{who}: the skeleton is not part of a World")
+        J = _single_world_com(w, self, who) if node is None else _single_world_point(w, node, offset, who)
+        return J[:, off:off + self.getNumDofs()].copy()
+
+    def getWorldJacobian(self, node, offset=None):
+        """Skeleton::getWorldJacobian(node[, offset]) [6, n_skel]: [omega; velocity of the point] in world axes at the current positions,
+        the columns of this skeleton's dofs (numpy fp64; fp64 kernels, nimblephysics_b200.world_jacobian)."""
+        return self._jacobian_columns("getWorldJacobian()", node, offset)
+
+    def getLinearJacobian(self, node, offset=None):
+        """Skeleton::getLinearJacobian(node[, offset]) [3, n_skel]: the point's velocity rows of getWorldJacobian."""
+        return self._jacobian_columns("getLinearJacobian()", node, offset)[3:]
+
+    def getAngularJacobian(self, node):
+        """Skeleton::getAngularJacobian(node) [3, n_skel]: the angular-velocity rows of getWorldJacobian."""
+        return self._jacobian_columns("getAngularJacobian()", node)[:3]
+
+    def getCOMLinearJacobian(self):
+        """Skeleton::getCOMLinearJacobian() [3, n_skel] (numpy fp64; fp64 kernels, nimblephysics_b200.com_jacobian)."""
+        return self._jacobian_columns("getCOMLinearJacobian()")
+
     def setVelocity(self, i, v):
         w, off = self._dof_offset_in_world()
         if w is None:
