@@ -301,6 +301,21 @@ int nb2_com_jacobian(const nb2_model* m, int B, const void* pos, int root_body, 
 int nb2_com_jacobian_backward(const nb2_model* m, int B, const void* pos, int root_body, const double* world_inertia, const void* grad_J,
                               void* grad_pos, double* grad_inertia, int precision, void* stream);
 
+/* Time derivatives of the two Jacobians above at the states state [B, 2 ndof] = [q ; qdot] (Skeleton::getJacobianClassicDeriv,
+ * getCOMLinearJacobianDeriv): dJ = d/dt J(q(t)) along a motion through q with velocity qdot (free joints: the tangent of the step's
+ * position update), so that J qddot + dJ qdot is the acceleration.  Nodes, offsets, world_inertia, layouts and error cases as
+ * nb2_world_jacobian / nb2_com_jacobian; B = 0 only validates.  The VJPs write grad_state [B, 2 ndof] = [dL/dq ; dL/dqdot] and, as the
+ * Jacobians' VJPs, grad_offsets [B, k, 3] per world / grad_inertia [10 * nb][B].  Stateless, nothing allocated. */
+int nb2_world_jacobian_deriv(const nb2_model* m, int B, const void* state, int k, const int32_t* body, const double* T_owner_from_node,
+                             const void* offsets, int offsets_per_world, void* dJ, int precision, void* stream);
+int nb2_world_jacobian_deriv_backward(const nb2_model* m, int B, const void* state, int k, const int32_t* body, const double* T_owner_from_node,
+                                      const void* offsets, int offsets_per_world, const void* grad_dJ, void* grad_state, void* grad_offsets,
+                                      int precision, void* stream);
+int nb2_com_jacobian_deriv(const nb2_model* m, int B, const void* state, int root_body, const double* world_inertia, void* dJ, int precision,
+                           void* stream);
+int nb2_com_jacobian_deriv_backward(const nb2_model* m, int B, const void* state, int root_body, const double* world_inertia, const void* grad_dJ,
+                                    void* grad_state, double* grad_inertia, int precision, void* stream);
+
 /* Batched boxed-LCP solves on the device: B independent problems, one warp each — the reference's pointer-style lower boundary
  * BoxedLcpSolver::solve(n, A, x, b, nub, lo, hi, findex, earlyTermination) (dart/constraint/BoxedLcpSolver.hpp:125-135) and the
  * solve chain of BoxedLcpConstraintSolver::solveLcp (BoxedLcpConstraintSolver.cpp:352-789).  Device pointers; problem w has dimension

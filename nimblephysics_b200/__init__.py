@@ -9,13 +9,15 @@ from .inverse_dynamics import (inverse_dynamics, InverseDynamicsLayer, contact_i
                                multiple_contact_inverse_dynamics, MultipleContactInverseDynamicsLayer)
 from .mass_matrix import mass_matrix, inverse_mass_matrix, MassMatrixLayer, InverseMassMatrixLayer
 from .world_jacobian import world_jacobian, com_jacobian, WorldJacobianLayer, ComJacobianLayer
+from .world_jacobian import world_jacobian_deriv, com_jacobian_deriv, WorldJacobianDerivLayer, ComJacobianDerivLayer
 from .engine import DeviceModel, device_model_for
 from .rollout import rollout, rollout_fused, rollout_tape_bytes, multishot_rollout, shard_range, shard_batch, allreduce_sum_, sharded_trajectory_loss
 
 __all__ = ["World", "Skeleton", "BodyNode", "Joint", "Isometry3", "BoxShape", "SphereShape", "CapsuleShape",
            "loadWorld", "load_skeleton", "timestep", "TimestepLayer", "inverse_dynamics", "InverseDynamicsLayer", "contact_inverse_dynamics", "ContactInverseDynamicsLayer",
            "multiple_contact_inverse_dynamics", "MultipleContactInverseDynamicsLayer", "mass_matrix", "inverse_mass_matrix", "MassMatrixLayer", "InverseMassMatrixLayer",
-           "world_jacobian", "com_jacobian", "WorldJacobianLayer", "ComJacobianLayer", "rollout", "rollout_fused", "DeviceModel", "device_model_for", "RawModel", "CanonModel", "flatten_world", "compile_model", "mass_to_inertia"]
+           "world_jacobian", "com_jacobian", "WorldJacobianLayer", "ComJacobianLayer",
+           "world_jacobian_deriv", "com_jacobian_deriv", "WorldJacobianDerivLayer", "ComJacobianDerivLayer", "rollout", "rollout_fused", "DeviceModel", "device_model_for", "RawModel", "CanonModel", "flatten_world", "compile_model", "mass_to_inertia"]
 from .lcp import solve_boxed_lcp_batch
 from .jacobians import step_jacobians, state_jacobian, action_jacobian
 from .mapping import IKMapping, map_to_pos, map_to_vel

@@ -535,6 +535,104 @@ k_jac_com_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int root, const R
   nb2::jcb_store_row<R>(M, ws, gpos + w * n, lane, 32);
 }
 
+// ---- time derivatives of the world Jacobians (nb2_world_jacobian_deriv / nb2_com_jacobian_deriv / _backward, nb2_jac.cuh §6j): the
+// items, blocks and staging of the kernels above; the inputs are state rows [q ; qdot] and the backwards write [dL/dq ; dL/dqdot].
+template <class R>
+__global__ void __launch_bounds__(32 * JAC_WPB)
+k_jacd_point_fwd(const __grid_constant__ Nb2ModelDev<R> M, const __grid_constant__ nb2::JacNodes<R> N, int B, const R* __restrict__ state,
+                 const R* __restrict__ off, int off_pw, R* __restrict__ out) {
+  extern __shared__ __align__(16) unsigned char nb2_smem[];
+  const int lane = threadIdx.x & 31, n = M.ndof, words = nb2::jpd_layout(n).total;
+  const size_t item = (size_t)blockIdx.x * JAC_WPB + (threadIdx.x >> 5);
+  if (item >= (size_t)B * N.k) return;
+  R* ws = reinterpret_cast<R*>(nb2_smem) + (threadIdx.x >> 5) * words;
+  const size_t w = item / N.k;
+  const int e = (int)(item - w * N.k), b = N.body[e];
+  const R* q = state + w * 2 * n;
+  const R* o = off ? off + ((off_pw ? w * N.k : 0) + e) * 3 : nullptr;
+  nb2::jp_zero<R>(M, ws, lane, 32);
+  __syncwarp();
+  nb2::jpd_walk<R>(M, q, q + n, b, N.T[e], o, ws, lane);
+  __syncwarp();
+  nb2::jpd_columns<R>(M, b, ws, lane, 32);
+  __syncwarp();
+  mm_store_block<R>(out + item * 6 * n, ws, 6 * n, lane);
+}
+template <class R>
+__global__ void __launch_bounds__(32 * JAC_WPB)
+k_jacd_point_bwd(const __grid_constant__ Nb2ModelDev<R> M, const __grid_constant__ nb2::JacNodes<R> N, int B, const R* __restrict__ state,
+                 const R* __restrict__ off, int off_pw, const R* __restrict__ grad, R* __restrict__ gstate, R* __restrict__ goff) {
+  extern __shared__ __align__(16) unsigned char nb2_smem[];
+  const int lane = threadIdx.x & 31, n = M.ndof;
+  const size_t w = (size_t)blockIdx.x * JAC_WPB + (threadIdx.x >> 5);
+  if (w >= (size_t)B) return;
+  R* ws = reinterpret_cast<R*>(nb2_smem) + (threadIdx.x >> 5) * nb2::jpdb_layout(M.nb, n).total;
+  const R* q = state + w * 2 * n;
+  nb2::jpdb_init<R>(M, ws, lane, 32);
+#pragma unroll 1
+  for (int e = 0; e < N.k; e++) {
+    const int b = N.body[e];
+    __syncwarp();
+    nb2::jpdb_walk<R>(M, q, q + n, b, N.T[e], off ? off + ((off_pw ? w * N.k : 0) + e) * 3 : nullptr, ws, lane);
+    __syncwarp();
+    nb2::jpdb_terms<R>(M, b, grad + (w * N.k + e) * 6 * n, ws, lane, 32);
+    __syncwarp();
+    nb2::jpdb_reduce<R>(M, q, q + n, b, ws, goff ? goff + (w * N.k + e) * 3 : nullptr, lane);
+  }
+  __syncwarp();
+  nb2::jd_store_row<R>(n, ws + nb2::jpdb_layout(M.nb, n).oGq, gstate + w * 2 * n, lane, 32);
+}
+template <class R>
+__global__ void __launch_bounds__(32 * JAC_WPB)
+k_jacd_com_fwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int root, const R* __restrict__ state, const double* __restrict__ winertia,
+               R* __restrict__ out) {
+  extern __shared__ __align__(16) unsigned char nb2_smem[];
+  const int lane = threadIdx.x & 31, n = M.ndof;
+  const nb2::JcdLayout L = nb2::jcd_layout(M.nb, n, false);
+  const size_t w = (size_t)blockIdx.x * JAC_WPB + (threadIdx.x >> 5);
+  if (w >= (size_t)B) return;
+  R* ws = reinterpret_cast<R*>(nb2_smem) + (threadIdx.x >> 5) * L.total;
+  const R* q = state + w * 2 * n;
+  const double* wi = winertia ? winertia + w : nullptr;
+  nb2::jc_init<R>(M, q, root, false, ws, lane, 32);
+  __syncwarp();
+  nb2::jc_moments<R>(M, root, wi, (size_t)B, ws, lane, 32);
+  __syncwarp();
+  nb2::jcd_vel<R>(M, q + n, root, wi, (size_t)B, false, ws, lane);
+  __syncwarp();
+  nb2::jcd_columns<R>(M, root, ws, lane, 32);
+  __syncwarp();
+  mm_store_block<R>(out + w * 3 * n, ws + L.oCol, 3 * n, lane);
+}
+template <class R>
+__global__ void __launch_bounds__(32 * JAC_WPB)
+k_jacd_com_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int root, const R* __restrict__ state, const double* __restrict__ winertia,
+               const R* __restrict__ grad, R* __restrict__ gstate, double* __restrict__ ginertia) {
+  extern __shared__ __align__(16) unsigned char nb2_smem[];
+  const int lane = threadIdx.x & 31, n = M.ndof;
+  const nb2::JcdLayout L = nb2::jcd_layout(M.nb, n, true);
+  const size_t w = (size_t)blockIdx.x * JAC_WPB + (threadIdx.x >> 5);
+  if (w >= (size_t)B) return;
+  R* ws = reinterpret_cast<R*>(nb2_smem) + (threadIdx.x >> 5) * L.total;
+  const R* q = state + w * 2 * n;
+  const double* wi = winertia ? winertia + w : nullptr;
+  nb2::jcdb_init<R>(M, q, root, ws, lane, 32);
+  __syncwarp();
+  nb2::jc_moments<R>(M, root, wi, (size_t)B, ws, lane, 32);
+  __syncwarp();
+  nb2::jcd_vel<R>(M, q + n, root, wi, (size_t)B, true, ws, lane);
+  __syncwarp();
+  nb2::jcdb_terms<R>(M, root, grad + w * 3 * n, ws, lane, 32);
+  __syncwarp();
+  nb2::jcdb_prefix<R>(M, root, ws, lane);
+  __syncwarp();
+  nb2::jcdb_bodies<R>(M, root, wi, (size_t)B, ws, ginertia ? ginertia + w : nullptr, (size_t)B, lane, 32);
+  __syncwarp();
+  nb2::jcdb_reduce<R>(M, q, q + n, root, ws, lane);
+  __syncwarp();
+  nb2::jd_store_row<R>(n, ws + L.oGq, gstate + w * 2 * n, lane, 32);
+}
+
 // ---- fused step kernels of worlds WITH a contact stage (fp64): ONE WARP PER WORLD.
 // Forward: group load -> the three ABA sweeps on the first M.lanes lanes (trunk / limb schedule) -> the warp-cooperative contact /
 // boxed-LCP stage on all 32 lanes (nb2_cw.cuh) -> store.  Everything a world needs — ABA scratch, contact list, LCP matrix and its
@@ -2111,6 +2209,90 @@ int nb2_com_jacobian_backward(const nb2_model* m, int B, const void* pos, int ro
     using R = decltype(r);
     return launch_jac_com<R>(m, B, (const R*)pos, root_body, world_inertia, nullptr, (const R*)grad_J, (R*)grad_pos, grad_inertia, (cudaStream_t)stream,
                              who);
+  });
+}
+}  // extern "C"
+
+// ---- time derivatives of the world Jacobians: the launch shapes of the Jacobians above, the working sets of nb2_jac.cuh §6j
+template <class R>
+static int launch_jacd_point(const nb2_model* m, int B, const R* state, int k, const int32_t* body, const double* T, const R* off, int off_pw, R* dJ,
+                             const R* gJ, R* gstate, R* goff, cudaStream_t st, const char* who) {
+  nb2::JacNodes<R> N;
+  if (int rc = jac_nodes<R>(m, k, body, T, &N, who)) return rc;
+  if (B == 0) return NB2_OK;
+  const nb2_variant& v = m->variants[0];
+  int rc;
+  if (dJ) {
+    const size_t smem = (size_t)JAC_WPB * nb2::jpd_layout(v.mf.ndof).total * sizeof(R);
+    if ((rc = jac_launch_prep<k_jacd_point_fwd<R>>(smem, who))) return rc;
+    k_jacd_point_fwd<R><<<jac_blocks((size_t)B * k), 32 * JAC_WPB, smem, st>>>(model_of<R>(v), N, B, state, off, off_pw, dJ);
+  } else {
+    const size_t smem = (size_t)JAC_WPB * nb2::jpdb_layout(v.mf.nb, v.mf.ndof).total * sizeof(R);
+    if ((rc = jac_launch_prep<k_jacd_point_bwd<R>>(smem, who))) return rc;
+    k_jacd_point_bwd<R><<<jac_blocks((size_t)B), 32 * JAC_WPB, smem, st>>>(model_of<R>(v), N, B, state, off, off_pw, gJ, gstate, goff);
+  }
+  g_launches++;
+  NB2_CUDA(cudaGetLastError());
+  return NB2_OK;
+}
+template <class R>
+static int launch_jacd_com(const nb2_model* m, int B, const R* state, int root, const double* wi, R* dJ, const R* gJ, R* gstate, double* gI,
+                           cudaStream_t st, const char* who) {
+  const nb2_variant& v = m->variants[0];
+  if (root < 0 || root >= v.mf.nb || v.mf.parent[root] >= 0) { g_err = std::string(who) + ": root_body " + std::to_string(root) + " is not a tree root"; return NB2_ERR_INVALID; }
+  if (B == 0) return NB2_OK;
+  const size_t smem = (size_t)JAC_WPB * nb2::jcd_layout(v.mf.nb, v.mf.ndof, dJ == nullptr).total * sizeof(R);
+  int rc;
+  if (dJ) {
+    if ((rc = jac_launch_prep<k_jacd_com_fwd<R>>(smem, who))) return rc;
+    k_jacd_com_fwd<R><<<jac_blocks((size_t)B), 32 * JAC_WPB, smem, st>>>(model_of<R>(v), B, root, state, wi, dJ);
+  } else {
+    if ((rc = jac_launch_prep<k_jacd_com_bwd<R>>(smem, who))) return rc;
+    k_jacd_com_bwd<R><<<jac_blocks((size_t)B), 32 * JAC_WPB, smem, st>>>(model_of<R>(v), B, root, state, wi, gJ, gstate, gI);
+  }
+  g_launches++;
+  NB2_CUDA(cudaGetLastError());
+  return NB2_OK;
+}
+extern "C" {
+int nb2_world_jacobian_deriv(const nb2_model* m, int B, const void* state, int k, const int32_t* body, const double* T_owner_from_node,
+                             const void* offsets, int offsets_per_world, void* dJ, int precision, void* stream) {
+  static const char* who = "nb2_world_jacobian_deriv";
+  if (int rc = mm_args_ok(m, B, state && dJ, who)) return rc;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    return launch_jacd_point<R>(m, B, (const R*)state, k, body, T_owner_from_node, (const R*)offsets, offsets_per_world, (R*)dJ, nullptr, nullptr,
+                                nullptr, (cudaStream_t)stream, who);
+  });
+}
+int nb2_world_jacobian_deriv_backward(const nb2_model* m, int B, const void* state, int k, const int32_t* body, const double* T_owner_from_node,
+                                      const void* offsets, int offsets_per_world, const void* grad_dJ, void* grad_state, void* grad_offsets,
+                                      int precision, void* stream) {
+  static const char* who = "nb2_world_jacobian_deriv_backward";
+  if (int rc = mm_args_ok(m, B, state && grad_dJ && grad_state, who)) return rc;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    return launch_jacd_point<R>(m, B, (const R*)state, k, body, T_owner_from_node, (const R*)offsets, offsets_per_world, nullptr, (const R*)grad_dJ,
+                                (R*)grad_state, (R*)grad_offsets, (cudaStream_t)stream, who);
+  });
+}
+int nb2_com_jacobian_deriv(const nb2_model* m, int B, const void* state, int root_body, const double* world_inertia, void* dJ, int precision,
+                           void* stream) {
+  static const char* who = "nb2_com_jacobian_deriv";
+  if (int rc = mm_args_ok(m, B, state && dJ, who)) return rc;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    return launch_jacd_com<R>(m, B, (const R*)state, root_body, world_inertia, (R*)dJ, nullptr, nullptr, nullptr, (cudaStream_t)stream, who);
+  });
+}
+int nb2_com_jacobian_deriv_backward(const nb2_model* m, int B, const void* state, int root_body, const double* world_inertia, const void* grad_dJ,
+                                    void* grad_state, double* grad_inertia, int precision, void* stream) {
+  static const char* who = "nb2_com_jacobian_deriv_backward";
+  if (int rc = mm_args_ok(m, B, state && grad_dJ && grad_state, who)) return rc;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    return launch_jacd_com<R>(m, B, (const R*)state, root_body, world_inertia, nullptr, (const R*)grad_dJ, (R*)grad_state, grad_inertia,
+                              (cudaStream_t)stream, who);
   });
 }
 int nb2_model_ndof(const nb2_model* m) { return m ? m->mf.ndof : -1; }

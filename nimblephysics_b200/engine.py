@@ -236,6 +236,30 @@ class DeviceModel:
         _cabi.check(_cabi.lib().nb2_com_jacobian_backward(self.handle, B, pos_ptr, int(root), wi_ptr, gJ_ptr, gpos_ptr, ginertia_ptr, precision,
                                                           stream))
 
+    def world_jacobian_deriv_device(self, B, state_ptr, bodies, T12, off_ptr, off_per_world, out_ptr, stream, precision=FP32):
+        """Jdot [B, k, 6, n] of body points at states [B, 2n] (include/nb2.h nb2_world_jacobian_deriv); nodes as world_jacobian_device."""
+        b = np.ascontiguousarray(bodies, np.int32)
+        T = np.ascontiguousarray(T12, np.float64)
+        _cabi.check(_cabi.lib().nb2_world_jacobian_deriv(self.handle, B, state_ptr, len(b), b.ctypes.data, T.ctypes.data, off_ptr,
+                                                         int(off_per_world), out_ptr, precision, stream))
+
+    def world_jacobian_deriv_backward_device(self, B, state_ptr, bodies, T12, off_ptr, off_per_world, gJ_ptr, gstate_ptr, goff_ptr, stream,
+                                             precision=FP32):
+        """VJP of world_jacobian_deriv_device into gstate [B, 2n]; goff_ptr: optional [B, k, 3] buffer (one row per world)."""
+        b = np.ascontiguousarray(bodies, np.int32)
+        T = np.ascontiguousarray(T12, np.float64)
+        _cabi.check(_cabi.lib().nb2_world_jacobian_deriv_backward(self.handle, B, state_ptr, len(b), b.ctypes.data, T.ctypes.data, off_ptr,
+                                                                  int(off_per_world), gJ_ptr, gstate_ptr, goff_ptr, precision, stream))
+
+    def com_jacobian_deriv_device(self, B, state_ptr, root, out_ptr, stream, precision=FP32, wi_ptr=None):
+        """Jdot_com [B, 3, n] of the tree rooted at canonical body `root` at states [B, 2n] (include/nb2.h nb2_com_jacobian_deriv)."""
+        _cabi.check(_cabi.lib().nb2_com_jacobian_deriv(self.handle, B, state_ptr, int(root), wi_ptr, out_ptr, precision, stream))
+
+    def com_jacobian_deriv_backward_device(self, B, state_ptr, root, gJ_ptr, gstate_ptr, stream, precision=FP32, ginertia_ptr=None, wi_ptr=None):
+        """VJP of com_jacobian_deriv_device into gstate [B, 2n]; ginertia_ptr: optional [10*nb, B] float64 buffer."""
+        _cabi.check(_cabi.lib().nb2_com_jacobian_deriv_backward(self.handle, B, state_ptr, int(root), wi_ptr, gJ_ptr, gstate_ptr, ginertia_ptr,
+                                                                precision, stream))
+
     def contact_workspace_bytes(self, B):
         return int(_cabi.lib().nb2_contact_workspace_bytes(self.handle, B))
 

@@ -453,6 +453,32 @@ class Skeleton:
         """Skeleton::getCOMLinearJacobian() [3, n_skel] (numpy fp64; fp64 kernels, nimblephysics_b200.com_jacobian)."""
         return self._jacobian_columns("getCOMLinearJacobian()")
 
+    def _jacobian_deriv_columns(self, who, node=None, offset=None):
+        from .world_jacobian import _single_world_com_deriv, _single_world_point_deriv
+
+        w, off = self._dof_offset_in_world()
+        if w is None:
+            raise ValueError(f"Skeleton.{who}: the skeleton is not part of a World")
+        dJ = _single_world_com_deriv(w, self, who) if node is None else _single_world_point_deriv(w, node, offset, who)
+        return dJ[:, off:off + self.getNumDofs()].copy()
+
+    def getJacobianClassicDeriv(self, node, offset=None):
+        """Skeleton::getJacobianClassicDeriv(node[, offset]) [6, n_skel]: d/dt getWorldJacobian at the current positions and velocities,
+        the columns of this skeleton's dofs (numpy fp64; fp64 kernels, nimblephysics_b200.world_jacobian_deriv)."""
+        return self._jacobian_deriv_columns("getJacobianClassicDeriv()", node, offset)
+
+    def getLinearJacobianDeriv(self, node, offset=None):
+        """Skeleton::getLinearJacobianDeriv(node[, offset]) [3, n_skel]: the point's rows of getJacobianClassicDeriv."""
+        return self._jacobian_deriv_columns("getLinearJacobianDeriv()", node, offset)[3:]
+
+    def getAngularJacobianDeriv(self, node):
+        """Skeleton::getAngularJacobianDeriv(node) [3, n_skel]: the angular rows of getJacobianClassicDeriv."""
+        return self._jacobian_deriv_columns("getAngularJacobianDeriv()", node)[:3]
+
+    def getCOMLinearJacobianDeriv(self):
+        """Skeleton::getCOMLinearJacobianDeriv() [3, n_skel] (numpy fp64; fp64 kernels, nimblephysics_b200.com_jacobian_deriv)."""
+        return self._jacobian_deriv_columns("getCOMLinearJacobianDeriv()")
+
     def setVelocity(self, i, v):
         w, off = self._dof_offset_in_world()
         if w is None:

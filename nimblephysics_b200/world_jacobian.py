@@ -10,11 +10,14 @@ body twist (S = I6), the convention of ``mass_matrix``, so that e.g. J M^-1 J^T 
   exactly 0; a static node gets an all-zero block.
 - Centre of mass: J_com [3, n] maps qdot to the skeleton's COM velocity (``Skeleton::getCOMLinearVelocity``, the IKMapping COM entry).  It
   depends on the masses.
+- Time derivatives: ``world_jacobian_deriv(world, state, nodes, offsets=None)`` and ``com_jacobian_deriv(world, state, skeleton,
+  mass=None)`` return Jdot = d/dt J(q(t)) at states [q ; qdot], so that J qddot + Jdot qdot is the acceleration of the point (with the
+  body's angular acceleration) or of the COM.  Their gradients reach both halves of the state.
 
 Precision follows the positions' dtype: float64 tensors run the fp64 kernels with fp64 rows, anything else the fp32 ones.  Gradients flow
 to ``positions``, ``offsets`` and ``mass`` (1-D: ``setMasses``, shared by the batch, gradient summed; 2-D ``[B, m]``: per world, the
-World is left untouched).  The work is done by libnb2.so (include/nb2.h ``nb2_world_jacobian``, ``nb2_com_jacobian`` and their
-backwards).
+World is left untouched).  The work is done by libnb2.so (include/nb2.h ``nb2_world_jacobian``, ``nb2_com_jacobian``, their
+``_deriv`` counterparts and their backwards).
 """
 from __future__ import annotations
 
@@ -222,6 +225,156 @@ def com_jacobian(world, positions: torch.Tensor, skeleton, mass: Optional[torch.
     return ComJacobianLayer.apply(world, positions, root, mass)
 
 
+_WHO_D = "world_jacobian_deriv()"
+_WHO_COM_D = "com_jacobian_deriv()"
+
+
+def _check_state(world, state, who):
+    """ValueError unless the world has dofs and state is [2n] / [B, 2n] = [q ; qdot]; nothing touches the device."""
+    n = world.getNumDofs()
+    if n == 0:
+        raise ValueError(f"{who}: the world has no degrees of freedom")
+    if state.dim() not in (1, 2) or state.shape[-1] != 2 * n or (state.dim() == 2 and state.shape[0] == 0):
+        raise ValueError(f"{who}: state has shape {tuple(state.shape)}, expected [{2 * n}] or [B, {2 * n}] (= getStateSize())")
+
+
+class WorldJacobianDerivLayer(torch.autograd.Function):
+    """Jdot_e of the given nodes at states [q ; qdot].  Arguments as world_jacobian_deriv, the nodes already resolved (resolve_nodes)."""
+
+    @staticmethod
+    def forward(ctx, world, state, bodies, T12, offsets):
+        dm = device_model_for(world)
+        single = state.dim() == 1
+        s2 = state.detach().reshape(1, -1) if single else state.detach()
+        dev = _device(s2, _WHO_D)
+        rdt = torch.float64 if state.dtype == torch.float64 else torch.float32
+        sd = s2.to(device=dev, dtype=rdt).contiguous()
+        B, n, k = sd.shape[0], dm.ndof, len(bodies)
+        od = None if offsets is None else offsets.detach().to(device=dev, dtype=rdt).contiguous()
+        prec = FP64 if rdt == torch.float64 else FP32
+        with torch.cuda.device(dev):
+            out = torch.empty((B, k, 6, n), dtype=rdt, device=dev)
+            dm.world_jacobian_deriv_device(B, sd.data_ptr(), bodies, T12, _ptr(od), od is not None and od.dim() == 3, out.data_ptr(),
+                                           torch.cuda.current_stream().cuda_stream, prec)
+        ctx.save_for_backward(sd, od)
+        ctx.dm, ctx.bodies, ctx.T12, ctx.prec, ctx.single = dm, bodies, T12, prec, single
+        ctx.in_meta = (state.device, state.dtype)
+        ctx.off_like = offsets
+        out = out[0] if single else out
+        return out.to(device=state.device, dtype=state.dtype)
+
+    @staticmethod
+    def backward(ctx, grad):
+        sd, od = ctx.saved_tensors
+        dm, dev = ctx.dm, sd.device
+        B, n, k = sd.shape[0], dm.ndof, len(ctx.bodies)
+        g = grad.detach().reshape(B, k, 6, n).to(device=dev, dtype=sd.dtype).contiguous()
+        want_off = ctx.off_like is not None and ctx.needs_input_grad[4]
+        with torch.cuda.device(dev):
+            gs = torch.empty((B, 2 * n), dtype=sd.dtype, device=dev)
+            go = torch.empty((B, k, 3), dtype=sd.dtype, device=dev) if want_off else None
+            dm.world_jacobian_deriv_backward_device(B, sd.data_ptr(), ctx.bodies, ctx.T12, _ptr(od), od is not None and od.dim() == 3, g.data_ptr(),
+                                                    gs.data_ptr(), _ptr(go), torch.cuda.current_stream().cuda_stream, ctx.prec)
+        dev0, dt0 = ctx.in_meta
+        gs = (gs[0] if ctx.single else gs).to(device=dev0, dtype=dt0)
+        if want_off:
+            if ctx.off_like.dim() == 2:  # offsets shared by the batch: the worlds' gradients add up
+                go = go.sum(dim=0)
+            go = go.to(device=ctx.off_like.device, dtype=ctx.off_like.dtype)
+        return None, gs, None, None, go
+
+
+class ComJacobianDerivLayer(torch.autograd.Function):
+    """Jdot_com of the tree rooted at canonical body `root` at states [q ; qdot]; mass / world_inertia as ComJacobianLayer."""
+
+    @staticmethod
+    def forward(ctx, world, state, root, mass, world_inertia=None):
+        dm = set_shared_masses(world, mass, _WHO_COM_D) if mass is not None else device_model_for(world)
+        single = state.dim() == 1
+        s2 = state.detach().reshape(1, -1) if single else state.detach()
+        dev = _device(s2, _WHO_COM_D)
+        rdt = torch.float64 if state.dtype == torch.float64 else torch.float32
+        sd = s2.to(device=dev, dtype=rdt).contiguous()
+        B, n = sd.shape[0], dm.ndof
+        wi = _word_major_inertia(dm, world_inertia, B, dev)
+        prec = FP64 if rdt == torch.float64 else FP32
+        with torch.cuda.device(dev):
+            out = torch.empty((B, 3, n), dtype=rdt, device=dev)
+            dm.com_jacobian_deriv_device(B, sd.data_ptr(), root, out.data_ptr(), torch.cuda.current_stream().cuda_stream, prec, wi_ptr=_ptr(wi))
+        ctx.save_for_backward(sd, wi)
+        ctx.dm, ctx.root, ctx.prec, ctx.single = dm, root, prec, single
+        ctx.wi_grad = world_inertia is not None and ctx.needs_input_grad[4]
+        ctx.wi_like = world_inertia
+        ctx.mass_grad = mass is not None and ctx.needs_input_grad[3]
+        if ctx.mass_grad:
+            ctx.mass_P = shared_mass_jacobian(world, dm, dev)
+            ctx.mass_like = mass
+        ctx.in_meta = (state.device, state.dtype)
+        out = out[0] if single else out
+        return out.to(device=state.device, dtype=state.dtype)
+
+    @staticmethod
+    def backward(ctx, grad):
+        sd, wi = ctx.saved_tensors
+        dm, dev = ctx.dm, sd.device
+        B, n = sd.shape[0], dm.ndof
+        g = grad.detach().reshape(B, 3, n).to(device=dev, dtype=sd.dtype).contiguous()
+        with torch.cuda.device(dev):
+            gs = torch.empty((B, 2 * n), dtype=sd.dtype, device=dev)
+            gi = torch.empty((10 * dm.cm.nb, B), dtype=torch.float64, device=dev) if (ctx.mass_grad or ctx.wi_grad) else None
+            dm.com_jacobian_deriv_backward_device(B, sd.data_ptr(), ctx.root, g.data_ptr(), gs.data_ptr(), torch.cuda.current_stream().cuda_stream,
+                                                  ctx.prec, ginertia_ptr=_ptr(gi), wi_ptr=_ptr(wi))
+        gm = None
+        if ctx.mass_grad:  # one mass vector shared by the batch: the worlds' gradients add up
+            gm = (ctx.mass_P @ gi.sum(dim=1)).to(device=ctx.mass_like.device, dtype=ctx.mass_like.dtype)
+        gw = _inertia_grad(gi, ctx.wi_like) if ctx.wi_grad else None
+        dev0, dt0 = ctx.in_meta
+        gs = (gs[0] if ctx.single else gs).to(device=dev0, dtype=dt0)
+        return None, gs, None, gm, gw
+
+
+def world_jacobian_deriv(world, state: torch.Tensor, nodes: Sequence, offsets: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Jdot_e [B, k, 6, n] of the k BodyNodes `nodes` at states [B, 2n] = [q ; qdot] ([k, 6, n] for [2n]): d/dt J_e(q(t)) along a motion
+    through q with velocity qdot (free joints: Rdot = R [omega]x, pdot = R v, the step's position update), so that the acceleration
+    [alpha_b ; d2/dt2 p_e] is J_e qddot + Jdot_e qdot.  Linear in qdot; columns, nodes and offsets as world_jacobian.  Gradients flow to
+    the state (both halves) and the offsets.  ValueError before any device work as world_jacobian, for a state that is not [2n] / [B, 2n]."""
+    _check_state(world, state, _WHO_D)
+    nodes = list(nodes)
+    if not nodes or len(nodes) > MAX_NODES:
+        raise ValueError(f"{_WHO_D}: {len(nodes)} nodes given, expected 1 to {MAX_NODES}")
+    index = _body_index(world)
+    for node in nodes:
+        if id(node) not in index:
+            raise ValueError(f"{_WHO_D}: body node {getattr(node, 'name', node)!r} does not belong to this world")
+    k = len(nodes)
+    if offsets is not None:
+        ok = (offsets.dim() == 2 and tuple(offsets.shape) == (k, 3)) or (
+            offsets.dim() == 3 and state.dim() == 2 and tuple(offsets.shape) == (state.shape[0], k, 3))
+        if not ok:
+            want = f"[{k}, 3]" + (f" or [{state.shape[0]}, {k}, 3]" if state.dim() == 2 else "")
+            raise ValueError(f"{_WHO_D}: offsets has shape {tuple(offsets.shape)}, expected {want}")
+    bodies, T12 = resolve_nodes(world, nodes, _WHO_D)
+    return WorldJacobianDerivLayer.apply(world, state, bodies, T12, offsets)
+
+
+def com_jacobian_deriv(world, state: torch.Tensor, skeleton, mass: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Jdot_com [B, 3, n] of `skeleton` at states [B, 2n] = [q ; qdot] ([3, n] for [2n]), so that the COM's acceleration is
+    J_com qddot + Jdot_com qdot; mass and the ValueErrors as com_jacobian, for a state that is not [2n] / [B, 2n]."""
+    _check_state(world, state, _WHO_COM_D)
+    _check_skeleton(world, skeleton, _WHO_COM_D)
+    m = world.getMassDims()
+    if mass is not None:
+        if mass.dim() == 2 and state.dim() != 2:
+            raise ValueError(f"{_WHO_COM_D}: a [B, getMassDims()] mass needs [B, 2n] states")
+        want = (m,) if mass.dim() == 1 else (state.shape[0], m)
+        if mass.dim() not in (1, 2) or tuple(mass.shape) != want:
+            raise ValueError(f"{_WHO_COM_D}: mass has shape {tuple(mass.shape)}, expected [{m}] or [B, {m}] (= getMassDims())")
+    root = com_root(world, skeleton, _WHO_COM_D)
+    if mass is not None and mass.dim() == 2:
+        return ComJacobianDerivLayer.apply(world, state, root, None, per_world_inertia(world, state, mass, _WHO_COM_D))
+    return ComJacobianDerivLayer.apply(world, state, root, mass)
+
+
 def _current(world, who):
     q = torch.tensor(np.asarray(world.getPositions(), dtype=np.float64), dtype=torch.float64)
     if not torch.cuda.is_available():
@@ -241,3 +394,24 @@ def _single_world_com(world, skeleton, who):
     q = _current(world, who)
     with torch.no_grad():
         return com_jacobian(world, q, skeleton).cpu().numpy()
+
+
+def _current_state(world, who):
+    s = torch.tensor(np.concatenate([world.getPositions(), world.getVelocities()]).astype(np.float64), dtype=torch.float64)
+    if not torch.cuda.is_available():
+        raise RuntimeError(f"nimblephysics_b200.{who} needs a CUDA device; there is no CPU fallback")
+    return s.to("cuda")
+
+
+def _single_world_point_deriv(world, node, offset, who):
+    """[6, n] numpy fp64 Jdot of one node at the world's current state (fp64 kernels, B = 1)."""
+    s = _current_state(world, who)
+    off = None if offset is None else torch.as_tensor(np.asarray(offset, np.float64).reshape(1, 3), dtype=torch.float64, device=s.device)
+    with torch.no_grad():
+        return world_jacobian_deriv(world, s, [node], off)[0].cpu().numpy()
+
+
+def _single_world_com_deriv(world, skeleton, who):
+    s = _current_state(world, who)
+    with torch.no_grad():
+        return com_jacobian_deriv(world, s, skeleton).cpu().numpy()

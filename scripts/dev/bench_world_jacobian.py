@@ -86,6 +86,57 @@ def main():
         tp = np.median([timed(lambda: nb.world_jacobian(world, q0, nodes), 20) for _ in range(3)]) * 1e3
         tc = np.median([timed(lambda: nb.com_jacobian(world, q0, sk), 20) for _ in range(3)]) * 1e3
         print(f"  B={B} fp32 forward split: body points {tp:.1f} us, COM {tc:.1f} us", flush=True)
+        jdot_leg(world, raw, nodes, sk, s)
+
+
+def jdot_leg(world, raw, nodes, sk, s, h=5e-3):
+    """Jdot (world_jacobian_deriv + com_jacobian_deriv) forward and backward, the same-process J forward, and the central-difference
+    workaround (J at q (+) h qdot and q (+) -h qdot, positions prepared outside the timed window) with its fp32 error against the fp64
+    kernel; the fp32 kernel's own error beside it."""
+    from tests.test_world_jacobian_deriv import advance
+    from tests.util import rel_err
+
+    B, n = s.shape[0], raw.ndof
+    qp = np.stack([advance(raw, s[w, :n], s[w, n:], h) for w in range(B)])
+    qm = np.stack([advance(raw, s[w, :n], s[w, n:], -h) for w in range(B)])
+    ref = None
+    for dt in (torch.float64, torch.float32):
+        st = torch.tensor(s, dtype=dt, device="cuda")
+        q0, ps, ms = st[:, :n].contiguous(), torch.tensor(qp, dtype=dt, device="cuda"), torch.tensor(qm, dtype=dt, device="cuda")
+        G = torch.randn(B, len(nodes), 6, n, dtype=dt, device="cuda")
+        Gc = torch.randn(B, 3, n, dtype=dt, device="cuda")
+        sg = st.clone().requires_grad_(True)
+        dJ, dJc = nb.world_jacobian_deriv(world, sg, nodes), nb.com_jacobian_deriv(world, sg, sk)
+
+        def jd_fwd():
+            with torch.no_grad():
+                return nb.world_jacobian_deriv(world, st, nodes), nb.com_jacobian_deriv(world, st, sk)
+
+        def jd_bwd():
+            torch.autograd.grad([dJ, dJc], sg, [G, Gc], retain_graph=True)
+
+        def j_fwd():
+            with torch.no_grad():
+                nb.world_jacobian(world, q0, nodes)
+                nb.com_jacobian(world, q0, sk)
+
+        def cd_fwd():
+            with torch.no_grad():
+                return ((nb.world_jacobian(world, ps, nodes) - nb.world_jacobian(world, ms, nodes)) / (2 * h),
+                        (nb.com_jacobian(world, ps, sk) - nb.com_jacobian(world, ms, sk)) / (2 * h))
+
+        res = {k: [] for k in ("jd_fwd", "jd_bwd", "j_fwd", "cd_fwd")}
+        for _ in range(3):
+            for k, f in (("jd_fwd", jd_fwd), ("jd_bwd", jd_bwd), ("j_fwd", j_fwd), ("cd_fwd", cd_fwd)):
+                res[k].append(timed(f, 20))
+        med = {k: float(np.median(v)) * 1e3 for k, v in res.items()}
+        flat = lambda pair: torch.cat([pair[0].reshape(B, -1), pair[1].reshape(B, -1)], 1).double().cpu().numpy()
+        if ref is None:
+            ref = flat(jd_fwd())
+        err = f", fp32 error vs the fp64 kernel: kernel {rel_err(flat(jd_fwd()), ref):.1e}, central differences (h = {h}) " \
+              f"{rel_err(flat(cd_fwd()), ref):.1e}" if dt == torch.float32 else ""
+        print(f"  B={B} {str(dt)[6:]} Jdot ({len(nodes)} nodes + COM): fwd {med['jd_fwd']:.1f} us, bwd {med['jd_bwd']:.1f} us; "
+              f"J fwd {med['j_fwd']:.1f} us; central-difference workaround {med['cd_fwd']:.1f} us{err}", flush=True)
 
 
 if __name__ == "__main__":

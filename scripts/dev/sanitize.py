@@ -1,6 +1,6 @@
 """Small end-to-end run for compute-sanitizer (memcheck): contact-free fwd+bwd (device + pinned-host paths, partial groups),
 contact fwd+bwd, fused rollout, inverse dynamics, contact and multiple-contact inverse dynamics fwd+bwd, the mass matrix and its inverse fwd+bwd, the world and COM Jacobians
-fwd+bwd (both precisions, per-world masses and offsets, partial groups and partial blocks)."""
+and their time derivatives fwd+bwd (both precisions, per-world masses and offsets, partial groups and partial blocks)."""
 import sys
 import numpy as np, torch
 sys.path.insert(0, ".")
@@ -46,5 +46,7 @@ for B in (7, 203):
             f(mw, q, mass * torch.tensor(mw.getMasses(), device="cuda")).sum().backward()
         off = torch.zeros((B, 4, 3), device="cuda", dtype=dt, requires_grad=True)
         (nb.world_jacobian(mw, q, bodies, off).sum() + nb.com_jacobian(mw, q, mw.skeletons[0], mass * torch.tensor(mw.getMasses(), device="cuda")).sum()).backward()
+        (nb.world_jacobian_deriv(mw, st, bodies, off).sum()
+         + nb.com_jacobian_deriv(mw, st, mw.skeletons[0], mass * torch.tensor(mw.getMasses(), device="cuda")).sum()).backward()
 torch.cuda.synchronize()
 print("sanitize run finished")
