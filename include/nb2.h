@@ -197,8 +197,29 @@ int nb2_model_contact_capacity(const nb2_model* m);
  * SimpleFeatherstone::forwardDynamics(s_t* pos, s_t* vel, s_t* force, s_t* accel) (dart/dynamics/SimpleFeatherstone.hpp:61-65,
  * SimpleFeatherstone.cpp:26-138) and of Skeleton::computeForwardDynamics + getAccelerations.  fp64 device arrays [B, ndof]; the model's
  * gravity applies (the reference's test zeroes it, unittests/comprehensive/test_SimpleFeatherstone.cpp:34).  Requires the default action
- * space (every dof). */
+ * space (every dof).  It is one launch of the fp64 kernel of nb2_forward_dynamics_batch, reading pos and vel in place; a model whose fp64
+ * working set fits no schedule's shared memory (which nb2_forward_dynamics_batch refuses with NB2_ERR_UNSUPPORTED) runs the same stages one
+ * thread per world with scratch in global memory, allocated stream-ordered for the call. */
 int nb2_forward_dynamics(const nb2_model* m, int B, const double* pos, const double* vel, const double* force, double* accel, void* stream);
+
+/* Contact-free forward dynamics of B worlds: the acceleration accel [B, ndof] the contact-free step applies at state = [q ; qdot] under the
+ * generalised force tau [B, ndof]:
+ *     accel = M(q)^-1 ( tau - C(q, qdot) - g(q) - K (q - q0 + qdot dt) - D qdot )      (v+ = qdot + dt accel)
+ * It is the exact inverse of nb2_inverse_dynamics: nb2_inverse_dynamics(state, qdot + dt accel) returns tau up to rounding.  tau is per dof,
+ * not gathered through the action map, so any action space works; free joints use the step's conventions (body-twist velocities and
+ * accelerations, the 6-vector joint force in the joint frame).  Contacts, joint-limit rows, velocity and force limits are ignored: a model with
+ * collision pairs gets the accelerations of its trees, and no LCP cache is read or written.
+ * Rows in the arithmetic type (float with NB2_FP32, double with NB2_FP64), device memory, one row per world.  world_inertia (may be NULL):
+ * per-world inertia as for nb2_step_forward_pw.  saved (may be NULL when no backward will follow): nb2_saved_words_per_world(m) * B words of
+ * the arithmetic type, [words][B], the step's saved-stream layout.  Launch shapes and lane schedules are picked per call as for the step;
+ * NB2_ERR_UNSUPPORTED when no schedule's working set fits in shared memory (as for the step, e.g. a 64-body chain in fp64). */
+int nb2_forward_dynamics_batch(const nb2_model* m, int B, const void* state, const void* tau, const double* world_inertia, void* accel, void* saved,
+                               int precision, void* stream);
+/* Vector-Jacobian product of the same call, with the SAME state, world_inertia and saved stream.  grad_accel [B, ndof] -> grad_state [B, 2*ndof]
+ * = [dL/dq ; dL/dqdot], grad_tau [B, ndof] (all in the arithmetic type); grad_inertia (may be NULL): [10*nb][B] DOUBLES, dL/d(m, h, Ibar) of every
+ * canonical body and world, laid out as nb2_inverse_dynamics_backward's.  No clipping is applied.  Allocates nothing. */
+int nb2_forward_dynamics_backward(const nb2_model* m, int B, const void* state, const double* world_inertia, const void* saved, const void* grad_accel,
+                                  void* grad_state, void* grad_tau, double* grad_inertia, int precision, void* stream);
 
 /* Contact-free inverse dynamics of B worlds: the generalised force tau [B, ndof] for which the contact-free step started at
  * state = [q ; qdot] reaches the next velocity next_vel [B, ndof]:

@@ -182,6 +182,8 @@ def lib() -> ctypes.CDLL:
         L.nb2_step_forward_contact_host.argtypes = [vp, ctypes.c_int, vp, vp, vp, ctypes.c_int, ctypes.c_int, vp]
         L.nb2_step_backward_contact_host.argtypes = [vp, ctypes.c_int, vp, vp, vp, vp]
         L.nb2_forward_dynamics.argtypes = [vp, ctypes.c_int, vp, vp, vp, vp, vp]
+        L.nb2_forward_dynamics_batch.argtypes = [vp, ctypes.c_int, vp, vp, vp, vp, vp, ctypes.c_int, vp]
+        L.nb2_forward_dynamics_backward.argtypes = [vp, ctypes.c_int, vp, vp, vp, vp, vp, vp, vp, ctypes.c_int, vp]
         L.nb2_inverse_dynamics.argtypes = [vp, ctypes.c_int, vp, vp, vp, vp, vp, ctypes.c_int, vp]
         L.nb2_inverse_dynamics_backward.argtypes = [vp, ctypes.c_int, vp, vp, vp, vp, vp, vp, vp, vp, ctypes.c_int, vp]
         L.nb2_contact_inverse_dynamics.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp, vp, vp, ctypes.c_int, vp]

@@ -317,7 +317,8 @@ NB2_HD void fwd_pass2(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool sav
 
 }
 
-template <class R, int ST>
+// FD (forward dynamics, DESIGN.md §6k): no integration; qdd replaces the body's force words (oAct, spent after pass 2) for fd_store
+template <class R, int ST, bool FD = false>
 NB2_HD void fwd_pass3(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool save, int lo, int hi, const R* bt = nullptr) {
   const int nb = M.nb, n = M.ndof;
   const FwdLayout L = fwd_layout(nb, n, M.nslots, M.nfree);
@@ -341,8 +342,11 @@ NB2_HD void fwd_pass3(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool sav
       A = Ap;
       if (jt == NB2_JT_REV) { A.a.z += qdd; A.a.x += V.a.y * vq; A.a.y -= V.a.x * vq; A.l.x += V.l.y * vq; A.l.y -= V.l.x * vq; }
       else { A.l.z += qdd; A.l.x += V.a.y * vq; A.l.y -= V.a.x * vq; }
-      scr[(size_t)(L.oQ + o) * ST] = qv + vq * dt;   // q+, v+ replace q, v in the scratch (nothing reads this body's q, v again);
-      scr[(size_t)(L.oV + o) * ST] = vq + qdd * dt;  // fwd_store writes them out coalesced
+      if (FD) scr[(size_t)(L.oAct + o) * ST] = qdd;
+      else {
+        scr[(size_t)(L.oQ + o) * ST] = qv + vq * dt;   // q+, v+ replace q, v in the scratch (nothing reads this body's q, v again);
+        scr[(size_t)(L.oV + o) * ST] = vq + qdd * dt;  // fwd_store writes them out coalesced
+      }
       if (save) {
         R* s = sv + (size_t)(i * 21) * B;
         sv_st6(s, B, 0, tof(V)); sv_st6(s, B, 6, tof(A)); sv_st6(s, B, 12, tof(U));
@@ -357,6 +361,8 @@ NB2_HD void fwd_pass3(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool sav
       const V6<R> y = ld6<R, ST>(fr + 12 * ST);
       const V6<R> qdd = y - Ap;
       A = y + ad(V, Vj);
+      if (FD) st6<R, ST>(scr + (size_t)(L.oAct + o) * ST, qdd);
+      else {
       // FreeJoint::integratePositionsExplicit, identity-Jacobian branch (FreeJoint.cpp:922-929)
       const V3<R> phi = mk3<R>(q[0], q[ST], q[2 * ST]);
       const M3<R> Rq = expmap(phi);
@@ -367,6 +373,7 @@ NB2_HD void fwd_pass3(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool sav
       qo[0] = phin.x; qo[ST] = phin.y; qo[2 * ST] = phin.z; qo[3 * ST] = pn.x; qo[4 * ST] = pn.y; qo[5 * ST] = pn.z;
       vo[0] = Vj.a.x + qdd.a.x * dt; vo[ST] = Vj.a.y + qdd.a.y * dt; vo[2 * ST] = Vj.a.z + qdd.a.z * dt;
       vo[3 * ST] = Vj.l.x + qdd.l.x * dt; vo[4 * ST] = Vj.l.y + qdd.l.y * dt; vo[5 * ST] = Vj.l.z + qdd.l.z * dt;
+      }
       if (save) {
         R* s = sv + (size_t)(i * 21) * B;
         sv_st6(s, B, 0, tof(V)); sv_st6(s, B, 6, tof(A));
@@ -485,10 +492,11 @@ NB2_HD void fwd_store(const Nb2ModelDev<R>& M, const R* scr0, float* out0, int n
 //   6 accelerations + integration, limbs (every lane)        | barrier
 //   7 group store of q+, v+ (fwd_store)
 // With lanes == 1 everything is trunk.  Each pass body is instantiated once (the stage index is a run-time value).
+// FD: the forward-dynamics variant of pass 3 (fwd_pass3), which the FD kernels use with their own group load / store.
 #define NB2_FWD_STAGES 8
 #define NB2_FWD_SYNC_MASK 0x6Bu       /* after stages 0, 1, 3, 5, 6 */
 #define NB2_FWD_SYNC_MASK_1LANE 0x41u /* lanes == 1: only the group load / store exchange data between threads */
-template <class R, int ST>
+template <class R, int ST, bool FD = false>
 NB2_HD void world_forward_stage(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool save, int lane, int stage, const R* bt = nullptr, R* iinv_out = nullptr,
                                 const double* wi = nullptr, size_t wiB = 0) {
   const int pass = (stage + 1) >> 1;                          // stages 1..6 -> passes 1, 2, 3
@@ -500,7 +508,7 @@ NB2_HD void world_forward_stage(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B
     const int lo = trunk ? M.trunk_lo[r] : M.limb_lo[lane][r], hi = trunk ? M.trunk_hi[r] : M.limb_hi[lane][r];
     if (pass == 1) fwd_pass1<R, ST>(M, scr, lo, hi, bt);
     else if (pass == 2) fwd_pass2<R, ST>(M, scr, sv, B, save, lo, hi, bt, iinv_out, wi, wiB);
-    else fwd_pass3<R, ST>(M, scr, sv, B, save, lo, hi, bt);
+    else fwd_pass3<R, ST, FD>(M, scr, sv, B, save, lo, hi, bt);
   }
 }
 
@@ -1149,6 +1157,104 @@ NB2_HD void id_bwd_store(const Nb2ModelDev<R>& M, const R* scr0, R* gstate0, R* 
   const BwdLayout L = bwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
   id_rows_store<R, ST>(scr0, gstate0, 2 * M.ndof, M.magic_n2, L.oQb, nworlds, tid, nthr);  // oVb = oQb + n
   id_rows_store<R, ST>(scr0, gnext0, M.ndof, M.magic_n, L.oGQ, nworlds, tid, nthr);
+}
+
+// =====================================================================================================
+// forward dynamics (DESIGN.md §6k): qdd = M(q)^-1 (tau - C(q, qdot) - g(q) - K (q - q0 + qdot dt) - D qdot), the acceleration the
+// contact-free step applies (v+ = qdot + dt qdd), with tau per dof.  The step's three passes run unchanged on a model whose action map
+// is the identity (fd_identity_actions), so pass 2 reads tau[d] from action word d; pass 3's FD variant leaves qdd in those words.
+// Rows are in the arithmetic type R.  With `save` the forward writes the step's whole saved stream, which the backward reads.
+// =====================================================================================================
+template <class R> NB2_HD void fd_identity_actions(Nb2ModelDev<R>& M) {
+  M.na = M.ndof;
+  M.magic_na = M.magic_n;
+  for (int d = 0; d < M.ndof; d++) { M.action_map[d] = (int16_t)d; M.act_of_dof[d] = (int16_t)d; }
+}
+// rows [nworlds] of `width` words, `stride` words apart -> scratch words [base, base + width)
+template <class R, int ST>
+NB2_HD void fd_rows_load(R* scr0, const R* src, size_t stride, int width, unsigned magic, int base, int nworlds, int tid, int nthr) {
+  for (int idx = tid; idx < nworlds * width; idx += nthr) {
+    const int slot = (int)fast_div((unsigned)idx, magic), d = idx - slot * width;
+    scr0[(size_t)(base + d) * ST + slot] = src[(size_t)slot * stride + d];
+  }
+}
+// group load: q and qdot from rows `qs` / `vs` words apart (state rows [q ; qdot], or separate position and velocity arrays), tau [*, n]
+template <class R, int ST>
+NB2_HD void fd_load(const Nb2ModelDev<R>& M, R* scr0, const R* q0, size_t qs, const R* v0, size_t vs, const R* tau0, int nworlds, int tid, int nthr) {
+  const FwdLayout L = fwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
+  fd_rows_load<R, ST>(scr0, q0, qs, M.ndof, M.magic_n, L.oQ, nworlds, tid, nthr);
+  fd_rows_load<R, ST>(scr0, v0, vs, M.ndof, M.magic_n, L.oV, nworlds, tid, nthr);
+  id_rows_load<R, ST>(scr0, tau0, M.ndof, M.magic_n, L.oAct, nworlds, tid, nthr);
+}
+template <class R, int ST>
+NB2_HD void fd_store(const Nb2ModelDev<R>& M, const R* scr0, R* qdd0, int nworlds, int tid, int nthr) {
+  const FwdLayout L = fwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
+  id_rows_store<R, ST>(scr0, qdd0, M.ndof, M.magic_n, L.oAct, nworlds, tid, nthr);
+}
+
+// ---- backward (VJP): dFD/dx = -M^-1 dID_a/dx at a = qdd.  With g = dL/dqdd and lambda = M^-1 g (B1 / B2 of the step, seeded with g where
+// they read g_v', on the forward's U, psi and inverse articulated inertias) and W its field, bwd_B3 gives qbar = (dID_a/dq)^T lambda and
+// vbar = (dID_a/dqdot)^T lambda (spring and damping excluded), and
+//   dL/dtau = lambda ;  dL/dq = -(qbar + K lambda) ;  dL/dqdot = -(vbar + (D + dt K) lambda) ;
+//   dL/d(m, h, Ibar) of body i = -[ t(W, A) - t(ad(V, W), V) ]   (bwd_B3's identity without its -dt, formed here in the arithmetic type).
+// Scratch: bwd_layout.  No clipping, no action map, no integration adjoint.
+template <class R, int ST>
+NB2_HD void fd_bwd_assemble(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, int lo, int hi, double* gI, size_t gIB) {
+  const BwdLayout L = bwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
+  const R dt = M.dt;
+  for (int i = lo; i < hi; i++) {
+    const int jt = M.jtype[i], o = M.dof_off[i];
+    if (gI) {
+      const R* s = sv + (size_t)(i * 21) * B;
+      const V6<R> V = sv_ld6<R>(s, B, 0), A = sv_ld6<R>(s, B, 6), W = ld6<R, ST>(scr + (size_t)(L.oBody + 7 * i + 1) * ST);
+      V6<R> Y2;
+      Y2.a = cross_rn(V.a, W.a);
+      Y2.l = cross_rn(V.a, W.l) + cross_rn(V.l, W.a);
+      R t[10], t2[10];
+      inertia_param_form(W, A, t);
+      inertia_param_form(Y2, V, t2);
+      for (int k = 0; k < 10; k++) gI[(size_t)(10 * i + k) * gIB] = (double)(t2[k] - t[k]);
+    }
+    const int nd = (jt == NB2_JT_FREE) ? 6 : 1;
+    for (int k = 0; k < nd; k++) {
+      const int d = o + k;
+      const R lam = scr[(size_t)(L.oLam + d) * ST];
+      scr[(size_t)(L.oQb + d) * ST] = -(scr[(size_t)(L.oQb + d) * ST] + M.spring[d] * lam);
+      scr[(size_t)(L.oVb + d) * ST] = -(scr[(size_t)(L.oVb + d) * ST] + (M.damping[d] + dt * M.spring[d]) * lam);
+    }
+  }
+}
+// Stages and barriers of the step's backward (NB2_BWD_STAGES, NB2_BWD_SYNC_MASK): 0 group load | B1, B2, B3 as world_backward_stage |
+// fd_bwd_assemble in place of bwd_assemble | 9 group store
+template <class R, int ST>
+NB2_HD void fd_backward_stage(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, int lane, int stage, const R* bt, const double* wi, size_t wiB,
+                              double* gI, size_t gIB) {
+  const int pass = (stage == 1 || stage == 2) ? 1 : (stage == 3 || stage == 4) ? 2 : (stage == 5 || stage == 7) ? 3 : 4;
+  const bool trunk = (stage == 2) | (stage == 3) | (stage == 7) | (stage == 8);
+  if (trunk && lane != 0) return;
+  BwdContactData<ST> cd; cd.active = 0; cd.error = 0; cd.inj_of_body = nullptr;
+  const int nr = trunk ? M.trunk_n : M.limb_n[lane];
+  for (int rr = 0; rr < nr; rr++) {
+    const int r = (pass == 1 || pass == 3) ? nr - 1 - rr : rr;
+    const int lo = trunk ? M.trunk_lo[r] : M.limb_lo[lane][r], hi = trunk ? M.trunk_hi[r] : M.limb_hi[lane][r];
+    if (pass == 1) bwd_B1<R, ST, false>(M, scr, nullptr, sv, B, lo, hi, bt);
+    else if (pass == 2) bwd_B2<R, ST, false>(M, scr, nullptr, sv, B, lo, hi, bt);
+    else if (pass == 3) bwd_B3<R, ST, false>(M, scr, nullptr, sv, B, cd, lo, hi, nullptr, bt, B, wi, wiB, nullptr);
+    else fd_bwd_assemble<R, ST>(M, scr, sv, B, lo, hi, gI, gIB);
+  }
+}
+// group load of [q ; qdot] (oSt) and dL/dqdd (oGV, B1's g_v'); group store of [dL/dq ; dL/dqdot] (oQb, oVb adjacent) and dL/dtau (oLam)
+template <class R, int ST>
+NB2_HD void fd_bwd_load(const Nb2ModelDev<R>& M, R* scr0, const R* st0, const R* gqdd0, int nworlds, int tid, int nthr) {
+  const BwdLayout L = bwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
+  id_rows_load<R, ST>(scr0, st0, 2 * M.ndof, M.magic_n2, L.oSt, nworlds, tid, nthr);
+  id_rows_load<R, ST>(scr0, gqdd0, M.ndof, M.magic_n, L.oGV, nworlds, tid, nthr);
+}
+template <class R, int ST>
+NB2_HD void fd_bwd_store(const Nb2ModelDev<R>& M, const R* scr0, R* gstate0, R* gtau0, int nworlds, int tid, int nthr) {
+  const BwdLayout L = bwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
+  id_rows_store<R, ST>(scr0, gstate0, 2 * M.ndof, M.magic_n2, L.oQb, nworlds, tid, nthr);  // oVb = oQb + n
+  id_rows_store<R, ST>(scr0, gtau0, M.ndof, M.magic_n, L.oLam, nworlds, tid, nthr);
 }
 
 // =====================================================================================================

@@ -21,6 +21,8 @@
 #include "nb2_jac.cuh"
 #include "nb2_cw.cuh"
 #include "nb2_host_model.h"
+#include "nb2_coop.cuh"
+#include "nb2_fd.h"
 
 static thread_local std::string g_err;
 static std::atomic<long long> g_launches{0};
@@ -35,41 +37,6 @@ static std::atomic<long long> g_launches{0};
   } while (0)
 
 namespace {
-
-// K lanes cooperate on one world (K = M.lanes, compile-time here so that the scratch stride is a constant):
-// a warp holds 32/K worlds, thread t of the warp is lane t % K of world slot t / K.  Scratch is [word][slot] with an
-// odd stride (32/K + 1) so that the lanes of one world and the slots of one lane spread over the banks.
-template <int K> struct CoopShape {
-  static constexpr int WPW = 32 / K;                    // worlds per warp
-  static constexpr int ST = (K == 1) ? 32 : WPW + 1;    // scratch stride in words
-};
-
-// With several lanes per world the per-body constants are staged once per block in shared memory (see nb2_dyn.cuh xtree):
-// lanes of a warp sit on different bodies, which a constant-bank load would serialise.
-template <int K> __host__ __device__ constexpr int body_table_words(int nb) { return (K > 1) ? ((nb * NB2_BT_WORDS + 3) & ~3) : 0; }
-template <class R, int K>
-__device__ __forceinline__ const R* stage_body_table(const Nb2ModelDev<R>& M, R* tab) {
-  if constexpr (K == 1) return nullptr;
-  else {
-  // copied in 8-byte units: these loads have lane-varying addresses too, and the constant bank replays a load once per
-  // distinct address, so fp32 tables take half the replays of a word-by-word copy.  The 8-byte loads need M itself 8-byte
-  // aligned in the parameter space: every kernel that calls this takes M as its FIRST parameter (the parameter space starts
-  // aligned), keep it there.  The member offsets are checked below; an alignas(8) on Nb2ModelDev would also guarantee it, but it
-  // changes the code generated for most kernels that read the model (inverse dynamics, mass matrix, the one-lane step kernels).
-  using U = std::conditional_t<sizeof(R) == 4, float2, double>;
-  constexpr int XU = 12 * sizeof(R) / sizeof(U), IU = 10 * sizeof(R) / sizeof(U), BU = XU + IU;  // units per Xtree / inertia row
-  static_assert(offsetof(Nb2ModelDev<R>, Xtree) % sizeof(U) == 0 && offsetof(Nb2ModelDev<R>, inertia) % sizeof(U) == 0, "unaligned body tables");
-  const U* xs = reinterpret_cast<const U*>(&M.Xtree[0][0]);
-  const U* is = reinterpret_cast<const U*>(&M.inertia[0][0]);
-  U* t = reinterpret_cast<U*>(tab);
-  for (int k = threadIdx.x; k < M.nb * BU; k += blockDim.x) {
-    const int i = k / BU, j = k - i * BU;
-    t[k] = (j < XU) ? xs[i * XU + j] : is[i * IU + j - XU];
-  }
-  __syncthreads();
-  return tab;
-  }
-}
 
 // ---- bulk (TMA) staging of a group's input rows.  The rows of the worlds of one warp are contiguous in global memory, so
 // ONE thread hands each block of rows to the copy engine of the SM (cp.async.bulk, completion counted on an mbarrier) instead
@@ -1026,24 +993,6 @@ k_ik_backward(const __grid_constant__ Nb2ModelDev<double> M, int B, int nent, in
   }
 }
 
-// ---- pointer-style forward dynamics (row a5: SimpleFeatherstone::forwardDynamics(pos, vel, force, accel), dynamics/SimpleFeatherstone.hpp:61-65):
-// fp64 in, fp64 out, one thread per world with its scratch in global memory — a convenience / parity entry, not a hot path.
-__global__ void __launch_bounds__(64)
-k_forward_dynamics(const __grid_constant__ Nb2ModelDev<double> M, int B, int words, const double* __restrict__ pos, const double* __restrict__ vel,
-                   const double* __restrict__ force, double* __restrict__ accel, double* __restrict__ scratch) {
-  const int w = blockIdx.x * blockDim.x + threadIdx.x;
-  if (w >= B) return;
-  double* scr = scratch + (size_t)w * words;
-  const nb2::FwdLayout L = nb2::fwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
-  const int n = M.ndof;
-  for (int d = 0; d < n; d++) { scr[L.oQ + d] = pos[(size_t)w * n + d]; scr[L.oV + d] = vel[(size_t)w * n + d]; }
-  for (int a = 0; a < M.na; a++) scr[L.oAct + a] = force[(size_t)w * n + M.action_map[a]];
-  for (int sg = 1; sg < NB2_FWD_STAGES - 1; sg++)
-    for (int lane = 0; lane < M.lanes; lane++) nb2::world_forward_stage<double, 1>(M, scr, nullptr, 1, false, lane, sg);
-  // pass 3 left v + dt * qdd in the velocity slots
-  for (int d = 0; d < n; d++) accel[(size_t)w * n + d] = (scr[L.oV + d] - vel[(size_t)w * n + d]) / M.dt;
-}
-
 // ---- batched boxed-LCP entry (the reference's pointer-style lower boundary: BoxedLcpSolver::solve, constraint/BoxedLcpSolver.hpp:125-135,
 // and BoxedLcpConstraintSolver::solveLcp): one warp per problem, the same device code the contact stage runs.
 //   mode 0: Dantzig only (DantzigBoxedLcpSolver::solve -> dSolveLCP);  mode 1: the whole solve chain with classification
@@ -1106,17 +1055,30 @@ template <auto Kern> static int allow_max_smem() {
   return NB2_OK;
 }
 
+// the same for the forward-dynamics kernels of nb2_fd.cu, reached through their host stubs
+template <class R, int K> static int allow_max_smem_fd(int bwd) {
+  static std::atomic<bool> done[2][64];
+  int dev = 0; NB2_CUDA(cudaGetDevice(&dev));
+  if (!done[bwd][dev & 63].load(std::memory_order_acquire)) {
+    NB2_CUDA(cudaFuncSetAttribute(nb2_fd_kernel<R>(K, bwd), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
+    done[bwd][dev & 63].store(true, std::memory_order_release);
+  }
+  return NB2_OK;
+}
+
 // one sweep schedule of the model (same bodies, different lane count / slot assignment)
 struct LaunchShape { int warps_per_block = 0; int resident_warps = 0; };  // filled lazily from the occupancy API
 struct nb2_variant {
   Nb2ModelDev<float> mf;
   Nb2ModelDev<double> md;
+  Nb2ModelDev<float> mf_fd;  // mf / md with an identity action map (nb2::fd_identity_actions): the forward-dynamics kernels' model
+  Nb2ModelDev<double> md_fd;
   int fwd_words, bwd_words, id_bwd_words;
   int depth;                 // bodies on the sequential path of one sweep: |trunk| + longest lane
-  LaunchShape shape[4][2];   // [launch family: LF_*][fp32/fp64]
+  LaunchShape shape[6][2];   // [launch family: LF_*][fp32/fp64]
 };
 // launch families of the contact-free kernels (one LaunchShape each per variant and precision)
-enum { LF_STEP_FWD = 0, LF_STEP_BWD = 1, LF_ID_FWD = 2, LF_ID_BWD = 3 };
+enum { LF_STEP_FWD = 0, LF_STEP_BWD = 1, LF_ID_FWD = 2, LF_ID_BWD = 3, LF_FD_FWD = 4, LF_FD_BWD = 5 };
 
 struct nb2_model {
   Nb2ModelDev<float> mf;   // the schedule given to nb2_model_create (also what the contact kernels use)
@@ -1146,8 +1108,14 @@ struct nb2_model {
 template <class R> static const Nb2ModelDev<R>& model_of(const nb2_variant& v);
 template <> const Nb2ModelDev<float>& model_of<float>(const nb2_variant& v) { return v.mf; }
 template <> const Nb2ModelDev<double>& model_of<double>(const nb2_variant& v) { return v.md; }
+template <class R> static const Nb2ModelDev<R>& fd_model_of(const nb2_variant& v);
+template <> const Nb2ModelDev<float>& fd_model_of<float>(const nb2_variant& v) { return v.mf_fd; }
+template <> const Nb2ModelDev<double>& fd_model_of<double>(const nb2_variant& v) { return v.md_fd; }
 
 static void init_variant(nb2_variant& v) {
+  v.mf_fd = v.mf; v.md_fd = v.md;
+  nb2::fd_identity_actions(v.mf_fd);
+  nb2::fd_identity_actions(v.md_fd);
   v.fwd_words = nb2::fwd_layout(v.mf.nb, v.mf.ndof, v.mf.nslots, v.mf.nfree).total;
   v.bwd_words = nb2::bwd_layout(v.mf.nb, v.mf.ndof, v.mf.nslots, v.mf.nfree).total;
   v.id_bwd_words = nb2::id_bwd_words(v.mf.nb, v.mf.ndof, v.mf.nslots, v.mf.nfree);
@@ -1192,10 +1160,11 @@ template <class R, int K>
 static int prepare_k(nb2_variant& v, int dir) {  // dir: LF_*
   constexpr int ST = CoopShape<K>::ST;
   LaunchShape& sh = v.shape[dir][sizeof(R) == 8];
-  // the occupancy query sizes a step warp with its scratch AND its input-staging buffer, in both directions (the inverse-dynamics
-  // kernels stage nothing)
+  // the occupancy query sizes a step warp with its scratch AND its input-staging buffer, in both directions (the inverse- and
+  // forward-dynamics kernels stage nothing)
   const size_t scratch_and_staging =
-      dir == LF_ID_FWD ? (size_t)v.fwd_words * ST * sizeof(R) : dir == LF_ID_BWD ? (size_t)v.id_bwd_words * ST * sizeof(R) :
+      dir == LF_ID_FWD || dir == LF_FD_FWD ? (size_t)v.fwd_words * ST * sizeof(R) : dir == LF_ID_BWD ? (size_t)v.id_bwd_words * ST * sizeof(R) :
+      dir == LF_FD_BWD ? (size_t)v.bwd_words * ST * sizeof(R) :
       (size_t)(dir ? v.bwd_words : v.fwd_words) * ST * sizeof(R) +
           (dir ? staging_bytes<K>(4 * v.mf.ndof + v.mf.na) : staging_bytes<K>(2 * v.mf.ndof + v.mf.na));
   const size_t per_block = (size_t)body_table_words<K>(v.mf.nb) * sizeof(R) + 16;
@@ -1212,9 +1181,13 @@ static int prepare_k(nb2_variant& v, int dir) {  // dir: LF_*
   } else if (dir == LF_ID_FWD) {
     if ((rc = allow_max_smem<k_id_fwd<R, K>>())) return rc;
     if (!sh.warps_per_block) sh = occupancy_shape(k_id_fwd<R, K>, scratch_and_staging, per_block);
-  } else {
+  } else if (dir == LF_ID_BWD) {
     if ((rc = allow_max_smem<k_id_bwd<R, K>>())) return rc;
     if (!sh.warps_per_block) sh = occupancy_shape(k_id_bwd<R, K>, scratch_and_staging, per_block);
+  } else {  // the forward-dynamics kernels live in nb2_fd.cu
+    const int bwd = dir == LF_FD_BWD;
+    if ((rc = allow_max_smem_fd<R, K>(bwd))) return rc;
+    if (!sh.warps_per_block) sh = occupancy_shape(nb2_fd_kernel<R>(K, bwd), scratch_and_staging, per_block);
   }
   if (!sh.warps_per_block) { g_err = "no launch shape fits this model"; return NB2_ERR_UNSUPPORTED; }
   return NB2_OK;
@@ -1345,6 +1318,29 @@ static int launch_id(nb2_model* m, int B, int dir, const R* state, const R* next
   return with_lanes(pv->mf.lanes, [&](auto k) {
     return launch_id_k<R, decltype(k)::value>(*pv, m->sm_count, B, dir, state, next_vel, tau, saved, gtau, gstate, gnext, gI, wi, st);
   });
+}
+
+// ---- forward dynamics: the same launch family, dir LF_FD_FWD (q, qdot rows qs / vs words apart) or LF_FD_BWD
+template <class R, int K>
+static int launch_fd_k(const nb2_variant& v, int sm_count, int B, int dir, const FdArgs& a, cudaStream_t st) {
+  constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
+  const int words = dir == LF_FD_FWD ? v.fwd_words : v.bwd_words;
+  const size_t per_warp = (size_t)words * ST * sizeof(R);
+  const int total_warps = (B + WPW - 1) / WPW;
+  const int warps = block_warps(total_warps, sm_count, v.shape[dir][sizeof(R) == 8], per_warp);
+  const int blocks = (total_warps + warps - 1) / warps;
+  const size_t smem = per_warp * warps + (size_t)body_table_words<K>(v.mf.nb) * sizeof(R);
+  nb2_fd_launch<R>(K, dir == LF_FD_BWD, blocks, warps * 32, smem, st, fd_model_of<R>(v), B, a, words);
+  g_launches++;
+  NB2_CUDA(cudaGetLastError());
+  return NB2_OK;
+}
+template <class R>
+static int launch_fd(nb2_model* m, int B, int dir, const FdArgs& a, cudaStream_t st) {
+  nb2_variant* pv = nullptr;
+  int rc = pick_variant<R>(m, B, dir, &pv);
+  if (rc) return rc;
+  return with_lanes(pv->mf.lanes, [&](auto k) { return launch_fd_k<R, decltype(k)::value>(*pv, m->sm_count, B, dir, a, st); });
 }
 
 // ---- contact inverse dynamics: the chain of the contact body, checked (in range, under a free root), and the chain kernels' launch
@@ -1546,7 +1542,7 @@ int nb2_model_set_inertia(nb2_model* m, const double* inertia) {
       for (int k = 0; k < 10; k++) { md.inertia[i][k] = inertia[10 * i + k]; mf.inertia[i][k] = (float)inertia[10 * i + k]; }
   };
   put(m->mf, m->md);
-  for (auto& v : m->variants) put(v.mf, v.md);
+  for (auto& v : m->variants) { put(v.mf, v.md); put(v.mf_fd, v.md_fd); }
   return NB2_OK;
 }
 int nb2_model_set_lanes(nb2_model* m, int lanes) {
@@ -1884,15 +1880,43 @@ int nb2_forward_dynamics(const nb2_model* cm, int B, const double* pos, const do
   if (!m || B < 0 || !pos || !vel || !force || !accel) { g_err = "nb2_forward_dynamics: bad argument"; return NB2_ERR_INVALID; }
   if (m->md.na != m->md.ndof) { g_err = "nb2_forward_dynamics: the action space must cover every dof (force is given per dof)"; return NB2_ERR_INVALID; }
   if (B == 0) return NB2_OK;
-  const nb2_variant& v = m->variants[0];
-  double* scratch = nullptr;
-  cudaStream_t st = (cudaStream_t)stream;
-  NB2_CUDA(cudaMallocAsync((void**)&scratch, (size_t)B * v.fwd_words * sizeof(double), st));
-  k_forward_dynamics<<<(B + 63) / 64, 64, 0, st>>>(v.md, B, v.fwd_words, pos, vel, force, accel, scratch);
+  FdArgs a{};
+  a.q = pos; a.qs = m->md.ndof; a.v = vel; a.vs = m->md.ndof; a.tau = force; a.qdd = accel;
+  const int rc = launch_fd<double>(m, B, LF_FD_FWD, a, (cudaStream_t)stream);
+  if (rc != NB2_ERR_UNSUPPORTED) return rc;
+  // no schedule's fp64 working set fits in shared memory (e.g. a 64-body chain): the same stages with the scratch in global memory
+  g_err.clear();
+  NB2_CUDA(nb2_fd_forward_global(m->variants[0].md_fd, B, a, (cudaStream_t)stream));
   g_launches++;
-  NB2_CUDA(cudaGetLastError());
-  NB2_CUDA(cudaFreeAsync(scratch, st));
   return NB2_OK;
+}
+int nb2_forward_dynamics_batch(const nb2_model* cm, int B, const void* state, const void* tau, const double* world_inertia, void* accel, void* saved,
+                               int precision, void* stream) {
+  nb2_model* m = const_cast<nb2_model*>(cm);
+  if (!m || B < 0 || !state || !tau || !accel) { g_err = "nb2_forward_dynamics_batch: bad argument"; return NB2_ERR_INVALID; }
+  if (B == 0) return NB2_OK;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    const int n = m->md.ndof;
+    FdArgs a{};
+    a.q = state; a.qs = 2 * n; a.v = (const R*)state + n; a.vs = 2 * n; a.tau = tau; a.qdd = accel; a.saved = saved; a.wi = world_inertia;
+    return launch_fd<R>(m, B, LF_FD_FWD, a, (cudaStream_t)stream);
+  });
+}
+int nb2_forward_dynamics_backward(const nb2_model* cm, int B, const void* state, const double* world_inertia, const void* saved, const void* grad_accel,
+                                  void* grad_state, void* grad_tau, double* grad_inertia, int precision, void* stream) {
+  nb2_model* m = const_cast<nb2_model*>(cm);
+  if (!m || B < 0 || !state || !saved || !grad_accel || !grad_state || !grad_tau) {
+    g_err = "nb2_forward_dynamics_backward: bad argument"; return NB2_ERR_INVALID;
+  }
+  if (B == 0) return NB2_OK;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    FdArgs a{};
+    a.state = state; a.saved = const_cast<void*>(saved); a.gqdd = grad_accel; a.gstate = grad_state; a.gtau = grad_tau; a.gI = grad_inertia;
+    a.wi = world_inertia;
+    return launch_fd<R>(m, B, LF_FD_BWD, a, (cudaStream_t)stream);
+  });
 }
 int nb2_lcp_solve_batch(int B, int mcap, int mode, int early_termination, double fallback_cfm, const int32_t* m, const double* A, const double* b,
                         const double* lo, const double* hi, const int32_t* findex, const double* x0, double* x, int32_t* labels, int32_t* status,

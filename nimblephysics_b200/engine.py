@@ -135,7 +135,8 @@ class DeviceModel:
 
     def forward_dynamics(self, pos, vel, force):
         """q-ddot [B, n] (float64 CUDA tensors in and out): pointer-style ABA, no integration, no contact stage
-        (SimpleFeatherstone::forwardDynamics / Skeleton::computeForwardDynamics + getAccelerations)."""
+        (SimpleFeatherstone::forwardDynamics / Skeleton::computeForwardDynamics + getAccelerations); the fp64 kernel of
+        forward_dynamics_device.  Needs an action space covering every dof."""
         import torch
 
         dev = pos.device
@@ -156,6 +157,16 @@ class DeviceModel:
         """VJP of inverse_dynamics_device; ginertia_ptr: optional [10*nb, B] float64 buffer receiving dL/d(inertia parameters)."""
         _cabi.check(_cabi.lib().nb2_inverse_dynamics_backward(self.handle, B, state_ptr, None, wi_ptr, saved_ptr, gtau_ptr, gstate_ptr,
                                                               gnext_ptr, ginertia_ptr, precision, stream))
+
+    def forward_dynamics_device(self, B, state_ptr, tau_ptr, qdd_ptr, saved_ptr, stream, precision=FP32, wi_ptr=None):
+        """Contact-free forward dynamics (include/nb2.h nb2_forward_dynamics_batch): rows in the arithmetic type of `precision`, tau per dof."""
+        _cabi.check(_cabi.lib().nb2_forward_dynamics_batch(self.handle, B, state_ptr, tau_ptr, wi_ptr, qdd_ptr, saved_ptr, precision, stream))
+
+    def forward_dynamics_backward_device(self, B, state_ptr, saved_ptr, gqdd_ptr, gstate_ptr, gtau_ptr, stream, precision=FP32,
+                                         ginertia_ptr=None, wi_ptr=None):
+        """VJP of forward_dynamics_device; ginertia_ptr: optional [10*nb, B] float64 buffer receiving dL/d(inertia parameters)."""
+        _cabi.check(_cabi.lib().nb2_forward_dynamics_backward(self.handle, B, state_ptr, wi_ptr, saved_ptr, gqdd_ptr, gstate_ptr, gtau_ptr,
+                                                              ginertia_ptr, precision, stream))
 
     def contact_inverse_dynamics_device(self, B, body, state_ptr, next_vel_ptr, tau_ptr, wrench_ptr, saved_ptr, stream, precision=FP32,
                                         wi_ptr=None):

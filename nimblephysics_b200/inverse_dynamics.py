@@ -32,10 +32,20 @@ with k contact bodies c_1..c_k of one skeleton, J_i their Jacobians as above, p_
 so the deviation from each guess is measured as [torque about p_i; force], independently of where the world origin is.  The w_i sum to the
 one-body wrench; the objective and the wrench frame are this package's, the reference's could not be checked.
 
+Forward dynamics, ``forward_dynamics(world, state, tau, mass=None)`` (the reference's ``Skeleton::computeForwardDynamics()`` followed by
+``getAccelerations()``, and ``SimpleFeatherstone::forwardDynamics``), is the exact inverse of ``inverse_dynamics``: the acceleration the
+contact-free step applies under the per-dof force tau,
+
+    qdd = M(q)^-1 ( tau - C(q, qdot) - g(q) - K (q - q0 + qdot dt) - D qdot ) ,    so that  v+ = qdot + dt qdd  and
+    inverse_dynamics(world, state, qdot + dt qdd) = tau  up to rounding.
+
+tau is per dof like the output of ``inverse_dynamics`` (any action space works); contacts, joint-limit rows, velocity and force limits are
+ignored, no gradient clipping is applied and the LCP cache is never touched.  Gradients flow to ``state``, ``tau`` and ``mass``.
+
 Precision follows the state's dtype: float64 tensors run the fp64 kernels with fp64 rows, anything else the fp32 ones.
 Gradients flow to ``state``, ``next_vel`` and ``mass`` (1-D: ``setMasses``, shared by the batch, gradient summed; 2-D ``[B, m]``:
 per world, the World is left untouched).  The work is done by libnb2.so (include/nb2.h ``nb2_inverse_dynamics``,
-``nb2_contact_inverse_dynamics``, ``nb2_multiple_contact_inverse_dynamics``).
+``nb2_contact_inverse_dynamics``, ``nb2_multiple_contact_inverse_dynamics``, ``nb2_forward_dynamics_batch``).
 """
 from __future__ import annotations
 
@@ -50,24 +60,26 @@ from .world import FREE
 _WHO = "inverse_dynamics()"
 _WHO_CONTACT = "contact_inverse_dynamics()"
 _WHO_MULTI = "multiple_contact_inverse_dynamics()"
+_WHO_FD = "forward_dynamics()"
 MAX_CONTACT_BODIES = 4  # include/nb2.h NB2_MAX_CONTACT_BODIES
 
 
-def _check_rows(world, state, next_vel, who):
-    """ValueError unless state is [2n] / [B, 2n] and next_vel [n] / [B, n] (n = getNumDofs()); nothing touches the device."""
+def _check_rows(world, state, next_vel, who, second="next_vel"):
+    """ValueError unless state is [2n] / [B, 2n] and the second row argument (`second`: its name in the message) [n] / [B, n]
+    (n = getNumDofs()); nothing touches the device."""
     n = world.getNumDofs()
     if state.dim() not in (1, 2) or state.shape[-1] != 2 * n:
         raise ValueError(f"{who}: state has shape {tuple(state.shape)}, expected [..., {2 * n}] (= getStateSize())")
     if next_vel.dim() != state.dim() or tuple(next_vel.shape) != tuple(state.shape[:-1]) + (n,):
-        raise ValueError(f"{who}: next_vel has shape {tuple(next_vel.shape)}, expected the state's batch shape with {n} (= getNumDofs()) entries")
+        raise ValueError(f"{who}: {second} has shape {tuple(next_vel.shape)}, expected the state's batch shape with {n} (= getNumDofs()) entries")
 
 
-def _prepare(ctx, world, state, next_vel, mass, world_inertia, who):
-    """The shared front of both layers: mass handling, device rows in the arithmetic type and what backward needs of it on ctx.
+def _prepare(ctx, world, state, next_vel, mass, world_inertia, who, second="next_vel"):
+    """The shared front of the layers: mass handling, device rows in the arithmetic type and what backward needs of it on ctx.
     Returns (dm, sd, vd, wi, need_grad)."""
     if mass is not None and world_inertia is not None:
         raise ValueError(f"{who}: give either a mass vector or a per-world inertia table, not both")
-    _check_rows(world, state, next_vel, who)
+    _check_rows(world, state, next_vel, who, second)
     dm = set_shared_masses(world, mass, who) if mass is not None else device_model_for(world)
     single = state.dim() == 1
     s2 = state.detach().reshape(1, -1) if single else state.detach()
@@ -94,7 +106,7 @@ def _prepare(ctx, world, state, next_vel, mass, world_inertia, who):
 
 
 def _backward_buffers(ctx, dev, dtype):
-    """g_state, g_next_vel and (when a mass or inertia gradient is wanted) the [10*nb, B] fp64 inertia gradient."""
+    """g_state, the gradient of the second row argument and (when a mass or inertia gradient is wanted) the [10*nb, B] fp64 inertia gradient."""
     dm, B = ctx.dm, ctx.B
     gs = torch.empty((B, 2 * dm.ndof), dtype=dtype, device=dev)
     gn = torch.empty((B, dm.ndof), dtype=dtype, device=dev)
@@ -103,7 +115,7 @@ def _backward_buffers(ctx, dev, dtype):
 
 
 def _input_grads(ctx, gs, gn, gi):
-    """(g_state, g_next_vel, g_mass, g_world_inertia) in the inputs' shapes, dtypes and devices."""
+    """(g_state, g of the second row argument, g_mass, g_world_inertia) in the inputs' shapes, dtypes and devices."""
     gm = None
     if ctx.mass_grad:  # one mass vector shared by the batch: the worlds' gradients add up
         gm = (ctx.mass_P @ gi.sum(dim=1)).to(device=ctx.mass_like.device, dtype=ctx.mass_like.dtype)
@@ -146,6 +158,56 @@ class InverseDynamicsLayer(torch.autograd.Function):
             dm.inverse_dynamics_backward_device(B, sd.data_ptr(), saved.data_ptr(), g.data_ptr(), gs.data_ptr(), gn.data_ptr(),
                                                 torch.cuda.current_stream().cuda_stream, ctx.prec, ginertia_ptr=_ptr(gi), wi_ptr=_ptr(wi))
         return (None,) + _input_grads(ctx, gs, gn, gi)
+
+
+def _check_fd(world, state, tau):
+    """ValueError unless the world has dofs and state / tau are rows as inverse_dynamics takes them; nothing touches the device."""
+    if world.getNumDofs() == 0:
+        raise ValueError(f"{_WHO_FD}: the world has no degrees of freedom")
+    _check_rows(world, state, tau, _WHO_FD, "tau")
+
+
+class ForwardDynamicsLayer(torch.autograd.Function):
+    """Forward dynamics qdd = FD(state, tau); world_inertia as for InverseDynamicsLayer (exclusive with the 1-D `mass`)."""
+
+    @staticmethod
+    def forward(ctx, world, state, tau, mass, world_inertia=None):
+        _check_fd(world, state, tau)
+        dm, sd, td, wi, need_grad = _prepare(ctx, world, state, tau, mass, world_inertia, _WHO_FD, "tau")
+        B, dev = ctx.B, sd.device
+        with torch.cuda.device(dev):
+            qdd = torch.empty((B, dm.ndof), dtype=sd.dtype, device=dev)
+            saved = torch.empty((dm.saved_words, B), dtype=sd.dtype, device=dev) if need_grad else None
+            if B > 0:  # an empty batch has no rows to hand over (its data pointers may be NULL)
+                dm.forward_dynamics_device(B, sd.data_ptr(), td.data_ptr(), qdd.data_ptr(), _ptr(saved), torch.cuda.current_stream().cuda_stream,
+                                           ctx.prec, wi_ptr=_ptr(wi))
+        if need_grad:
+            ctx.save_for_backward(sd, saved, wi)
+        out = qdd[0] if ctx.single else qdd
+        return out.to(device=state.device, dtype=state.dtype)
+
+    @staticmethod
+    def backward(ctx, grad_qdd):
+        dm, B = ctx.dm, ctx.B
+        sd, saved, wi = ctx.saved_tensors
+        dev = sd.device
+        g = grad_qdd.detach().reshape(B, dm.ndof).to(device=dev, dtype=sd.dtype).contiguous()
+        with torch.cuda.device(dev):
+            gs, gt, gi = _backward_buffers(ctx, dev, sd.dtype)
+            if B > 0:
+                dm.forward_dynamics_backward_device(B, sd.data_ptr(), saved.data_ptr(), g.data_ptr(), gs.data_ptr(), gt.data_ptr(),
+                                                    torch.cuda.current_stream().cuda_stream, ctx.prec, ginertia_ptr=_ptr(gi), wi_ptr=_ptr(wi))
+        return (None,) + _input_grads(ctx, gs, gt, gi)
+
+
+def forward_dynamics(world, state: torch.Tensor, tau: torch.Tensor, mass: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Joint accelerations qdd [B, n] (or [n] for a 1-D state) of every world at `state` [B, 2n] under the per-dof generalised force `tau`
+    [B, n]: the acceleration the contact-free step applies, the exact inverse of inverse_dynamics (see the module docstring).  mass as for
+    inverse_dynamics.  ValueError before any device work for a wrong shape, a world without dofs or a mass of the wrong size."""
+    _check_fd(world, state, tau)
+    if mass is not None and mass.dim() == 2:
+        return ForwardDynamicsLayer.apply(world, state, tau, None, per_world_inertia(world, state, mass, _WHO_FD))
+    return ForwardDynamicsLayer.apply(world, state, tau, mass)
 
 
 def contact_body_index(world, body, who: str = _WHO_CONTACT) -> int:

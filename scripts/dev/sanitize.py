@@ -1,6 +1,7 @@
 """Small end-to-end run for compute-sanitizer (memcheck): contact-free fwd+bwd (device + pinned-host paths, partial groups),
 contact fwd+bwd, fused rollout, inverse dynamics, contact and multiple-contact inverse dynamics fwd+bwd, the mass matrix and its inverse fwd+bwd, the world and COM Jacobians
-and their time derivatives fwd+bwd (both precisions, per-world masses and offsets, partial groups and partial blocks)."""
+and their time derivatives fwd+bwd, forward dynamics fwd+bwd and the pointer-style forward dynamics (both precisions, per-world masses and
+offsets, partial groups and partial blocks)."""
 import sys
 import numpy as np, torch
 sys.path.insert(0, ".")
@@ -48,5 +49,9 @@ for B in (7, 203):
         (nb.world_jacobian(mw, q, bodies, off).sum() + nb.com_jacobian(mw, q, mw.skeletons[0], mass * torch.tensor(mw.getMasses(), device="cuda")).sum()).backward()
         (nb.world_jacobian_deriv(mw, st, bodies, off).sum()
          + nb.com_jacobian_deriv(mw, st, mw.skeletons[0], mass * torch.tensor(mw.getMasses(), device="cuda")).sum()).backward()
+        tau = (vn.detach() * 10).requires_grad_()
+        nb.forward_dynamics(mw, st, tau, mass * torch.tensor(mw.getMasses(), device="cuda")).sum().backward()
+    sd = torch.tensor(s, device="cuda", dtype=torch.float64)
+    nb.device_model_for(w).forward_dynamics(sd[:, :raw.ndof], sd[:, raw.ndof:], sd[:, raw.ndof:] * 10)
 torch.cuda.synchronize()
 print("sanitize run finished")

@@ -1,6 +1,6 @@
 """Dev: per-stage cycles of the contact-free step kernels (k_step_fwd / k_step_bwd), Atlas fp32, from a -DNB2_STEP_CLOCKS build.
 
-    nvcc <the flags of __graft_entry__.NVCC_FLAGS> -DNB2_STEP_CLOCKS -o build/clk/libnb2.so nimblephysics_b200/csrc/nb2_kernels.cu
+    nvcc <the flags of __graft_entry__.NVCC_FLAGS> -DNB2_STEP_CLOCKS -o build/clk/libnb2.so nimblephysics_b200/csrc/nb2_kernels.cu nimblephysics_b200/csrc/nb2_fd.cu
     NB2_LIB=build/clk/libnb2.so python scripts/dev/stage_clocks.py [--batch 4096] [--lanes 4 1] [--reps 20]
 
 Thread 0 of a few warps spread over the grid records clock64() at kernel entry, after the body-table / input staging and after
