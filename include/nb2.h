@@ -300,6 +300,20 @@ int nb2_mass_matrix_backward(const nb2_model* m, int B, const void* pos, const d
 int nb2_inverse_mass_matrix_backward(const nb2_model* m, int B, const void* pos, const double* world_inertia, const void* Minv, const void* grad_Minv,
                                      void* workspace, void* grad_pos, double* grad_inertia, int precision, void* stream);
 
+/* Dense Jacobians of nb2_inverse_dynamics and nb2_forward_dynamics_batch, with their outputs, in one launch.  J[w][i][j] = d out_i / d in_j,
+ * row-major [B, ndof, ndof] blocks in the arithmetic type of `precision`, device memory; state, next_vel, tau and world_inertia as for the
+ * two calls.  Row i is the call's vector-Jacobian product with the seed e_i (free joints: body-twist velocity columns, position columns
+ * through the six stored coordinates), so the blocks equal what the _backward entries give row by row:
+ *   inverse dynamics  tau [B, ndof];  J_q = dtau/dq,  J_qdot = dtau/dqdot (next_vel held fixed),  J_next_vel = dtau/dnext_vel = M / dt
+ *   forward dynamics  accel [B, ndof];  J_q = daccel/dq,  J_qdot = daccel/dqdot,  J_tau = daccel/dtau = M^-1
+ * Contacts, limits and clipping are ignored; no LCP cache is read or written.  One warp per world, the working set in shared memory, which
+ * every model of the mass-matrix envelope fits in both precisions (a 64-body chain in fp64 included).  Nothing is allocated.
+ * NB2_ERR_INVALID for a model without dofs or a bad argument; NB2_ERR_UNSUPPORTED when the working set does not fit shared memory. */
+int nb2_inverse_dynamics_jacobians(const nb2_model* m, int B, const void* state, const void* next_vel, const double* world_inertia, void* tau, void* J_q,
+                                   void* J_qdot, void* J_next_vel, int precision, void* stream);
+int nb2_forward_dynamics_jacobians(const nb2_model* m, int B, const void* state, const void* tau, const double* world_inertia, void* accel, void* J_q,
+                                   void* J_qdot, void* J_tau, int precision, void* stream);
+
 /* World Jacobians of body points [B, k, 6, ndof] (row-major per (world, node)) at the positions pos [B, ndof]: columns in the step's
  * velocity coordinates (free joints: body twist), J_e qdot = [omega_b ; d/dt p_e] in world axes for the point p_e = W_b T_e o_e of
  * canonical body b = body[e] (-1: static, an all-zero block).  T_owner_from_node [12k] (host, fp64: R row-major, p) places each node on

@@ -184,6 +184,8 @@ def lib() -> ctypes.CDLL:
         L.nb2_forward_dynamics.argtypes = [vp, ctypes.c_int, vp, vp, vp, vp, vp]
         L.nb2_forward_dynamics_batch.argtypes = [vp, ctypes.c_int, vp, vp, vp, vp, vp, ctypes.c_int, vp]
         L.nb2_forward_dynamics_backward.argtypes = [vp, ctypes.c_int, vp, vp, vp, vp, vp, vp, vp, ctypes.c_int, vp]
+        L.nb2_inverse_dynamics_jacobians.argtypes = [vp, ctypes.c_int] + [vp] * 7 + [ctypes.c_int, vp]
+        L.nb2_forward_dynamics_jacobians.argtypes = [vp, ctypes.c_int] + [vp] * 7 + [ctypes.c_int, vp]
         L.nb2_inverse_dynamics.argtypes = [vp, ctypes.c_int, vp, vp, vp, vp, vp, ctypes.c_int, vp]
         L.nb2_inverse_dynamics_backward.argtypes = [vp, ctypes.c_int, vp, vp, vp, vp, vp, vp, vp, vp, ctypes.c_int, vp]
         L.nb2_contact_inverse_dynamics.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp, vp, vp, ctypes.c_int, vp]

@@ -22,6 +22,7 @@
 #include "nb2_cw.cuh"
 #include "nb2_host_model.h"
 #include "nb2_coop.cuh"
+#include "nb2_djac.h"
 #include "nb2_fd.h"
 
 static thread_local std::string g_err;
@@ -2126,6 +2127,36 @@ int nb2_inverse_mass_matrix_backward(const nb2_model* m, int B, const void* pos,
     return launch_mm<R>(m, MM_INV_BWD, B, (const R*)pos, world_inertia, nullptr, (const R*)grad_Minv, (const R*)Minv, (R*)workspace, (R*)grad_pos,
                         grad_inertia, (cudaStream_t)stream, who);
   });
+}
+}  // extern "C"
+
+// ---- dense Jacobians of inverse / forward dynamics (nb2_djac.cu): one warp per world on the create-time schedule, as many row slots as the
+// working set leaves room for in shared memory
+static int launch_dj(const nb2_model* m, bool fd, int B, const void* state, const void* x, const double* wi, void* out, void* J1, void* J2, void* J3,
+                     int precision, void* stream, const char* who) {
+  if (!m || B < 0 || !state || !x || !out || !J1 || !J2 || !J3) { g_err = std::string(who) + ": bad argument"; return NB2_ERR_INVALID; }
+  if (m->mf.ndof == 0) { g_err = std::string(who) + ": the model has no dofs"; return NB2_ERR_INVALID; }
+  if (B == 0) return NB2_OK;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    const nb2_variant& v = m->variants[0];
+    const Nb2ModelDev<R>& M = fd ? fd_model_of<R>(v) : model_of<R>(v);
+    size_t smem = 0;
+    const int slots = nb2_dj_slots(M.nb, M.ndof, M.nslots, M.nfree, fd, sizeof(R), kMaxSmem, &smem);
+    if (!slots) { g_err = std::string(who) + ": the model's working set does not fit in shared memory"; return NB2_ERR_UNSUPPORTED; }
+    NB2_CUDA(nb2_dj_launch<R>(fd, slots, smem, (cudaStream_t)stream, M, B, (const R*)state, (const R*)x, wi, (R*)out, (R*)J1, (R*)J2, (R*)J3));
+    g_launches++;
+    return NB2_OK;
+  });
+}
+extern "C" {
+int nb2_inverse_dynamics_jacobians(const nb2_model* m, int B, const void* state, const void* next_vel, const double* world_inertia, void* tau, void* J_q,
+                                   void* J_qdot, void* J_next_vel, int precision, void* stream) {
+  return launch_dj(m, false, B, state, next_vel, world_inertia, tau, J_q, J_qdot, J_next_vel, precision, stream, "nb2_inverse_dynamics_jacobians");
+}
+int nb2_forward_dynamics_jacobians(const nb2_model* m, int B, const void* state, const void* tau, const double* world_inertia, void* accel, void* J_q,
+                                   void* J_qdot, void* J_tau, int precision, void* stream) {
+  return launch_dj(m, true, B, state, tau, world_inertia, accel, J_q, J_qdot, J_tau, precision, stream, "nb2_forward_dynamics_jacobians");
 }
 }  // extern "C"
 

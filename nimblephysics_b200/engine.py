@@ -168,6 +168,16 @@ class DeviceModel:
         _cabi.check(_cabi.lib().nb2_forward_dynamics_backward(self.handle, B, state_ptr, wi_ptr, saved_ptr, gqdd_ptr, gstate_ptr, gtau_ptr,
                                                               ginertia_ptr, precision, stream))
 
+    def inverse_dynamics_jacobians_device(self, B, state_ptr, next_vel_ptr, tau_ptr, jq_ptr, jqdot_ptr, jnext_ptr, stream, precision=FP32, wi_ptr=None):
+        """tau and its dense Jacobians [B, n, n] d/dq, d/dqdot, d/dnext_vel (include/nb2.h nb2_inverse_dynamics_jacobians)."""
+        _cabi.check(_cabi.lib().nb2_inverse_dynamics_jacobians(self.handle, B, state_ptr, next_vel_ptr, wi_ptr, tau_ptr, jq_ptr, jqdot_ptr, jnext_ptr,
+                                                               precision, stream))
+
+    def forward_dynamics_jacobians_device(self, B, state_ptr, tau_ptr, qdd_ptr, jq_ptr, jqdot_ptr, jtau_ptr, stream, precision=FP32, wi_ptr=None):
+        """qdd and its dense Jacobians [B, n, n] d/dq, d/dqdot, d/dtau (include/nb2.h nb2_forward_dynamics_jacobians)."""
+        _cabi.check(_cabi.lib().nb2_forward_dynamics_jacobians(self.handle, B, state_ptr, tau_ptr, wi_ptr, qdd_ptr, jq_ptr, jqdot_ptr, jtau_ptr,
+                                                               precision, stream))
+
     def contact_inverse_dynamics_device(self, B, body, state_ptr, next_vel_ptr, tau_ptr, wrench_ptr, saved_ptr, stream, precision=FP32,
                                         wi_ptr=None):
         """Contact inverse dynamics (include/nb2.h nb2_contact_inverse_dynamics); body: canonical index of the contact body."""

@@ -46,6 +46,10 @@ Precision follows the state's dtype: float64 tensors run the fp64 kernels with f
 Gradients flow to ``state``, ``next_vel`` and ``mass`` (1-D: ``setMasses``, shared by the batch, gradient summed; 2-D ``[B, m]``:
 per world, the World is left untouched).  The work is done by libnb2.so (include/nb2.h ``nb2_inverse_dynamics``,
 ``nb2_contact_inverse_dynamics``, ``nb2_multiple_contact_inverse_dynamics``, ``nb2_forward_dynamics_batch``).
+
+``inverse_dynamics_jacobians`` and ``forward_dynamics_jacobians`` return the dense Jacobians of ``inverse_dynamics`` and
+``forward_dynamics`` (with their outputs) in one launch (``nb2_inverse_dynamics_jacobians`` / ``nb2_forward_dynamics_jacobians``), for
+iLQR / DDP, Gauss-Newton or linearised-MPC users who need the matrices rather than products with one gradient.
 """
 from __future__ import annotations
 
@@ -61,6 +65,8 @@ _WHO = "inverse_dynamics()"
 _WHO_CONTACT = "contact_inverse_dynamics()"
 _WHO_MULTI = "multiple_contact_inverse_dynamics()"
 _WHO_FD = "forward_dynamics()"
+_WHO_IDJ = "inverse_dynamics_jacobians()"
+_WHO_FDJ = "forward_dynamics_jacobians()"
 MAX_CONTACT_BODIES = 4  # include/nb2.h NB2_MAX_CONTACT_BODIES
 
 
@@ -160,11 +166,11 @@ class InverseDynamicsLayer(torch.autograd.Function):
         return (None,) + _input_grads(ctx, gs, gn, gi)
 
 
-def _check_fd(world, state, tau):
+def _check_fd(world, state, tau, who=_WHO_FD, second="tau"):
     """ValueError unless the world has dofs and state / tau are rows as inverse_dynamics takes them; nothing touches the device."""
     if world.getNumDofs() == 0:
-        raise ValueError(f"{_WHO_FD}: the world has no degrees of freedom")
-    _check_rows(world, state, tau, _WHO_FD, "tau")
+        raise ValueError(f"{who}: the world has no degrees of freedom")
+    _check_rows(world, state, tau, who, second)
 
 
 class ForwardDynamicsLayer(torch.autograd.Function):
@@ -208,6 +214,62 @@ def forward_dynamics(world, state: torch.Tensor, tau: torch.Tensor, mass: Option
     if mass is not None and mass.dim() == 2:
         return ForwardDynamicsLayer.apply(world, state, tau, None, per_world_inertia(world, state, mass, _WHO_FD))
     return ForwardDynamicsLayer.apply(world, state, tau, mass)
+
+
+def _dynamics_jacobians(world, state, x, mass, who, second, fd):
+    """The shared body of inverse_dynamics_jacobians / forward_dynamics_jacobians: (out, J_q, J_qdot, J_x) in the state's dtype and device."""
+    _check_fd(world, state, x, who, second)
+    wi = per_world_inertia(world, state, mass, who) if mass is not None and mass.dim() == 2 else None
+    dm = set_shared_masses(world, mass, who) if mass is not None and wi is None else device_model_for(world)
+    if not torch.cuda.is_available():
+        raise RuntimeError(f"nimblephysics_b200.{who[:-2]} needs a CUDA device; there is no CPU fallback")
+    single = state.dim() == 1
+    s2 = state.detach().reshape(1, -1) if single else state.detach()
+    x2 = x.detach().reshape(1, -1) if single else x.detach()
+    dev = s2.device if s2.is_cuda else torch.device("cuda", torch.cuda.current_device())
+    rdt = torch.float64 if state.dtype == torch.float64 else torch.float32
+    sd = s2.to(device=dev, dtype=rdt).contiguous()
+    xd = x2.to(device=dev, dtype=rdt).contiguous()
+    B, n = sd.shape[0], dm.ndof
+    with torch.cuda.device(dev):
+        out = torch.empty((B, n), dtype=rdt, device=dev)
+        J = [torch.empty((B, n, n), dtype=rdt, device=dev) for _ in range(3)]
+        if B > 0:  # an empty batch has no rows to hand over (its data pointers may be NULL)
+            run = dm.forward_dynamics_jacobians_device if fd else dm.inverse_dynamics_jacobians_device
+            run(B, sd.data_ptr(), xd.data_ptr(), out.data_ptr(), J[0].data_ptr(), J[1].data_ptr(), J[2].data_ptr(), torch.cuda.current_stream().cuda_stream,
+                FP64 if rdt == torch.float64 else FP32, wi_ptr=_ptr(_word_major_inertia(dm, wi, B, dev)))
+    res = [out] + J
+    if single:
+        res = [r[0] for r in res]
+    return tuple(r.to(device=state.device, dtype=state.dtype) for r in res)
+
+
+def inverse_dynamics_jacobians(world, state: torch.Tensor, next_vel: torch.Tensor, mass: Optional[torch.Tensor] = None):
+    """(tau, dtau_dq, dtau_dqdot, dtau_dnext_vel): tau = inverse_dynamics(world, state, next_vel, mass) [B, n] and its dense Jacobians
+    [B, n, n], J[w, i, j] = d tau_i / d x_j (the layout of torch.autograd.functional.jacobian), next_vel held fixed in the first two:
+
+        dtau_dnext_vel = M / dt ,   dtau_dqdot = dID_a/dqdot + D + dt K - M / dt ,   dtau_dq = dID_a/dq + K ,
+
+    with ID_a(q, qdot, a) = M a + C + g at a = (next_vel - qdot) / dt.  Row i is inverse_dynamics's vector-Jacobian product with the seed
+    e_i, so the blocks equal autograd's Jacobian of inverse_dynamics up to rounding; free joints follow its conventions (body-twist velocity
+    columns, position columns for the six stored coordinates).  state [B, 2n] or [2n] (then [n] and [n, n] outputs), mass as for
+    inverse_dynamics; precision follows state.dtype.  Contacts, limits and clipping are ignored and the LCP cache is not touched.
+    The outputs carry no autograd history: there are no second derivatives and no mass Jacobian.  ValueError before any device work for a
+    wrong shape, a world without dofs or a mass of the wrong size."""
+    return _dynamics_jacobians(world, state, next_vel, mass, _WHO_IDJ, "next_vel", False)
+
+
+def forward_dynamics_jacobians(world, state: torch.Tensor, tau: torch.Tensor, mass: Optional[torch.Tensor] = None):
+    """(qdd, dqdd_dq, dqdd_dqdot, dqdd_dtau): qdd = forward_dynamics(world, state, tau, mass) [B, n] and its dense Jacobians [B, n, n],
+    J[w, i, j] = d qdd_i / d x_j:
+
+        dqdd_dtau = M^-1 ,   dqdd_dq = -M^-1 (dID_a/dq + K) ,   dqdd_dqdot = -M^-1 (dID_a/dqdot + D + dt K)    at a = qdd.
+
+    Row i is forward_dynamics's vector-Jacobian product with the seed e_i, so the blocks equal autograd's Jacobian of forward_dynamics up to
+    rounding.  Arguments, shapes, precision and what is ignored as for inverse_dynamics_jacobians; unlike forward_dynamics this runs on
+    every model inverse_mass_matrix runs on, in both precisions.  The outputs carry no autograd history: there are no second derivatives
+    and no mass Jacobian.  ValueError before any device work for a wrong shape, a world without dofs or a mass of the wrong size."""
+    return _dynamics_jacobians(world, state, tau, mass, _WHO_FDJ, "tau", True)
 
 
 def contact_body_index(world, body, who: str = _WHO_CONTACT) -> int:
