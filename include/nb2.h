@@ -351,6 +351,19 @@ int nb2_com_jacobian_deriv(const nb2_model* m, int B, const void* state, int roo
 int nb2_com_jacobian_deriv_backward(const nb2_model* m, int B, const void* state, int root_body, const double* world_inertia, const void* grad_dJ,
                                     void* grad_state, double* grad_inertia, int precision, void* stream);
 
+/* Kinetic and potential energy and centroidal momentum of the tree rooted at canonical body root_body at the states state [B, 2 ndof]
+ * (Skeleton::computeKineticEnergy / computePotentialEnergy, DESIGN.md §6m): kinetic [B] = 1/2 sum_i V_i . G_i V_i, potential [B] =
+ * -g . sum_i (m_i p_i + R_i h_i) + 1/2 sum_d k_d (q_d - q0_d)^2 over the tree's bodies and dofs, momentum [B, 6] = [angular momentum about
+ * the tree's COM ; linear momentum] in world axes.  Rows in the arithmetic type of `precision`; world_inertia as nb2_com_jacobian.  The
+ * VJP reads grad_kinetic [B], grad_potential [B] and grad_momentum [B, 6] (each may be NULL: zero) and writes grad_state [B, 2 ndof] =
+ * [dL/dq ; dL/dqdot] (0 on other trees' dofs) and, if not NULL, grad_inertia [10 * nb][B] fp64.  One warp per world; stateless, nothing
+ * allocated, B = 0 only validates.  NB2_ERR_INVALID for a root_body that is not a tree root or a model without dofs. */
+int nb2_energy_momentum(const nb2_model* m, int B, const void* state, int root_body, const double* world_inertia, void* kinetic, void* potential,
+                        void* momentum, int precision, void* stream);
+int nb2_energy_momentum_backward(const nb2_model* m, int B, const void* state, int root_body, const double* world_inertia, const void* grad_kinetic,
+                                 const void* grad_potential, const void* grad_momentum, void* grad_state, double* grad_inertia, int precision,
+                                 void* stream);
+
 /* Batched boxed-LCP solves on the device: B independent problems, one warp each — the reference's pointer-style lower boundary
  * BoxedLcpSolver::solve(n, A, x, b, nub, lo, hi, findex, earlyTermination) (dart/constraint/BoxedLcpSolver.hpp:125-135) and the
  * solve chain of BoxedLcpConstraintSolver::solveLcp (BoxedLcpConstraintSolver.cpp:352-789).  Device pointers; problem w has dimension

@@ -23,6 +23,7 @@
 #include "nb2_host_model.h"
 #include "nb2_coop.cuh"
 #include "nb2_djac.h"
+#include "nb2_energy.h"
 #include "nb2_fd.h"
 
 static thread_local std::string g_err;
@@ -2349,6 +2350,40 @@ int nb2_com_jacobian_deriv_backward(const nb2_model* m, int B, const void* state
     return launch_jacd_com<R>(m, B, (const R*)state, root_body, world_inertia, nullptr, (const R*)grad_dJ, (R*)grad_state, grad_inertia,
                               (cudaStream_t)stream, who);
   });
+}
+}  // extern "C"
+
+// ---- energy and momentum (nb2_energy.cu): one warp per world, NB2_EM_WPB worlds per block, the working set of nb2_energy.cuh
+static int launch_em(const nb2_model* m, int B, const void* state, int root, const double* wi, void* kin, void* pot, void* mom, const void* gkin,
+                     const void* gpot, const void* gmom, void* gstate, double* gI, int precision, void* stream, const char* who) {
+  const nb2_variant& v = m->variants[0];
+  if (root < 0 || root >= v.mf.nb || v.mf.parent[root] >= 0) { g_err = std::string(who) + ": root_body " + std::to_string(root) + " is not a tree root"; return NB2_ERR_INVALID; }
+  if (B == 0) return NB2_OK;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    const size_t smem = nb2_em_smem(v.mf.nb, v.mf.ndof, gstate != nullptr, sizeof(R));
+    if (smem > (size_t)kMaxSmem) { g_err = std::string(who) + ": the model's working set does not fit in shared memory"; return NB2_ERR_INVALID; }
+    NB2_CUDA(nb2_em_launch<R>((cudaStream_t)stream, smem, model_of<R>(v), B, root, (const R*)state, wi, (R*)kin, (R*)pot, (R*)mom, (const R*)gkin,
+                              (const R*)gpot, (const R*)gmom, (R*)gstate, gI));
+    g_launches++;
+    return NB2_OK;
+  });
+}
+extern "C" {
+int nb2_energy_momentum(const nb2_model* m, int B, const void* state, int root_body, const double* world_inertia, void* kinetic, void* potential,
+                        void* momentum, int precision, void* stream) {
+  static const char* who = "nb2_energy_momentum";
+  if (int rc = mm_args_ok(m, B, state && kinetic && potential && momentum, who)) return rc;
+  return launch_em(m, B, state, root_body, world_inertia, kinetic, potential, momentum, nullptr, nullptr, nullptr, nullptr, nullptr, precision, stream,
+                   who);
+}
+int nb2_energy_momentum_backward(const nb2_model* m, int B, const void* state, int root_body, const double* world_inertia, const void* grad_kinetic,
+                                 const void* grad_potential, const void* grad_momentum, void* grad_state, double* grad_inertia, int precision,
+                                 void* stream) {
+  static const char* who = "nb2_energy_momentum_backward";
+  if (int rc = mm_args_ok(m, B, state && grad_state, who)) return rc;
+  return launch_em(m, B, state, root_body, world_inertia, nullptr, nullptr, nullptr, grad_kinetic, grad_potential, grad_momentum, grad_state,
+                   grad_inertia, precision, stream, who);
 }
 int nb2_model_ndof(const nb2_model* m) { return m ? m->mf.ndof : -1; }
 int nb2_model_na(const nb2_model* m) { return m ? m->mf.na : -1; }

@@ -281,6 +281,17 @@ class DeviceModel:
         _cabi.check(_cabi.lib().nb2_com_jacobian_deriv_backward(self.handle, B, state_ptr, int(root), wi_ptr, gJ_ptr, gstate_ptr, ginertia_ptr,
                                                                 precision, stream))
 
+    def energy_momentum_device(self, B, state_ptr, root, kin_ptr, pot_ptr, mom_ptr, stream, precision=FP32, wi_ptr=None):
+        """kinetic [B], potential [B] and momentum [B, 6] of the tree rooted at canonical body `root` at states [B, 2n] (include/nb2.h
+        nb2_energy_momentum)."""
+        _cabi.check(_cabi.lib().nb2_energy_momentum(self.handle, B, state_ptr, int(root), wi_ptr, kin_ptr, pot_ptr, mom_ptr, precision, stream))
+
+    def energy_momentum_backward_device(self, B, state_ptr, root, gkin_ptr, gpot_ptr, gmom_ptr, gstate_ptr, stream, precision=FP32,
+                                        ginertia_ptr=None, wi_ptr=None):
+        """VJP of energy_momentum_device into gstate [B, 2n]; ginertia_ptr: optional [10*nb, B] float64 buffer."""
+        _cabi.check(_cabi.lib().nb2_energy_momentum_backward(self.handle, B, state_ptr, int(root), wi_ptr, gkin_ptr, gpot_ptr, gmom_ptr, gstate_ptr,
+                                                             ginertia_ptr, precision, stream))
+
     def contact_workspace_bytes(self, B):
         return int(_cabi.lib().nb2_contact_workspace_bytes(self.handle, B))
 

@@ -479,6 +479,28 @@ class Skeleton:
         """Skeleton::getCOMLinearJacobianDeriv() [3, n_skel] (numpy fp64; fp64 kernels, nimblephysics_b200.com_jacobian_deriv)."""
         return self._jacobian_deriv_columns("getCOMLinearJacobianDeriv()")
 
+    def _energies(self, who):
+        from .energy import _single_world_energy
+
+        w, _ = self._dof_offset_in_world()
+        if w is None:
+            raise ValueError(f"Skeleton.{who}: the skeleton is not part of a World")
+        return _single_world_energy(w, self, who)
+
+    def computeKineticEnergy(self):
+        """Skeleton::computeKineticEnergy() at the current positions and velocities (float, fp64 kernels,
+        nimblephysics_b200.energy_and_momentum)."""
+        return self._energies("computeKineticEnergy()")[0]
+
+    def computePotentialEnergy(self):
+        """Skeleton::computePotentialEnergy(): gravity at each body's centre of mass plus the joint springs (float; DESIGN.md §6m)."""
+        return self._energies("computePotentialEnergy()")[1]
+
+    def computeLagrangian(self):
+        """Skeleton::computeLagrangian() = computeKineticEnergy() - computePotentialEnergy() (float)."""
+        T, U = self._energies("computeLagrangian()")
+        return T - U
+
     def setVelocity(self, i, v):
         w, off = self._dof_offset_in_world()
         if w is None:

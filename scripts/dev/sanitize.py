@@ -53,6 +53,7 @@ for B in (7, 203):
         nb.forward_dynamics(mw, st, tau, mass * torch.tensor(mw.getMasses(), device="cuda")).sum().backward()
         nb.inverse_dynamics_jacobians(mw, st, vn, mass.detach() * torch.tensor(mw.getMasses(), device="cuda"))
         nb.forward_dynamics_jacobians(mw, st, tau, mass.detach() * torch.tensor(mw.getMasses(), device="cuda"))
+        sum(x.sum() for x in nb.energy_and_momentum(mw, st, mw.skeletons[0], mass * torch.tensor(mw.getMasses(), device="cuda"))).backward()
     sd = torch.tensor(s, device="cuda", dtype=torch.float64)
     nb.device_model_for(w).forward_dynamics(sd[:, :raw.ndof], sd[:, raw.ndof:], sd[:, raw.ndof:] * 10)
 torch.cuda.synchronize()
