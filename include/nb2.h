@@ -364,6 +364,21 @@ int nb2_energy_momentum_backward(const nb2_model* m, int B, const void* state, i
                                  const void* grad_potential, const void* grad_momentum, void* grad_state, double* grad_inertia, int precision,
                                  void* stream);
 
+/* Inverse-dynamics regressor (DESIGN.md §6n): nb2_inverse_dynamics as a linear map of the canonical inertia table.  At state [B, 2 ndof]
+ * and next_vel [B, ndof] it writes Y [B, ndof, nb, 10] and tau_passive [B, ndof] = K (q - q0 + qdot dt) + D qdot such that, for ANY
+ * per-world inertia table pi ([nb][10] per world, the layout of world_inertia),
+ *     nb2_inverse_dynamics(state, next_vel, world_inertia = pi)[w, d] = sum_{j,k} Y[w, d, j, k] pi[w, j, k] + tau_passive[w, d].
+ * Y[w, d, j] is 0 unless dof d's joint is at or above canonical body j; every entry of the B rows is written.  Energy regressor: at state
+ * [B, 2 ndof], Y_kinetic and Y_potential [B, nb, 10] and spring_energy [B] with sum_{j,k} Y_kinetic[w, j, k] pi[w, j, k] = 1/2 qdot^T M qdot,
+ * sum_{j,k} Y_potential[w, j, k] pi[w, j, k] = -g . sum_j (m_j p_j + R_j h_j) (gravity at every body's COM), spring_energy =
+ * 1/2 sum_d k_d (q_d - q0_d)^2 over all dofs.  Rows in the arithmetic type of `precision`.  Contacts, limits and clipping are ignored and
+ * no LCP cache is read or written.  One warp per world; stateless, nothing allocated, B = 0 only validates.  NB2_ERR_INVALID for a model
+ * without dofs. */
+int nb2_inverse_dynamics_regressor(const nb2_model* m, int B, const void* state, const void* next_vel, void* Y, void* tau_passive, int precision,
+                                   void* stream);
+int nb2_energy_regressor(const nb2_model* m, int B, const void* state, void* Y_kinetic, void* Y_potential, void* spring_energy, int precision,
+                         void* stream);
+
 /* Batched boxed-LCP solves on the device: B independent problems, one warp each — the reference's pointer-style lower boundary
  * BoxedLcpSolver::solve(n, A, x, b, nub, lo, hi, findex, earlyTermination) (dart/constraint/BoxedLcpSolver.hpp:125-135) and the
  * solve chain of BoxedLcpConstraintSolver::solveLcp (BoxedLcpConstraintSolver.cpp:352-789).  Device pointers; problem w has dimension

@@ -25,6 +25,7 @@
 #include "nb2_djac.h"
 #include "nb2_energy.h"
 #include "nb2_fd.h"
+#include "nb2_reg.h"
 
 static thread_local std::string g_err;
 static std::atomic<long long> g_launches{0};
@@ -2384,6 +2385,39 @@ int nb2_energy_momentum_backward(const nb2_model* m, int B, const void* state, i
   if (int rc = mm_args_ok(m, B, state && grad_state, who)) return rc;
   return launch_em(m, B, state, root_body, world_inertia, nullptr, nullptr, nullptr, grad_kinetic, grad_potential, grad_momentum, grad_state,
                    grad_inertia, precision, stream, who);
+}
+}  // extern "C"
+
+// ---- regressors (nb2_reg.cu): one warp per world, NB2_REG_WPB worlds per block, the working set of nb2_reg.cuh.  The kinematics stages run
+// on the widest lane schedule the model has: the warp has 32 lanes, and the body sweeps are its serial part.
+static int launch_reg(const nb2_model* m, int B, const void* state, const void* next_vel, void* Y, void* tau_passive, void* YT, void* YU, void* spring,
+                      int precision, void* stream, const char* who) {
+  if (B == 0) return NB2_OK;
+  const nb2_variant* widest = &m->variants[0];
+  for (const auto& o : m->variants) if (o.mf.lanes > widest->mf.lanes) widest = &o;
+  const nb2_variant& v = *widest;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    const size_t smem = nb2_reg_smem(v.mf.nb, v.mf.ndof, model_of<R>(v).nslots, model_of<R>(v).nfree, Y == nullptr, sizeof(R));
+    if (smem > (size_t)kMaxSmem) { g_err = std::string(who) + ": the model's working set does not fit in shared memory"; return NB2_ERR_UNSUPPORTED; }
+    NB2_CUDA(nb2_reg_launch<R>((cudaStream_t)stream, smem, model_of<R>(v), B, (const R*)state, (const R*)next_vel, (R*)Y, (R*)tau_passive, (R*)YT,
+                               (R*)YU, (R*)spring));
+    g_launches++;
+    return NB2_OK;
+  });
+}
+extern "C" {
+int nb2_inverse_dynamics_regressor(const nb2_model* m, int B, const void* state, const void* next_vel, void* Y, void* tau_passive, int precision,
+                                   void* stream) {
+  static const char* who = "nb2_inverse_dynamics_regressor";
+  if (int rc = mm_args_ok(m, B, state && next_vel && Y && tau_passive, who)) return rc;
+  return launch_reg(m, B, state, next_vel, Y, tau_passive, nullptr, nullptr, nullptr, precision, stream, who);
+}
+int nb2_energy_regressor(const nb2_model* m, int B, const void* state, void* Y_kinetic, void* Y_potential, void* spring_energy, int precision,
+                         void* stream) {
+  static const char* who = "nb2_energy_regressor";
+  if (int rc = mm_args_ok(m, B, state && Y_kinetic && Y_potential && spring_energy, who)) return rc;
+  return launch_reg(m, B, state, nullptr, nullptr, nullptr, Y_kinetic, Y_potential, spring_energy, precision, stream, who);
 }
 int nb2_model_ndof(const nb2_model* m) { return m ? m->mf.ndof : -1; }
 int nb2_model_na(const nb2_model* m) { return m ? m->mf.na : -1; }

@@ -292,6 +292,15 @@ class DeviceModel:
         _cabi.check(_cabi.lib().nb2_energy_momentum_backward(self.handle, B, state_ptr, int(root), wi_ptr, gkin_ptr, gpot_ptr, gmom_ptr, gstate_ptr,
                                                              ginertia_ptr, precision, stream))
 
+    def inverse_dynamics_regressor_device(self, B, state_ptr, next_vel_ptr, Y_ptr, tau_passive_ptr, stream, precision=FP32):
+        """Y [B, n, nb, 10] and tau_passive [B, n] of inverse dynamics at states [B, 2n] and next velocities [B, n] (include/nb2.h
+        nb2_inverse_dynamics_regressor)."""
+        _cabi.check(_cabi.lib().nb2_inverse_dynamics_regressor(self.handle, B, state_ptr, next_vel_ptr, Y_ptr, tau_passive_ptr, precision, stream))
+
+    def energy_regressor_device(self, B, state_ptr, YT_ptr, YU_ptr, spring_ptr, stream, precision=FP32):
+        """Y_kinetic, Y_potential [B, nb, 10] and the spring energy [B] at states [B, 2n] (include/nb2.h nb2_energy_regressor)."""
+        _cabi.check(_cabi.lib().nb2_energy_regressor(self.handle, B, state_ptr, YT_ptr, YU_ptr, spring_ptr, precision, stream))
+
     def contact_workspace_bytes(self, B):
         return int(_cabi.lib().nb2_contact_workspace_bytes(self.handle, B))
 

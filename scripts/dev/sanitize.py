@@ -1,7 +1,7 @@
 """Small end-to-end run for compute-sanitizer (memcheck): contact-free fwd+bwd (device + pinned-host paths, partial groups),
 contact fwd+bwd, fused rollout, inverse dynamics, contact and multiple-contact inverse dynamics fwd+bwd, the mass matrix and its inverse fwd+bwd, the world and COM Jacobians
 and their time derivatives fwd+bwd, forward dynamics fwd+bwd, the pointer-style forward dynamics and the dense Jacobians of inverse and
-forward dynamics (both precisions, per-world masses and offsets, partial groups and partial blocks)."""
+forward dynamics and the inverse-dynamics and energy regressors (both precisions, per-world masses and offsets, partial groups and partial blocks)."""
 import sys
 import numpy as np, torch
 sys.path.insert(0, ".")
@@ -54,6 +54,8 @@ for B in (7, 203):
         nb.inverse_dynamics_jacobians(mw, st, vn, mass.detach() * torch.tensor(mw.getMasses(), device="cuda"))
         nb.forward_dynamics_jacobians(mw, st, tau, mass.detach() * torch.tensor(mw.getMasses(), device="cuda"))
         sum(x.sum() for x in nb.energy_and_momentum(mw, st, mw.skeletons[0], mass * torch.tensor(mw.getMasses(), device="cuda"))).backward()
+        nb.inverse_dynamics_regressor(mw, st, vn)
+        nb.energy_regressor(mw, st)
     sd = torch.tensor(s, device="cuda", dtype=torch.float64)
     nb.device_model_for(w).forward_dynamics(sd[:, :raw.ndof], sd[:, raw.ndof:], sd[:, raw.ndof:] * 10)
 torch.cuda.synchronize()
