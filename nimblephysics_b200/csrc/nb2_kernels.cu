@@ -13,6 +13,7 @@
 #include <mutex>
 #include <string>
 #include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "../../include/nb2.h"
@@ -73,14 +74,21 @@ template <int K> __host__ __device__ constexpr size_t staging_bytes(int floats_p
   return (((size_t)floats_per_world * CoopShape<K>::WPW * sizeof(float) + 15) & ~(size_t)15) + 16;
 }
 
+// ---- programmatic dependent launch (launch_dependent below): a step kernel's launch is processed, and its blocks are placed, while the
+// kernel before it in the stream completes.  grid_dependency_wait() returns once that grid has completed and its memory is visible,
+// so every global load AND store of the kernel comes after it: the previous kernel may still be reading a buffer this one writes.
+// Every thread executes it (no early return ahead of it), so the chain of waits orders each launch after all earlier ones.
+__device__ __forceinline__ void grid_dependency_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
 // ---- optional stage clocks of the contact-free step kernels (-DNB2_STEP_CLOCKS; dev builds only, scripts/dev/stage_clocks.py):
 // thread 0 of every NB2_CLK_EVERY-th warp of the grid (up to NB2_CLK_WARPS of them) records clock64() at kernel entry, after the
-// body-table and input staging, and after every stage including its barrier.  Default builds compile none of it.
+// wait for the previous kernel, after the body-table and input staging, and after every stage including its barrier.  Default
+// builds compile none of it.
 #ifdef NB2_STEP_CLOCKS
 #define NB2_CLK_WARPS 8
 #define NB2_CLK_EVERY 64
 #define NB2_CLK_SLOTS 16
-__device__ long long nb2_step_clk[2][NB2_CLK_WARPS][NB2_CLK_SLOTS];  // [forward, backward][sampled warp][entry, staged, stage 0, 1, ...]
+__device__ long long nb2_step_clk[2][NB2_CLK_WARPS][NB2_CLK_SLOTS];  // [forward, backward][sampled warp][entry, waited, staged, stage 0, 1, ...]
 #define NB2_CLK(dir, k)                                                                                                   \
   do {                                                                                                                    \
     const int w_ = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);                                                   \
@@ -111,6 +119,8 @@ k_step_fwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
   R* sv = saved ? saved + wg + (valid ? slot : 0) : nullptr;
   const double* wi = PW ? winertia + wg + (valid ? slot : 0) : nullptr;
   constexpr unsigned sync_mask = (K > 1) ? NB2_FWD_SYNC_MASK : NB2_FWD_SYNC_MASK_1LANE;
+  grid_dependency_wait();
+  NB2_CLK(0, 1);
   // input rows of the group: through the bulk-copy staging buffer when they qualify, else read in place.  The copy is in
   // flight while the block stages the body table: the table's constant-bank loads (one replay per distinct address) and
   // the DRAM round trip of the rows overlap instead of adding up.
@@ -138,7 +148,7 @@ k_step_fwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
     __syncwarp();
     mbar_wait(bar, 0);
   }
-  NB2_CLK(0, 1);
+  NB2_CLK(0, 2);
 #pragma unroll 1
   for (int sg = 0; sg < NB2_FWD_STAGES; sg++) {
     if (sg == 0) {
@@ -148,7 +158,7 @@ k_step_fwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
     else if (sg == NB2_FWD_STAGES - 1) { if (nworlds > 0) nb2::fwd_store<R, ST>(M, scr0, next + wg * 2 * M.ndof, nworlds, li, 32); }
     else if (valid) nb2::world_forward_stage<R, ST>(M, scr, sv, (size_t)B, saved != nullptr, lane, sg, bt, nullptr, wi, (size_t)B);
     if ((sync_mask >> sg) & 1u) __syncwarp();
-    NB2_CLK(0, 2 + sg);
+    NB2_CLK(0, 3 + sg);
   }
 }
 
@@ -169,6 +179,8 @@ k_step_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
   const size_t w = wg + (valid ? slot : 0);
   R* scr0 = reinterpret_cast<R*>(nb2_smem) + body_table_words<K>(M.nb) + (size_t)(threadIdx.x >> 5) * words * ST;
   R* scr = scr0 + slot;
+  grid_dependency_wait();  // no global access above this line (see k_step_fwd)
+  NB2_CLK(1, 1);
   // input rows (dL/dx', x, u) of the group through the bulk-copy staging buffer when they qualify; in flight, like the
   // saved-stream burst below, while the block stages the body table (see k_step_fwd)
   const float* g_src = gnext + wg * 2 * M.ndof;
@@ -220,7 +232,7 @@ k_step_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
     __syncwarp();
     mbar_wait(bar, 0);
   }
-  NB2_CLK(1, 1);
+  NB2_CLK(1, 2);
 #pragma unroll 1
   for (int sg = 0; sg < NB2_BWD_STAGES; sg++) {
     if (sg == 0) { if (nworlds > 0) nb2::bwd_load<R, ST, false>(M, scr0, st_src, act_src, g_src, nworlds, li, 32); }
@@ -230,7 +242,7 @@ k_step_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
                                                        (PW && winertia) ? winertia + w : nullptr, (size_t)B, (PW && ginertia_acc) ? ginertia_acc + w : nullptr);
     if (sg == 0 && stage_saved) asm volatile("cp.async.wait_group 0;" ::: "memory");
     if (((sync_mask >> sg) & 1u) || (sg == 0 && stage_saved)) __syncwarp();
-    NB2_CLK(1, 2 + sg);
+    NB2_CLK(1, 3 + sg);
   }
 }
 
@@ -1220,6 +1232,25 @@ static int pick_variant(nb2_model* m, int B, int dir, nb2_variant** out) {
   return NB2_OK;
 }
 
+// launches a step kernel as a programmatic dependent of the previous kernel in the stream.  The step kernels never execute
+// griddepcontrol.launch_dependents, so a dependent is launched as the previous kernel's blocks exit, and its launch processing
+// (the model parameter included) and block placement overlap that kernel's completion and memory flush; an explicit trigger
+// measured slower (DESIGN.md §3).  A failed launch leaves its error for cudaGetLastError(), like <<<>>>.
+template <class... P, class... A>
+static void launch_dependent(void (*kern)(P...), int blocks, int threads, size_t smem, cudaStream_t st, A&&... args) {
+  cudaLaunchAttribute attr[1] = {};
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(blocks);
+  cfg.blockDim = dim3(threads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  cudaLaunchKernelEx(&cfg, kern, std::forward<A>(args)...);
+}
+
 template <class R, int K>
 static int launch_fwd_k(const nb2_variant& v, int sm_count, int Btot, int w0, int B, const float* state, const float* action,
                         float* next, R* saved, cudaStream_t st, float* state_copy, float* action_copy, const double* wi) {
@@ -1230,8 +1261,10 @@ static int launch_fwd_k(const nb2_variant& v, int sm_count, int Btot, int w0, in
   const int warps = block_warps(total_warps, sm_count, sh, per_warp);
   const int blocks = (total_warps + warps - 1) / warps;
   const size_t smem = per_warp * warps + (size_t)body_table_words<K>(v.mf.nb) * sizeof(R) + 16;
-  if (wi) k_step_fwd<R, K, true><<<blocks, warps * 32, smem, st>>>(model_of<R>(v), Btot, w0, B, state, action, next, saved, v.fwd_words, state_copy, action_copy, wi);
-  else k_step_fwd<R, K, false><<<blocks, warps * 32, smem, st>>>(model_of<R>(v), Btot, w0, B, state, action, next, saved, v.fwd_words, state_copy, action_copy, nullptr);
+  if (wi) launch_dependent(k_step_fwd<R, K, true>, blocks, warps * 32, smem, st, model_of<R>(v), Btot, w0, B, state, action, next, saved, v.fwd_words,
+                           state_copy, action_copy, wi);
+  else launch_dependent(k_step_fwd<R, K, false>, blocks, warps * 32, smem, st, model_of<R>(v), Btot, w0, B, state, action, next, saved, v.fwd_words,
+                        state_copy, action_copy, nullptr);
   g_launches++;
   NB2_CUDA(cudaGetLastError());
   return NB2_OK;
@@ -1274,10 +1307,10 @@ static int launch_bwd_k(const nb2_variant& v, int sm_count, int Btot, int w0, in
   const size_t base = ((stage ? smem_staged : scratch_per_warp * warps + tab) + 15) & ~(size_t)15;
   const bool in_stage = base + in_per_warp * warps <= (size_t)kMaxSmem;
   const size_t smem = in_stage ? base + in_per_warp * warps : base;
-  if (wi || gIa) k_step_bwd<R, K, true><<<blocks, warps * 32, smem, st>>>(model_of<R>(v), Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia,
-                                                                   v.bwd_words, stage ? 1 : 0, accumulate, in_stage ? (unsigned)base : 0u, wi, gIa);
-  else k_step_bwd<R, K, false><<<blocks, warps * 32, smem, st>>>(model_of<R>(v), Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia,
-                                                                 v.bwd_words, stage ? 1 : 0, accumulate, in_stage ? (unsigned)base : 0u, nullptr, nullptr);
+  if (wi || gIa) launch_dependent(k_step_bwd<R, K, true>, blocks, warps * 32, smem, st, model_of<R>(v), Btot, w0, B, state, action, saved, gnext, gstate,
+                                  gaction, ginertia, v.bwd_words, stage ? 1 : 0, accumulate, in_stage ? (unsigned)base : 0u, wi, gIa);
+  else launch_dependent(k_step_bwd<R, K, false>, blocks, warps * 32, smem, st, model_of<R>(v), Btot, w0, B, state, action, saved, gnext, gstate,
+                        gaction, ginertia, v.bwd_words, stage ? 1 : 0, accumulate, in_stage ? (unsigned)base : 0u, nullptr, nullptr);
   g_launches++;
   NB2_CUDA(cudaGetLastError());
   return NB2_OK;

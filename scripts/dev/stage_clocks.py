@@ -3,11 +3,13 @@
     nvcc <the flags of __graft_entry__.NVCC_FLAGS> -DNB2_STEP_CLOCKS -o build/clk/libnb2.so nimblephysics_b200/csrc/nb2_kernels.cu nimblephysics_b200/csrc/nb2_fd.cu
     NB2_LIB=build/clk/libnb2.so python scripts/dev/stage_clocks.py [--batch 4096] [--lanes 4 1] [--reps 20]
 
-Thread 0 of a few warps spread over the grid records clock64() at kernel entry, after the body-table / input staging and after
-every stage with its barrier (nb2_kernels.cu, NB2_CLK).  Thread 0 is lane 0 of the group's first world: the lane that sweeps
-the trunk.  For every stage the table gives the median over the sampled warps and launches, and for the body sweeps the
-number of bodies lane 0 walks in it and the cycles per body.  Cycles are SM clocks; the instrumented build adds a few
-instructions per stage, so compare stages with each other, not with the default build's kernel times.
+Thread 0 of a few warps spread over the grid records clock64() at kernel entry, after the wait for the previous kernel
+(griddepcontrol.wait), after the body-table / input staging and after every stage with its barrier (nb2_kernels.cu, NB2_CLK).
+The backward of a rep is launched right behind its forward, so its wait covers the forward's tail.  Thread 0 is lane 0 of the
+group's first world: the lane that sweeps the trunk.  For every stage the table gives the median over the sampled warps and
+launches, and for the body sweeps the number of bodies lane 0 walks in it and the cycles per body.  Cycles are SM clocks; the
+instrumented build adds a few instructions per stage, so compare stages with each other, not with the default build's kernel
+times.
 """
 import argparse
 import ctypes
@@ -72,7 +74,7 @@ def main():
             c = np.frombuffer(buf, dtype=np.int64).reshape(2, WARPS, SLOTS)
             for d, stages in ((0, FWD), (1, BWD)):
                 for w in range(WARPS):
-                    t = c[d, w, :len(stages) + 2]
+                    t = c[d, w, :len(stages) + 3]
                     if t[0] and np.all(t[1:] >= t[:-1]):
                         runs[d].append(np.diff(t))
         print(f"\n--- K = {K} lanes per world: lane 0 sweeps {nbody['trunk']} trunk bodies and {nbody['limb']} limb bodies ---")
@@ -82,15 +84,16 @@ def main():
                 continue
             med = np.median(np.stack(runs[d]), axis=0)
             print(f"{kname} ({len(runs[d])} samples)   {'stage':<22}{'cycles':>9}{'bodies':>8}{'per body':>10}")
-            print(f"{'':<24}{'entry: body table + input staging':<33}{med[0]:>9.0f}")
-            groups = {"fixed": med[0], "trunk": 0.0, "limb": 0.0}
+            print(f"{'':<24}{'entry: wait for previous kernel':<33}{med[0]:>9.0f}")
+            print(f"{'':<24}{'entry: body table + input staging':<33}{med[1]:>9.0f}")
+            groups = {"fixed": med[1], "trunk": 0.0, "limb": 0.0}
             for k, (name, part) in enumerate(stages):
-                cyc = med[1 + k]
+                cyc = med[2 + k]
                 nbk = nbody[part] if part else 0
                 per = f"{cyc / nbk:>10.0f}" if nbk else ""
                 print(f"{'':<24}{k:>2} {name:<30}{cyc:>9.0f}{(nbk or ''):>8}{per}")
                 groups[part or "fixed"] += cyc
-            tot = sum(groups.values())
+            tot = sum(groups.values())  # without the wait: the chain of the kernel itself
             print(f"{'':<24}total {tot:.0f} cycles: fixed {groups['fixed'] / tot:.0%}, trunk stages {groups['trunk'] / tot:.0%}, "
                   f"limb stages {groups['limb'] / tot:.0%}")
     dm.set_lanes(0)
