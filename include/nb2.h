@@ -379,6 +379,30 @@ int nb2_inverse_dynamics_regressor(const nb2_model* m, int B, const void* state,
 int nb2_energy_regressor(const nb2_model* m, int B, const void* state, void* Y_kinetic, void* Y_potential, void* spring_energy, int precision,
                          void* stream);
 
+/* Constrained forward dynamics (DESIGN.md §6o): joint accelerations and contact wrenches of worlds whose k contact points are held by
+ * bilateral constraints.  Contact i is canonical body body[i] (1 <= k <= NB2_MAX_CONTACT_BODIES, distinct, none static) at the point
+ * T_owner_from_node[i] (R row-major 9, p 3: the node's placement on its body) applied to offsets[i] (NULL: the node's origin; [k, 3], or
+ * [B, k, 3] with offsets_per_world).  It constrains the [omega ; pdot] rows of the point's world Jacobian J (nb2_world_jacobian), or only
+ * its three linear rows with point_contacts.  With J [m, ndof] the stack, Jdot its time derivative (nb2_world_jacobian_deriv) and rho =
+ * damping >= 0,
+ *     M qdd + C + g + K (q - q0 + qdot dt) + D qdot = tau + J^T lam ,    J qdd + Jdot qdot = -rho lam ,
+ * tau per dof as for nb2_forward_dynamics_batch.  accel [B, ndof] = qdd; wrenches [B, k, 6] = [lam_a + p_i x lam_l ; lam_l] (lam_i =
+ * [torque about p_i ; force], world axes: the wrench about the world origin, as nb2_multiple_contact_inverse_dynamics) or, with
+ * point_contacts, [B, k, 3] = the force.  A world whose J M^-1 J^T + rho I has a Cholesky pivot at or below 64 eps max(diagonal) gets NaN
+ * rows.  The backward recomputes the forward and writes grad_state [B, 2 ndof], grad_tau [B, ndof], grad_offsets [B, k, 3] (or NULL, one
+ * row per world also for shared offsets) and grad_inertia ([10 nb, B] fp64, or NULL).  Rows in the arithmetic type of `precision`;
+ * contacts of the model, limits and the LCP cache play no part.  One warp per world; stateless, nothing allocated, B = 0 only validates.
+ * NB2_ERR_INVALID for k out of range, a body out of range or repeated, a negative or non-finite damping or a model without dofs;
+ * NB2_ERR_UNSUPPORTED when the working set does not fit shared memory. */
+int nb2_constrained_forward_dynamics(const nb2_model* m, int B, const void* state, const void* tau, int k, const int32_t* body,
+                                     const double* T_owner_from_node, const void* offsets, int offsets_per_world, int point_contacts, double damping,
+                                     const double* world_inertia, void* accel, void* wrenches, int precision, void* stream);
+int nb2_constrained_forward_dynamics_backward(const nb2_model* m, int B, const void* state, const void* tau, int k, const int32_t* body,
+                                              const double* T_owner_from_node, const void* offsets, int offsets_per_world, int point_contacts,
+                                              double damping, const double* world_inertia, const void* grad_accel, const void* grad_wrenches,
+                                              void* grad_state, void* grad_tau, void* grad_offsets, double* grad_inertia, int precision,
+                                              void* stream);
+
 /* Batched boxed-LCP solves on the device: B independent problems, one warp each — the reference's pointer-style lower boundary
  * BoxedLcpSolver::solve(n, A, x, b, nub, lo, hi, findex, earlyTermination) (dart/constraint/BoxedLcpSolver.hpp:125-135) and the
  * solve chain of BoxedLcpConstraintSolver::solveLcp (BoxedLcpConstraintSolver.cpp:352-789).  Device pointers; problem w has dimension

@@ -208,6 +208,10 @@ def lib() -> ctypes.CDLL:
         L.nb2_energy_momentum_backward.argtypes = [vp, ctypes.c_int, vp, ctypes.c_int] + [vp] * 6 + [ctypes.c_int, vp]
         L.nb2_inverse_dynamics_regressor.argtypes = [vp, ctypes.c_int] + [vp] * 4 + [ctypes.c_int, vp]
         L.nb2_energy_regressor.argtypes = [vp, ctypes.c_int] + [vp] * 4 + [ctypes.c_int, vp]
+        L.nb2_constrained_forward_dynamics.argtypes = ([vp, ctypes.c_int, vp, vp, ctypes.c_int, vp, vp, vp, ctypes.c_int, ctypes.c_int, ctypes.c_double]
+                                                       + [vp] * 3 + [ctypes.c_int, vp])
+        L.nb2_constrained_forward_dynamics_backward.argtypes = ([vp, ctypes.c_int, vp, vp, ctypes.c_int, vp, vp, vp, ctypes.c_int, ctypes.c_int,
+                                                                 ctypes.c_double] + [vp] * 7 + [ctypes.c_int, vp])
         L.nb2_lcp_solve_batch.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double] + [vp] * 11
         L.nb2_model_set_contact_capacity.argtypes = [vp, ctypes.c_int]
         L.nb2_model_contact_capacity.argtypes = [vp]

@@ -1,0 +1,141 @@
+"""``constrained_forward_dynamics(world, state, tau, contact_nodes, offsets=None, point_contacts=False, damping=0.0, mass=None)``:
+joint accelerations and contact wrenches of worlds whose contact points are held by bilateral constraints, batched and differentiable.
+
+For whole-body control, trajectory optimisation over a fixed stance schedule, MPC and policy learning through stance phases: the contact
+set is known, and qdd and the contact wrenches are wanted as smooth functions of the state, the force and the masses.  With k contact
+points p_i (1 <= k <= 4; each on a BodyNode, at an offset o_i in the node's frame, as in ``world_jacobian``), J the stack of their
+world-Jacobian rows ([omega ; pdot], or only the three linear rows with ``point_contacts=True``), Jdot its time derivative
+(``world_jacobian_deriv``) and rho = ``damping`` >= 0,
+
+    M qdd + C + g + K (q - q0 + qdot dt) + D qdot = tau + J^T lam ,     J qdd + Jdot qdot = -rho lam ,
+
+the dynamics of ``forward_dynamics`` with the contact forces added, so that
+
+    lam = -(J M^-1 J^T + rho I)^-1 (J qdd_free + Jdot qdot) ,   qdd = forward_dynamics(state, tau + J^T lam) ,   qdd_free = forward_dynamics(state, tau).
+
+lam_i is [torque about p_i ; force] in world axes.  The returned wrench of a 6-D contact is the wrench about the world origin,
+[lam_a + p_i x lam_l ; lam_l], the convention of ``multiple_contact_inverse_dynamics``; a point contact returns its force lam_l.  The
+constraints are equalities: no unilateral limits, friction cones or Baumgarte terms, and the world's own contacts, joint-limit rows and LCP
+cache play no part.  tau is per dof and free joints use the step's velocity coordinates, as in ``forward_dynamics``.
+
+A contact set that does not fix independent directions (J M^-1 J^T singular: e.g. a leg at a straight knee, or two 6-D contacts on one
+chain) has no unique wrench.  A world whose J M^-1 J^T + rho I has a Cholesky pivot at or below 64 eps max(diagonal) (eps of the
+arithmetic type) returns NaN in its qdd and wrench rows, and in its gradients; other worlds are unaffected.  A small rho > 0 makes the
+problem regular: it picks the solution with the least wrench norm in the limit.
+
+The reference simulator has no counterpart: it resolves contact only through its LCP step.  The work is done by libnb2.so (include/nb2.h
+``nb2_constrained_forward_dynamics`` and its backward), one warp per world.
+"""
+from __future__ import annotations
+
+import math
+from typing import Optional, Sequence
+
+import torch
+
+from .inverse_dynamics import MAX_CONTACT_BODIES, _backward_buffers, _check_fd, _input_grads, _prepare, _ptr
+from .timestep import per_world_inertia
+from .world_jacobian import _body_index, resolve_nodes
+
+_WHO = "constrained_forward_dynamics()"
+
+
+def _check_contacts(world, state, tau, nodes, offsets, damping):
+    """ValueError before any device work for a bad contact set, offsets, damping or dtype; returns the nodes as a list."""
+    _check_fd(world, state, tau, _WHO, "tau")
+    for name, t in (("state", state), ("tau", tau)):
+        if not t.dtype.is_floating_point:
+            raise ValueError(f"{_WHO}: {name} has dtype {t.dtype}, expected a floating-point tensor")
+    nodes = list(nodes)
+    if not 1 <= len(nodes) <= MAX_CONTACT_BODIES:
+        raise ValueError(f"{_WHO}: {len(nodes)} contact nodes, expected 1 to {MAX_CONTACT_BODIES}")
+    if len({id(b) for b in nodes}) != len(nodes):
+        raise ValueError(f"{_WHO}: a contact node appears twice")
+    index = _body_index(world)
+    for node in nodes:
+        if id(node) not in index:
+            raise ValueError(f"{_WHO}: body node {getattr(node, 'name', node)!r} does not belong to this world")
+        sk = node.skeleton
+        if sk is None or not sk.mobile or sk.getNumDofs() == 0:
+            raise ValueError(f"{_WHO}: body node {node.name!r} belongs to an immobile skeleton")
+    k = len(nodes)
+    if offsets is not None:
+        ok = offsets.dtype.is_floating_point and ((offsets.dim() == 2 and tuple(offsets.shape) == (k, 3)) or (
+            offsets.dim() == 3 and state.dim() == 2 and tuple(offsets.shape) == (state.shape[0], k, 3)))
+        if not ok:
+            want = f"[{k}, 3]" + (f" or [{state.shape[0]}, {k}, 3]" if state.dim() == 2 else "")
+            raise ValueError(f"{_WHO}: offsets has shape {tuple(offsets.shape)} and dtype {offsets.dtype}, expected a floating-point {want}")
+    if isinstance(damping, torch.Tensor) or not isinstance(damping, (int, float)) or not math.isfinite(damping) or damping < 0:
+        raise ValueError(f"{_WHO}: damping must be a finite float >= 0, got {damping!r}")
+    return nodes
+
+
+def _resolve(world, nodes):
+    """(canonical bodies, T12) of checked contact nodes; ValueError when two of them move with the same body."""
+    bodies, T12 = resolve_nodes(world, nodes, _WHO)
+    if len(set(bodies.tolist())) != len(nodes) or (bodies < 0).any():
+        raise ValueError(f"{_WHO}: two contact nodes move with the same body (several points on one body are not supported)")
+    return bodies, T12
+
+
+class ConstrainedForwardDynamicsLayer(torch.autograd.Function):
+    """(qdd, wrenches) of the canonical contact bodies `bodies` with placements T12 (world_jacobian.resolve_nodes); world_inertia as for
+    InverseDynamicsLayer (exclusive with the 1-D `mass`); offsets None, [k, 3] or [B, k, 3]; point and damping as
+    constrained_forward_dynamics."""
+
+    @staticmethod
+    def forward(ctx, world, state, tau, mass, world_inertia, offsets, bodies, T12, point, damping):
+        dm, sd, td, wi, need_grad = _prepare(ctx, world, state, tau, mass, world_inertia, _WHO, "tau")
+        need_grad = need_grad or ctx.needs_input_grad[5]
+        B, dev, k = ctx.B, sd.device, len(bodies)
+        od = None if offsets is None else offsets.detach().to(device=dev, dtype=sd.dtype).contiguous()
+        ctx.bodies, ctx.T12, ctx.point, ctx.damping, ctx.off_like = bodies, T12, bool(point), float(damping), offsets
+        with torch.cuda.device(dev):
+            qdd = torch.empty((B, dm.ndof), dtype=sd.dtype, device=dev)
+            wr = torch.empty((B, k, 3 if point else 6), dtype=sd.dtype, device=dev)
+            dm.constrained_forward_dynamics_device(B, sd.data_ptr(), td.data_ptr(), bodies, T12, _ptr(od), od is not None and od.dim() == 3,
+                                                   ctx.point, ctx.damping, qdd.data_ptr(), wr.data_ptr(), torch.cuda.current_stream().cuda_stream,
+                                                   ctx.prec, wi_ptr=_ptr(wi))
+        if need_grad:
+            ctx.save_for_backward(sd, td, od, wi)
+        if ctx.single:
+            qdd, wr = qdd[0], wr[0]
+        return qdd.to(device=state.device, dtype=state.dtype), wr.to(device=state.device, dtype=state.dtype)
+
+    @staticmethod
+    def backward(ctx, grad_qdd, grad_wrenches):
+        dm, B = ctx.dm, ctx.B
+        sd, td, od, wi = ctx.saved_tensors
+        dev, k = sd.device, len(ctx.bodies)
+        g = grad_qdd.detach().reshape(B, dm.ndof).to(device=dev, dtype=sd.dtype).contiguous()
+        gw = grad_wrenches.detach().reshape(B, k, 3 if ctx.point else 6).to(device=dev, dtype=sd.dtype).contiguous()
+        want_off = ctx.off_like is not None and ctx.needs_input_grad[5]
+        with torch.cuda.device(dev):
+            gs, gt, gi = _backward_buffers(ctx, dev, sd.dtype)
+            go = torch.empty((B, k, 3), dtype=sd.dtype, device=dev) if want_off else None
+            dm.constrained_forward_dynamics_backward_device(B, sd.data_ptr(), td.data_ptr(), ctx.bodies, ctx.T12, _ptr(od),
+                                                            od is not None and od.dim() == 3, ctx.point, ctx.damping, g.data_ptr(), gw.data_ptr(),
+                                                            gs.data_ptr(), gt.data_ptr(), _ptr(go), torch.cuda.current_stream().cuda_stream,
+                                                            ctx.prec, ginertia_ptr=_ptr(gi), wi_ptr=_ptr(wi))
+        if want_off:
+            if ctx.off_like.dim() == 2:  # offsets shared by the batch: the worlds' gradients add up
+                go = go.sum(dim=0)
+            go = go.to(device=ctx.off_like.device, dtype=ctx.off_like.dtype)
+        return (None,) + _input_grads(ctx, gs, gt, gi) + (go, None, None, None, None)
+
+
+def constrained_forward_dynamics(world, state: torch.Tensor, tau: torch.Tensor, contact_nodes: Sequence, offsets: Optional[torch.Tensor] = None,
+                                 point_contacts: bool = False, damping: float = 0.0, mass: Optional[torch.Tensor] = None):
+    """(qdd, wrenches): qdd [B, n] and wrenches [B, k, 6] ([B, k, 3] with point_contacts; [n] and [k, 6] / [k, 3] for a 1-D state) of every
+    world at `state` [B, 2n] under the per-dof force `tau` [B, n] with the k `contact_nodes` held (see the module docstring).
+    contact_nodes: 1 to 4 distinct BodyNodes of mobile skeletons of `world` (different skeletons allowed; a welded node counts through the
+    body it is welded to, and no two may move with the same body).  offsets: None (the nodes' origins), [k, 3] (shared by the batch) or
+    [B, k, 3], in each node's frame.  damping: rho >= 0, a float.  mass as for forward_dynamics: None, 1-D (setMasses, shared) or
+    [B, getMassDims()] (per world).  Precision follows state.dtype.  Gradients of both outputs reach state, tau, offsets and mass.
+    ValueError before any device work for a bad contact set, shape, dtype or damping."""
+    nodes = _check_contacts(world, state, tau, contact_nodes, offsets, damping)
+    if mass is not None and mass.dim() == 2:
+        wi = per_world_inertia(world, state, mass, _WHO)
+        return ConstrainedForwardDynamicsLayer.apply(world, state, tau, None, wi, offsets, *_resolve(world, nodes), point_contacts, damping)
+    bodies, T12 = _resolve(world, nodes)
+    return ConstrainedForwardDynamicsLayer.apply(world, state, tau, mass, None, offsets, bodies, T12, point_contacts, damping)

@@ -27,6 +27,7 @@
 #include "nb2_energy.h"
 #include "nb2_fd.h"
 #include "nb2_reg.h"
+#include "nb2_cfd.h"
 
 static thread_local std::string g_err;
 static std::atomic<long long> g_launches{0};
@@ -2451,6 +2452,59 @@ int nb2_energy_regressor(const nb2_model* m, int B, const void* state, void* Y_k
   static const char* who = "nb2_energy_regressor";
   if (int rc = mm_args_ok(m, B, state && Y_kinetic && Y_potential && spring_energy, who)) return rc;
   return launch_reg(m, B, state, nullptr, nullptr, nullptr, Y_kinetic, Y_potential, spring_energy, precision, stream, who);
+}
+}  // extern "C"
+
+// ---- constrained forward dynamics (nb2_cfd.cu): one warp per world, one world per block, the create-time schedule's FD model, as many row
+// slots as shared memory leaves room for.  The contacts are checked here: 1..NB2_MAX_CONTACT_BODIES distinct movable canonical bodies.
+static int launch_cfd(const nb2_model* m, int B, int k, const int32_t* body, const double* T, int point, double damping, CfdArgs a, int precision,
+                      void* stream, const char* who) {
+  if (!m || B < 0 || (B > 0 && (!a.state || !a.tau))) { g_err = std::string(who) + ": bad argument"; return NB2_ERR_INVALID; }
+  if (m->mf.ndof == 0) { g_err = std::string(who) + ": the model has no dofs"; return NB2_ERR_INVALID; }
+  if (k < 1 || k > NB2_MAX_CONTACT_BODIES || !body || !T) {
+    g_err = std::string(who) + ": " + std::to_string(k) + " contacts, expected 1.." + std::to_string(NB2_MAX_CONTACT_BODIES);
+    return NB2_ERR_INVALID;
+  }
+  for (int e = 0; e < k; e++) {
+    if (body[e] < 0 || body[e] >= m->mf.nb) { g_err = std::string(who) + ": contact " + std::to_string(e) + " names body " + std::to_string(body[e]); return NB2_ERR_INVALID; }
+    for (int f = 0; f < e; f++)
+      if (body[f] == body[e]) { g_err = std::string(who) + ": body " + std::to_string(body[e]) + " is held twice"; return NB2_ERR_INVALID; }
+  }
+  if (!(damping >= 0.0) || damping > 1.7976931348623157e308) { g_err = std::string(who) + ": damping must be finite and >= 0"; return NB2_ERR_INVALID; }
+  if (B == 0) return NB2_OK;
+  a.k = k; a.body = body; a.T = T; a.point = point ? 1 : 0; a.rho = damping;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    const Nb2ModelDev<R>& M = fd_model_of<R>(m->variants[0]);
+    size_t smem = 0;
+    const int slots = nb2_cfd_slots(M.nb, M.ndof, M.nslots, M.nfree, k * (a.point ? 3 : 6), sizeof(R), kMaxSmem, &smem);
+    if (!slots) { g_err = std::string(who) + ": the model's working set does not fit in shared memory"; return NB2_ERR_UNSUPPORTED; }
+    NB2_CUDA(nb2_cfd_launch<R>(a.gqdd != nullptr, slots, smem, (cudaStream_t)stream, M, B, a));
+    g_launches++;
+    return NB2_OK;
+  });
+}
+extern "C" {
+int nb2_constrained_forward_dynamics(const nb2_model* m, int B, const void* state, const void* tau, int k, const int32_t* body,
+                                     const double* T_owner_from_node, const void* offsets, int offsets_per_world, int point_contacts, double damping,
+                                     const double* world_inertia, void* accel, void* wrenches, int precision, void* stream) {
+  static const char* who = "nb2_constrained_forward_dynamics";
+  if (B > 0 && (!accel || !wrenches)) { g_err = std::string(who) + ": bad argument"; return NB2_ERR_INVALID; }
+  CfdArgs a{};
+  a.state = state; a.tau = tau; a.off = offsets; a.off_pw = offsets_per_world; a.wi = world_inertia; a.qdd = accel; a.wrench = wrenches;
+  return launch_cfd(m, B, k, body, T_owner_from_node, point_contacts, damping, a, precision, stream, who);
+}
+int nb2_constrained_forward_dynamics_backward(const nb2_model* m, int B, const void* state, const void* tau, int k, const int32_t* body,
+                                              const double* T_owner_from_node, const void* offsets, int offsets_per_world, int point_contacts,
+                                              double damping, const double* world_inertia, const void* grad_accel, const void* grad_wrenches,
+                                              void* grad_state, void* grad_tau, void* grad_offsets, double* grad_inertia, int precision,
+                                              void* stream) {
+  static const char* who = "nb2_constrained_forward_dynamics_backward";
+  if (B > 0 && (!grad_accel || !grad_wrenches || !grad_state || !grad_tau)) { g_err = std::string(who) + ": bad argument"; return NB2_ERR_INVALID; }
+  CfdArgs a{};
+  a.state = state; a.tau = tau; a.off = offsets; a.off_pw = offsets_per_world; a.wi = world_inertia;
+  a.gqdd = grad_accel; a.gw = grad_wrenches; a.gstate = grad_state; a.gtau = grad_tau; a.goff = grad_offsets; a.gI = grad_inertia;
+  return launch_cfd(m, B, k, body, T_owner_from_node, point_contacts, damping, a, precision, stream, who);
 }
 int nb2_model_ndof(const nb2_model* m) { return m ? m->mf.ndof : -1; }
 int nb2_model_na(const nb2_model* m) { return m ? m->mf.na : -1; }

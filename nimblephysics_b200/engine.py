@@ -301,6 +301,27 @@ class DeviceModel:
         """Y_kinetic, Y_potential [B, nb, 10] and the spring energy [B] at states [B, 2n] (include/nb2.h nb2_energy_regressor)."""
         _cabi.check(_cabi.lib().nb2_energy_regressor(self.handle, B, state_ptr, YT_ptr, YU_ptr, spring_ptr, precision, stream))
 
+    def constrained_forward_dynamics_device(self, B, state_ptr, tau_ptr, bodies, T12, off_ptr, off_per_world, point, damping, qdd_ptr, wrench_ptr,
+                                            stream, precision=FP32, wi_ptr=None):
+        """qdd [B, n] and contact wrenches [B, k, 6 or 3] with the bodies held (include/nb2.h nb2_constrained_forward_dynamics); bodies [k]
+        int32 and T12 [k, 12] fp64 are host arrays."""
+        b = np.ascontiguousarray(bodies, np.int32)
+        T = np.ascontiguousarray(T12, np.float64)
+        _cabi.check(_cabi.lib().nb2_constrained_forward_dynamics(self.handle, B, state_ptr, tau_ptr, len(b), b.ctypes.data, T.ctypes.data, off_ptr,
+                                                                 int(off_per_world), int(point), float(damping), wi_ptr, qdd_ptr, wrench_ptr,
+                                                                 precision, stream))
+
+    def constrained_forward_dynamics_backward_device(self, B, state_ptr, tau_ptr, bodies, T12, off_ptr, off_per_world, point, damping, gqdd_ptr,
+                                                     gwrench_ptr, gstate_ptr, gtau_ptr, goff_ptr, stream, precision=FP32, ginertia_ptr=None,
+                                                     wi_ptr=None):
+        """VJP of constrained_forward_dynamics_device; goff_ptr: optional [B, k, 3], ginertia_ptr: optional [10*nb, B] float64."""
+        b = np.ascontiguousarray(bodies, np.int32)
+        T = np.ascontiguousarray(T12, np.float64)
+        _cabi.check(_cabi.lib().nb2_constrained_forward_dynamics_backward(self.handle, B, state_ptr, tau_ptr, len(b), b.ctypes.data, T.ctypes.data,
+                                                                          off_ptr, int(off_per_world), int(point), float(damping), wi_ptr, gqdd_ptr,
+                                                                          gwrench_ptr, gstate_ptr, gtau_ptr, goff_ptr, ginertia_ptr, precision,
+                                                                          stream))
+
     def contact_workspace_bytes(self, B):
         return int(_cabi.lib().nb2_contact_workspace_bytes(self.handle, B))
 

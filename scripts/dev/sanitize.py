@@ -1,7 +1,7 @@
 """Small end-to-end run for compute-sanitizer (memcheck): contact-free fwd+bwd (device + pinned-host paths, partial groups),
 contact fwd+bwd, fused rollout, inverse dynamics, contact and multiple-contact inverse dynamics fwd+bwd, the mass matrix and its inverse fwd+bwd, the world and COM Jacobians
 and their time derivatives fwd+bwd, forward dynamics fwd+bwd, the pointer-style forward dynamics and the dense Jacobians of inverse and
-forward dynamics and the inverse-dynamics and energy regressors (both precisions, per-world masses and offsets, partial groups and partial blocks)."""
+forward dynamics, the inverse-dynamics and energy regressors and constrained forward dynamics fwd+bwd (both precisions, per-world masses and offsets, partial groups and partial blocks)."""
 import sys
 import numpy as np, torch
 sys.path.insert(0, ".")
@@ -56,6 +56,10 @@ for B in (7, 203):
         sum(x.sum() for x in nb.energy_and_momentum(mw, st, mw.skeletons[0], mass * torch.tensor(mw.getMasses(), device="cuda"))).backward()
         nb.inverse_dynamics_regressor(mw, st, vn)
         nb.energy_regressor(mw, st)
+        q2, w2 = nb.constrained_forward_dynamics(mw, st, tau, bodies, off, mass=mass * torch.tensor(mw.getMasses(), device="cuda"))
+        (q2.sum() + w2.sum()).backward()
+        q2, w2 = nb.constrained_forward_dynamics(mw, st, tau, bodies, point_contacts=True, damping=1e-3)
+        (q2.sum() + w2.sum()).backward()
     sd = torch.tensor(s, device="cuda", dtype=torch.float64)
     nb.device_model_for(w).forward_dynamics(sd[:, :raw.ndof], sd[:, raw.ndof:], sd[:, raw.ndof:] * 10)
 torch.cuda.synchronize()
