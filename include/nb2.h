@@ -402,6 +402,21 @@ int nb2_constrained_forward_dynamics_backward(const nb2_model* m, int B, const v
                                               double damping, const double* world_inertia, const void* grad_accel, const void* grad_wrenches,
                                               void* grad_state, void* grad_tau, void* grad_offsets, double* grad_inertia, int precision,
                                               void* stream);
+/* Dense Jacobians of constrained forward dynamics (DESIGN.md §6p), in one launch.  Arguments as nb2_constrained_forward_dynamics, whose
+ * accel [B, ndof] and wrenches [B, k, r] (r = 6, or 3 with point_contacts) it also writes, with m = k r and
+ *     J_q, J_qdot, J_tau [B, ndof, ndof] :  J_x[w, i, j] = d accel[w, i] / d x[w, j] ,
+ *     W_q, W_qdot, W_tau [B, m, ndof]    :  W_x[w, i r + c, j] = d wrenches[w, i, c] / d x[w, j] ,
+ * x = the positions, the velocities (both halves of state) and tau.  Row i of each block is nb2_constrained_forward_dynamics_backward
+ * with the seed e_i on that output, so free joints follow its conventions (position columns for the six stored coordinates, body-twist
+ * velocity columns) and the blocks equal the VJP's rows up to rounding.  accel and the wrenches are written by the forward of
+ * nb2_constrained_forward_dynamics itself (a second launch on the stream), so they equal its outputs bit for bit.  Offsets and masses are
+ * held fixed.  A singular world gets NaN in
+ * its outputs and every block.  Stateless, stream-ordered, nothing allocated, B = 0 only validates.  NB2_ERR_INVALID as
+ * nb2_constrained_forward_dynamics; NB2_ERR_UNSUPPORTED when the working set does not fit shared memory even at one row slot. */
+int nb2_constrained_forward_dynamics_jacobians(const nb2_model* m, int B, const void* state, const void* tau, int k, const int32_t* body,
+                                                const double* T_owner_from_node, const void* offsets, int offsets_per_world, int point_contacts,
+                                                double damping, const double* world_inertia, void* accel, void* wrenches, void* J_q, void* J_qdot,
+                                                void* J_tau, void* W_q, void* W_qdot, void* W_tau, int precision, void* stream);
 
 /* Batched boxed-LCP solves on the device: B independent problems, one warp each — the reference's pointer-style lower boundary
  * BoxedLcpSolver::solve(n, A, x, b, nub, lo, hi, findex, earlyTermination) (dart/constraint/BoxedLcpSolver.hpp:125-135) and the

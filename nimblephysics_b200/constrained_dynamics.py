@@ -23,8 +23,11 @@ chain) has no unique wrench.  A world whose J M^-1 J^T + rho I has a Cholesky pi
 arithmetic type) returns NaN in its qdd and wrench rows, and in its gradients; other worlds are unaffected.  A small rho > 0 makes the
 problem regular: it picks the solution with the least wrench norm in the limit.
 
+``constrained_forward_dynamics_jacobians`` returns qdd, the wrenches and their dense Jacobians in state and tau in one launch, for iLQR /
+DDP, linearised MPC and contact-force constraints that need the matrices rather than products with one gradient.
+
 The reference simulator has no counterpart: it resolves contact only through its LCP step.  The work is done by libnb2.so (include/nb2.h
-``nb2_constrained_forward_dynamics`` and its backward), one warp per world.
+``nb2_constrained_forward_dynamics``, its backward and ``nb2_constrained_forward_dynamics_jacobians``), one warp per world.
 """
 from __future__ import annotations
 
@@ -33,48 +36,50 @@ from typing import Optional, Sequence
 
 import torch
 
+from .engine import FP32, FP64, device_model_for
 from .inverse_dynamics import MAX_CONTACT_BODIES, _backward_buffers, _check_fd, _input_grads, _prepare, _ptr
-from .timestep import per_world_inertia
+from .timestep import _word_major_inertia, per_world_inertia, set_shared_masses
 from .world_jacobian import _body_index, resolve_nodes
 
 _WHO = "constrained_forward_dynamics()"
+_WHO_J = "constrained_forward_dynamics_jacobians()"
 
 
-def _check_contacts(world, state, tau, nodes, offsets, damping):
+def _check_contacts(world, state, tau, nodes, offsets, damping, who=_WHO):
     """ValueError before any device work for a bad contact set, offsets, damping or dtype; returns the nodes as a list."""
-    _check_fd(world, state, tau, _WHO, "tau")
+    _check_fd(world, state, tau, who, "tau")
     for name, t in (("state", state), ("tau", tau)):
         if not t.dtype.is_floating_point:
-            raise ValueError(f"{_WHO}: {name} has dtype {t.dtype}, expected a floating-point tensor")
+            raise ValueError(f"{who}: {name} has dtype {t.dtype}, expected a floating-point tensor")
     nodes = list(nodes)
     if not 1 <= len(nodes) <= MAX_CONTACT_BODIES:
-        raise ValueError(f"{_WHO}: {len(nodes)} contact nodes, expected 1 to {MAX_CONTACT_BODIES}")
+        raise ValueError(f"{who}: {len(nodes)} contact nodes, expected 1 to {MAX_CONTACT_BODIES}")
     if len({id(b) for b in nodes}) != len(nodes):
-        raise ValueError(f"{_WHO}: a contact node appears twice")
+        raise ValueError(f"{who}: a contact node appears twice")
     index = _body_index(world)
     for node in nodes:
         if id(node) not in index:
-            raise ValueError(f"{_WHO}: body node {getattr(node, 'name', node)!r} does not belong to this world")
+            raise ValueError(f"{who}: body node {getattr(node, 'name', node)!r} does not belong to this world")
         sk = node.skeleton
         if sk is None or not sk.mobile or sk.getNumDofs() == 0:
-            raise ValueError(f"{_WHO}: body node {node.name!r} belongs to an immobile skeleton")
+            raise ValueError(f"{who}: body node {node.name!r} belongs to an immobile skeleton")
     k = len(nodes)
     if offsets is not None:
         ok = offsets.dtype.is_floating_point and ((offsets.dim() == 2 and tuple(offsets.shape) == (k, 3)) or (
             offsets.dim() == 3 and state.dim() == 2 and tuple(offsets.shape) == (state.shape[0], k, 3)))
         if not ok:
             want = f"[{k}, 3]" + (f" or [{state.shape[0]}, {k}, 3]" if state.dim() == 2 else "")
-            raise ValueError(f"{_WHO}: offsets has shape {tuple(offsets.shape)} and dtype {offsets.dtype}, expected a floating-point {want}")
+            raise ValueError(f"{who}: offsets has shape {tuple(offsets.shape)} and dtype {offsets.dtype}, expected a floating-point {want}")
     if isinstance(damping, torch.Tensor) or not isinstance(damping, (int, float)) or not math.isfinite(damping) or damping < 0:
-        raise ValueError(f"{_WHO}: damping must be a finite float >= 0, got {damping!r}")
+        raise ValueError(f"{who}: damping must be a finite float >= 0, got {damping!r}")
     return nodes
 
 
-def _resolve(world, nodes):
+def _resolve(world, nodes, who=_WHO):
     """(canonical bodies, T12) of checked contact nodes; ValueError when two of them move with the same body."""
-    bodies, T12 = resolve_nodes(world, nodes, _WHO)
+    bodies, T12 = resolve_nodes(world, nodes, who)
     if len(set(bodies.tolist())) != len(nodes) or (bodies < 0).any():
-        raise ValueError(f"{_WHO}: two contact nodes move with the same body (several points on one body are not supported)")
+        raise ValueError(f"{who}: two contact nodes move with the same body (several points on one body are not supported)")
     return bodies, T12
 
 
@@ -139,3 +144,49 @@ def constrained_forward_dynamics(world, state: torch.Tensor, tau: torch.Tensor, 
         return ConstrainedForwardDynamicsLayer.apply(world, state, tau, None, wi, offsets, *_resolve(world, nodes), point_contacts, damping)
     bodies, T12 = _resolve(world, nodes)
     return ConstrainedForwardDynamicsLayer.apply(world, state, tau, mass, None, offsets, bodies, T12, point_contacts, damping)
+
+
+def constrained_forward_dynamics_jacobians(world, state: torch.Tensor, tau: torch.Tensor, contact_nodes: Sequence,
+                                           offsets: Optional[torch.Tensor] = None, point_contacts: bool = False, damping: float = 0.0,
+                                           mass: Optional[torch.Tensor] = None):
+    """(qdd, wrenches, dqdd_dq, dqdd_dqdot, dqdd_dtau, dwrench_dq, dwrench_dqdot, dwrench_dtau): the outputs of
+    constrained_forward_dynamics for the same arguments and their dense Jacobians in the layout of torch.autograd.functional.jacobian,
+    dqdd_dx [B, n, n] and dwrench_dx [B, k, r, n] (r = 6, or 3 with point_contacts), entry [w, ..., j] = d out / d x_j, x = the positions,
+    the velocities and tau.  Row i of each block is constrained_forward_dynamics's vector-Jacobian product with the seed e_i on that output,
+    so the blocks equal autograd's Jacobian up to rounding; free joints follow its conventions (position columns for the six stored
+    coordinates, body-twist velocity columns) and the wrenches are about the world origin.  From the definition, with A = J M^-1 J^T + rho I:
+
+        dqdd_dtau = M^-1 - M^-1 J^T A^-1 J M^-1 ,   dlam_dtau = -A^-1 J M^-1 ,   J dqdd_dtau = -rho dlam_dtau .
+
+    Arguments, shapes, masses and precision as constrained_forward_dynamics; a 1-D state gives the same blocks without B.  The outputs carry
+    no autograd history: there are no second derivatives and no offset or mass Jacobian.  A singular world gets NaN in every output and
+    block.  ValueError before any device work for the argument errors of constrained_forward_dynamics."""
+    nodes = _check_contacts(world, state, tau, contact_nodes, offsets, damping, _WHO_J)
+    wi = per_world_inertia(world, state, mass, _WHO_J) if mass is not None and mass.dim() == 2 else None
+    bodies, T12 = _resolve(world, nodes, _WHO_J)
+    dm = set_shared_masses(world, mass, _WHO_J) if mass is not None and wi is None else device_model_for(world)
+    if not torch.cuda.is_available():
+        raise RuntimeError(f"nimblephysics_b200.{_WHO_J[:-2]} needs a CUDA device; there is no CPU fallback")
+    single = state.dim() == 1
+    s2 = state.detach().reshape(1, -1) if single else state.detach()
+    t2 = tau.detach().reshape(1, -1) if single else tau.detach()
+    dev = s2.device if s2.is_cuda else torch.device("cuda", torch.cuda.current_device())
+    rdt = torch.float64 if state.dtype == torch.float64 else torch.float32
+    sd = s2.to(device=dev, dtype=rdt).contiguous()
+    td = t2.to(device=dev, dtype=rdt).contiguous()
+    od = None if offsets is None else offsets.detach().to(device=dev, dtype=rdt).contiguous()
+    B, n, k, r = sd.shape[0], dm.ndof, len(nodes), 3 if point_contacts else 6
+    with torch.cuda.device(dev):
+        qdd = torch.empty((B, n), dtype=rdt, device=dev)
+        wr = torch.empty((B, k, r), dtype=rdt, device=dev)
+        J = [torch.empty((B, n, n), dtype=rdt, device=dev) for _ in range(3)] + [torch.empty((B, k, r, n), dtype=rdt, device=dev) for _ in range(3)]
+        if B > 0:  # an empty batch has no rows to hand over (its data pointers may be NULL)
+            dm.constrained_forward_dynamics_jacobians_device(B, sd.data_ptr(), td.data_ptr(), bodies, T12, _ptr(od), od is not None and od.dim() == 3,
+                                                             bool(point_contacts), float(damping), qdd.data_ptr(), wr.data_ptr(),
+                                                             [x.data_ptr() for x in J], torch.cuda.current_stream().cuda_stream,
+                                                             FP64 if rdt == torch.float64 else FP32,
+                                                             wi_ptr=_ptr(_word_major_inertia(dm, wi, B, dev)))
+    res = [qdd, wr] + J
+    if single:
+        res = [x[0] for x in res]
+    return tuple(x.to(device=state.device, dtype=state.dtype) for x in res)

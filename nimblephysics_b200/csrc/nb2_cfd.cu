@@ -41,21 +41,17 @@ cudaError_t launch(size_t smem, cudaStream_t s, const Nb2ModelDev<R>& M, const n
 
 }  // namespace
 
-int nb2_cfd_slots(int nb, int n, int nslots, int nfree, int m, size_t word, size_t max_smem, size_t* smem) {
+int nb2_cfd_slots(int nb, int n, int nslots, int nfree, int m, int jac, size_t word, size_t max_smem, size_t* smem) {
   for (int st = 8; st >= 1; st = st == 8 ? 1 : 0) {
-    const size_t bytes = (size_t)nb2::cfd_layout(nb, n, nslots, nfree, m, st).total * word;
+    const int words = jac ? nb2::cfdj_layout(nb, n, nslots, nfree, m, st).total : nb2::cfd_layout(nb, n, nslots, nfree, m, st).total;
+    const size_t bytes = (size_t)words * word;
     if (bytes <= max_smem) { *smem = bytes; return st; }
   }
   return 0;
 }
 template <class R>
 cudaError_t nb2_cfd_launch(int bwd, int slots, size_t smem, cudaStream_t s, const Nb2ModelDev<R>& M, int B, const CfdArgs& a) {
-  nb2::CfdNodes<R> N;
-  N.k = a.k; N.point = a.point;
-  for (int e = 0; e < NB2_MAX_CONTACT_BODIES; e++) {
-    N.body[e] = e < a.k ? a.body[e] : -1;
-    for (int c = 0; c < 12; c++) N.T[e][c] = e < a.k ? (R)a.T[12 * e + c] : R(0);
-  }
+  const nb2::CfdNodes<R> N = nb2::cfd_nodes<R>(a.k, a.point, a.body, a.T);
   if (slots == 8) return bwd ? launch<R, 8, true>(smem, s, M, N, B, a) : launch<R, 8, false>(smem, s, M, N, B, a);
   return bwd ? launch<R, 1, true>(smem, s, M, N, B, a) : launch<R, 1, false>(smem, s, M, N, B, a);
 }

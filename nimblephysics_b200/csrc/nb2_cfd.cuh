@@ -21,6 +21,8 @@
 //   dL/dqdot += -Jdot^T mu - d<mu, Jdot qdot>/dqdot|_Jdot (jpdb_*),   dL/do_i from both.
 // A 6-D output is the wrench about the world origin, [lam_a + p x lam_l ; lam_l]; its seed wbar becomes lambar = [wbar_a ; wbar_l +
 // wbar_a x p] and adds pbar = lam_l x wbar_a to the point, which jpdb_reduce carries to q and the offset with the point's own adjoint.
+//
+// Dense Jacobians (cfdj_world, §6p): the forward of cfd_world once, then the backward above per seed e_i, in rounds of ST seeds.
 #pragma once
 #include <math.h>
 
@@ -37,6 +39,16 @@ template <class R> struct CfdNodes {
   int body[NB2_MAX_CONTACT_BODIES];
   R T[NB2_MAX_CONTACT_BODIES][12];
 };
+// k contacts from the host's canonical bodies and body <- node transforms [k][12] (fp64); unused entries -1 / 0
+template <class R> inline CfdNodes<R> cfd_nodes(int k, int point, const int32_t* body, const double* T) {
+  CfdNodes<R> N;
+  N.k = k; N.point = point;
+  for (int e = 0; e < NB2_MAX_CONTACT_BODIES; e++) {
+    N.body[e] = e < k ? body[e] : -1;
+    for (int c = 0; c < 12; c++) N.T[e][c] = e < k ? (R)T[12 * e + c] : R(0);
+  }
+  return N;
+}
 // one world's rows.  Forward: state [2n], tau [n], offsets ([k][3], or NULL), qdd [n], wrench [k][6 or 3].  Backward adds the seeds gqdd
 // [n] and gw [k][6 or 3] and writes gstate [2n], gtau [n], goff [k][3] (or NULL) and gI (word-major [10 nb][wiB], or NULL).
 template <class R> struct CfdRows {
@@ -116,6 +128,78 @@ template <class R> NB2_HD void cfd_solve(const R* A, int m, R* x) {
 // stream written)
 template <class R, class Stage> NB2_HD void cfd_fd_forward(const Nb2ModelDev<R>& M, R* ws, const double* wi, size_t wiB, Stage&& stage) {
   for (int sg = 1; sg < NB2_FWD_STAGES - 1; sg++) stage([&](int lane, int) { dj_forward_stage<R, true>(M, ws, lane, sg, wi, wiB); });
+}
+
+// contact i's wrench seed gw (its 6 or 3 entries) in point form: lambar lb and the point adjoint pb.  lb may be gw (every entry is read
+// before any is written).
+template <class R> NB2_HD void cfd_point_form(const CfdNodes<R>& N, const CfdLayout& L, const R* ws, int i, const R* gw, R* lb, R* pb) {
+  if (N.point) {
+    for (int j = 0; j < 3; j++) { lb[j] = gw[j]; pb[j] = R(0); }
+    return;
+  }
+  const V3<R> ga = mk3<R>(gw[0], gw[1], gw[2]), p = mk3<R>(ws[L.oP + 3 * i], ws[L.oP + 3 * i + 1], ws[L.oP + 3 * i + 2]);
+  const R* lam = ws + L.oC + 6 * i;
+  const V3<R> gl = mk3<R>(gw[3], gw[4], gw[5]) + cross(ga, p), pbar = cross(mk3<R>(lam[3], lam[4], lam[5]), ga);
+  lb[0] = ga.x; lb[1] = ga.y; lb[2] = ga.z; lb[3] = gl.x; lb[4] = gl.y; lb[5] = gl.z;
+  pb[0] = pbar.x; pb[1] = pbar.y; pb[2] = pbar.z;
+}
+
+// one seed's point-Jacobian VJPs, added to its [dL/dq ; dL/dqdot] G: J with lam u^T - mu qdd^T, then Jdot with -mu qdot^T and the points'
+// own adjoints pb, and -Jdot^T mu.  The offset gradients land in the go words.  The walks are seed-free, but jpdb_terms overwrites its
+// walk's screws and velocities in place, so each seed walks again.
+template <class R, class Stage>
+NB2_HD void cfd_point_vjps(const Nb2ModelDev<R>& M, const CfdNodes<R>& N, const CfdRows<R>& io, const CfdLayout& L, R* ws, const R* mu,
+                           const R* u, const R* pb, R* G, Stage&& stage) {
+  const int n = M.ndof, k = N.k, rpc = N.point ? 3 : 6, r0c = N.point ? 3 : 0, m = k * rpc;
+  const FwdLayout F = fwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
+  const R* s = io.state;
+  const R* qd = s + n;
+  R* K = ws + L.oK;
+  R* gb = ws + L.oGb;
+  for (int deriv = 0; deriv < 2; deriv++) {
+    if (deriv) stage([&](int lane, int nl) { jpdb_init<R>(M, K, lane, nl); });
+    else stage([&](int lane, int nl) { jpb_init<R>(M, K, lane, nl); });
+    for (int i = 0; i < k; i++) {
+      const int b = N.body[i];
+      const R* o = io.off ? io.off + 3 * i : nullptr;
+      R* go = ws + L.oGo + 12 * deriv + 3 * i;
+      stage([&](int lane, int nl) {
+        for (int idx = lane; idx < 6 * n; idx += nl) {
+          const int row = idx / n, d = idx - row * n, j = row - r0c;
+          R g = R(0);
+          if (j >= 0) {
+            const int r = i * rpc + j;
+            g = deriv ? -mu[r] * qd[d] : ws[L.oC + r] * u[d] - mu[r] * ws[F.oAct + d];
+          }
+          gb[idx] = g;
+        }
+      });
+      if (deriv) {
+        stage([&](int lane, int) { jpdb_walk<R>(M, s, qd, b, N.T[i], o, K, lane); });
+        stage([&](int lane, int nl) { jpdb_terms<R>(M, b, gb, K, lane, nl); });
+        stage([&](int lane, int) {
+          if (lane == 0) for (int c = 0; c < 3; c++) K[jpdb_layout(M.nb, n).oPP + 3 + c] += pb[3 * i + c];
+        });
+        stage([&](int lane, int) { jpdb_reduce<R>(M, s, qd, b, K, go, lane); });
+      } else {
+        stage([&](int lane, int) { jpb_walk<R>(M, s, b, N.T[i], o, K, lane); });
+        stage([&](int lane, int nl) { jpb_terms<R>(M, b, gb, K, lane, nl); });
+        stage([&](int lane, int) { jpb_reduce<R>(M, s, b, K, go, lane); });
+      }
+    }
+    stage([&](int lane, int nl) {
+      for (int d = lane; d < n; d += nl) {
+        if (deriv) {
+          R v = K[jpdb_layout(M.nb, n).oGq + n + d];
+          for (int r = 0; r < m; r++) v -= ws[L.oJd + r * n + d] * mu[r];
+          G[d] += K[jpdb_layout(M.nb, n).oGq + d];
+          G[n + d] += v;
+        } else {
+          G[d] += K[jpb_layout(M.nb, n).oGq + d];
+        }
+      }
+    });
+  }
 }
 
 // The program of one world.  BWD: the backward recomputes the forward (nothing is kept between the calls) and continues.
@@ -315,6 +399,102 @@ NB2_HD void cfd_world(const Nb2ModelDev<R>& M, const CfdNodes<R>& N, const CfdRo
     if (io.gI && bad)
       for (int idx = lane; idx < 10 * M.nb; idx += nl) io.gI[(size_t)idx * io.wiB] = (double)cfd_nan<R>();
   });
+}
+
+// ---- dense Jacobians (DESIGN.md §6p).  Row i of each block is the VJP above with the seed e_i on one output: n seeds on qdd, then m on
+// the wrenches.  The forward is cfd_world's own, run once; the seed-free words it leaves (J, Jdot, Y, the factor, lam, qdd, the saved
+// stream) serve every row.  Rounds of ST seeds: seed t's backward words sit in the extension below, its FD backward runs in row slot t,
+// swept by thread t over every lane of the schedule (as k_dj's rows), and the point-Jacobian VJPs take the seeds one after the other on
+// the warp.  The world's blocks: dqdd/dq, dqdd/dqdot, dqdd/dtau [n][n] and dwrench/dq, dwrench/dqdot, dwrench/dtau [m][n], row-major.
+template <class R> struct CfdJacRows { R* Jq; R* Jqd; R* Jt; R* Wq; R* Wqd; R* Wt; };
+// the working set: cfd_layout's, then per seed slot t mu [m], lambar [m], pbar [12], qddbar [n], [dL/dq ; dL/dqdot] [2n], u [n]
+struct CfdjLayout { CfdLayout C; int oMu, oLb, oPb, oQb, oG, oU, total; };
+NB2_HD CfdjLayout cfdj_layout(int nb, int n, int nslots, int nfree, int m, int st) {
+  CfdjLayout L;
+  L.C = cfd_layout(nb, n, nslots, nfree, m, st);
+  L.oMu = L.C.total; L.oLb = L.oMu + st * m; L.oPb = L.oLb + st * m; L.oQb = L.oPb + 12 * st; L.oG = L.oQb + st * n; L.oU = L.oG + 2 * n * st;
+  L.total = L.oU + n * st;
+  return L;
+}
+
+template <class R, int ST, class Stage>
+NB2_HD void cfdj_world(const Nb2ModelDev<R>& M, const CfdNodes<R>& N, const CfdRows<R>& io, const CfdJacRows<R>& out, R* ws, Stage&& stage) {
+  const int n = M.ndof, k = N.k, rpc = N.point ? 3 : 6, m = k * rpc, rows = n + m;
+  const CfdjLayout X = cfdj_layout(M.nb, M.ndof, M.nslots, M.nfree, m, ST);
+  const CfdLayout& L = X.C;
+  const BwdLayout BL = bwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
+  const R* s = io.state;
+  cfd_world<R, ST, false>(M, N, io, ws, stage);  // qdd and the wrenches written
+  for (int s0 = 0; s0 < rows; s0 += ST) {
+    const int ns = (rows - s0 < ST) ? rows - s0 : ST;
+    // the seeds: e_row on qdd (row < n) or on the wrench entry row - n; then in point form, in place
+    stage([&](int lane, int nl) {
+      for (int idx = lane; idx < ns * rows; idx += nl) {
+        const int t = idx / rows, e = idx - t * rows;
+        if (e < n) ws[X.oQb + t * n + e] = (s0 + t == e) ? R(1) : R(0);
+        else ws[X.oLb + t * m + e - n] = (s0 + t == e) ? R(1) : R(0);
+      }
+    });
+    stage([&](int lane, int nl) {
+      for (int idx = lane; idx < ns * k; idx += nl) {
+        const int t = idx / k, i = idx - t * k;
+        R* lb = ws + X.oLb + t * m + i * rpc;
+        cfd_point_form<R>(N, L, ws, i, lb, lb, ws + X.oPb + 12 * t + 3 * i);
+      }
+    });
+    // mu = (J M^-1 J^T + rho I)^-1 (lambar + Y qddbar), slot t on lane t
+    stage([&](int lane, int nl) {
+      for (int idx = lane; idx < ns * m; idx += nl) {
+        const int t = idx / m, r = idx - t * m;
+        R v = ws[X.oLb + t * m + r];
+        for (int d = 0; d < n; d++) v += ws[L.oY + r * n + d] * ws[X.oQb + t * n + d];
+        ws[X.oMu + t * m + r] = v;
+      }
+    });
+    stage([&](int lane, int) { if (lane < ns && ws[L.oFlag] == R(0)) cfd_solve<R>(ws + L.oA, m, ws + X.oMu + lane * m); });
+    // g = qddbar - J^T mu, the FD backward seeded with g (slot t on thread t), then its rows
+    stage([&](int lane, int nl) {
+      for (int idx = lane; idx < ns * n; idx += nl) {
+        const int t = idx / n, d = idx - t * n;
+        R* rb = ws + L.D.oB + t;
+        R g = ws[X.oQb + t * n + d];
+        for (int r = 0; r < m; r++) g -= ws[L.oJ + r * n + d] * ws[X.oMu + t * m + r];
+        rb[(size_t)(BL.oGV + d) * ST] = g;
+        rb[(size_t)(BL.oSt + d) * ST] = s[d];
+        rb[(size_t)(BL.oSt + n + d) * ST] = s[n + d];
+      }
+    });
+    stage([&](int lane, int) {
+      if (lane >= ns) return;
+      R* rb = ws + L.D.oB + lane;
+      for (int sg = 1; sg < NB2_BWD_STAGES - 1; sg++)
+        for (int l = 0; l < M.lanes; l++) fd_backward_stage<R, ST>(M, rb, ws + L.D.oS, 1, l, sg, nullptr, io.wi, io.wiB, nullptr, 0);
+    });
+    stage([&](int lane, int nl) {
+      for (int idx = lane; idx < ns * n; idx += nl) {
+        const int t = idx / n, d = idx - t * n;
+        const R* rb = ws + L.D.oB + t;
+        ws[X.oG + 2 * n * t + d] = rb[(size_t)(BL.oQb + d) * ST];
+        ws[X.oG + 2 * n * t + n + d] = rb[(size_t)(BL.oVb + d) * ST];
+        ws[X.oU + n * t + d] = rb[(size_t)(BL.oLam + d) * ST];
+      }
+    });
+    for (int t = 0; t < ns; t++)
+      cfd_point_vjps<R>(M, N, io, L, ws, ws + X.oMu + t * m, ws + X.oU + t * n, ws + X.oPb + 12 * t, ws + X.oG + 2 * n * t, stage);
+    // the round's rows, in address order within each block
+    stage([&](int lane, int nl) {
+      const bool bad = ws[L.oFlag] != R(0);
+      for (int idx = lane; idx < ns * n; idx += nl) {
+        const int t = idx / n, j = idx - t * n, row = s0 + t;
+        const bool acc = row < n;
+        const size_t e = (size_t)(acc ? row : row - n) * n + j;
+        const R gq = ws[X.oG + 2 * n * t + j], gv = ws[X.oG + 2 * n * t + n + j], gt = ws[X.oU + n * t + j];
+        (acc ? out.Jq : out.Wq)[e] = bad ? cfd_nan<R>() : gq;
+        (acc ? out.Jqd : out.Wqd)[e] = bad ? cfd_nan<R>() : gv;
+        (acc ? out.Jt : out.Wt)[e] = bad ? cfd_nan<R>() : gt;
+      }
+    });
+  }
 }
 
 }  // namespace nb2

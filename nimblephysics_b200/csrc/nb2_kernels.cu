@@ -2455,8 +2455,9 @@ int nb2_energy_regressor(const nb2_model* m, int B, const void* state, void* Y_k
 }
 }  // extern "C"
 
-// ---- constrained forward dynamics (nb2_cfd.cu): one warp per world, one world per block, the create-time schedule's FD model, as many row
-// slots as shared memory leaves room for.  The contacts are checked here: 1..NB2_MAX_CONTACT_BODIES distinct movable canonical bodies.
+// ---- constrained forward dynamics (nb2_cfd.cu; its dense Jacobians nb2_cfdj.cu): one warp per world, one world per block, the create-time
+// schedule's FD model, as many row slots as shared memory leaves room for.  The contacts are checked here: 1..NB2_MAX_CONTACT_BODIES
+// distinct movable canonical bodies.
 static int launch_cfd(const nb2_model* m, int B, int k, const int32_t* body, const double* T, int point, double damping, CfdArgs a, int precision,
                       void* stream, const char* who) {
   if (!m || B < 0 || (B > 0 && (!a.state || !a.tau))) { g_err = std::string(who) + ": bad argument"; return NB2_ERR_INVALID; }
@@ -2477,9 +2478,19 @@ static int launch_cfd(const nb2_model* m, int B, int k, const int32_t* body, con
     using R = decltype(r);
     const Nb2ModelDev<R>& M = fd_model_of<R>(m->variants[0]);
     size_t smem = 0;
-    const int slots = nb2_cfd_slots(M.nb, M.ndof, M.nslots, M.nfree, k * (a.point ? 3 : 6), sizeof(R), kMaxSmem, &smem);
+    const int slots = nb2_cfd_slots(M.nb, M.ndof, M.nslots, M.nfree, k * (a.point ? 3 : 6), a.J[0] != nullptr, sizeof(R), kMaxSmem, &smem);
     if (!slots) { g_err = std::string(who) + ": the model's working set does not fit in shared memory"; return NB2_ERR_UNSUPPORTED; }
-    NB2_CUDA(nb2_cfd_launch<R>(a.gqdd != nullptr, slots, smem, (cudaStream_t)stream, M, B, a));
+    if (a.J[0]) {
+      NB2_CUDA(nb2_cfdj_launch<R>(slots, smem, (cudaStream_t)stream, M, B, a));
+      g_launches++;
+      // then k_cfd's own forward rewrites accel and the wrenches, so that they are nb2_constrained_forward_dynamics's bit for bit: the
+      // Jacobian kernel runs the same program, but compiled into another kernel it is not rounded identically (ulp-level differences)
+      size_t fsmem = 0;
+      const int fslots = nb2_cfd_slots(M.nb, M.ndof, M.nslots, M.nfree, k * (a.point ? 3 : 6), 0, sizeof(R), kMaxSmem, &fsmem);
+      NB2_CUDA(nb2_cfd_launch<R>(0, fslots, fsmem, (cudaStream_t)stream, M, B, a));
+    } else {
+      NB2_CUDA(nb2_cfd_launch<R>(a.gqdd != nullptr, slots, smem, (cudaStream_t)stream, M, B, a));
+    }
     g_launches++;
     return NB2_OK;
   });
@@ -2504,6 +2515,20 @@ int nb2_constrained_forward_dynamics_backward(const nb2_model* m, int B, const v
   CfdArgs a{};
   a.state = state; a.tau = tau; a.off = offsets; a.off_pw = offsets_per_world; a.wi = world_inertia;
   a.gqdd = grad_accel; a.gw = grad_wrenches; a.gstate = grad_state; a.gtau = grad_tau; a.goff = grad_offsets; a.gI = grad_inertia;
+  return launch_cfd(m, B, k, body, T_owner_from_node, point_contacts, damping, a, precision, stream, who);
+}
+int nb2_constrained_forward_dynamics_jacobians(const nb2_model* m, int B, const void* state, const void* tau, int k, const int32_t* body,
+                                                const double* T_owner_from_node, const void* offsets, int offsets_per_world, int point_contacts,
+                                                double damping, const double* world_inertia, void* accel, void* wrenches, void* J_q, void* J_qdot,
+                                                void* J_tau, void* W_q, void* W_qdot, void* W_tau, int precision, void* stream) {
+  static const char* who = "nb2_constrained_forward_dynamics_jacobians";
+  if (B > 0 && (!accel || !wrenches || !J_q || !J_qdot || !J_tau || !W_q || !W_qdot || !W_tau)) {
+    g_err = std::string(who) + ": bad argument";
+    return NB2_ERR_INVALID;
+  }
+  CfdArgs a{};
+  a.state = state; a.tau = tau; a.off = offsets; a.off_pw = offsets_per_world; a.wi = world_inertia; a.qdd = accel; a.wrench = wrenches;
+  a.J[0] = J_q; a.J[1] = J_qdot; a.J[2] = J_tau; a.J[3] = W_q; a.J[4] = W_qdot; a.J[5] = W_tau;
   return launch_cfd(m, B, k, body, T_owner_from_node, point_contacts, damping, a, precision, stream, who);
 }
 int nb2_model_ndof(const nb2_model* m) { return m ? m->mf.ndof : -1; }

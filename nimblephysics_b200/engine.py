@@ -322,6 +322,16 @@ class DeviceModel:
                                                                           gwrench_ptr, gstate_ptr, gtau_ptr, goff_ptr, ginertia_ptr, precision,
                                                                           stream))
 
+    def constrained_forward_dynamics_jacobians_device(self, B, state_ptr, tau_ptr, bodies, T12, off_ptr, off_per_world, point, damping, qdd_ptr,
+                                                      wrench_ptr, jac_ptrs, stream, precision=FP32, wi_ptr=None):
+        """qdd, wrenches and the dense Jacobians of constrained_forward_dynamics_device (include/nb2.h
+        nb2_constrained_forward_dynamics_jacobians); jac_ptrs: (J_q, J_qdot, J_tau [B, n, n], W_q, W_qdot, W_tau [B, m, n])."""
+        b = np.ascontiguousarray(bodies, np.int32)
+        T = np.ascontiguousarray(T12, np.float64)
+        _cabi.check(_cabi.lib().nb2_constrained_forward_dynamics_jacobians(self.handle, B, state_ptr, tau_ptr, len(b), b.ctypes.data, T.ctypes.data,
+                                                                           off_ptr, int(off_per_world), int(point), float(damping), wi_ptr, qdd_ptr,
+                                                                           wrench_ptr, *jac_ptrs, precision, stream))
+
     def contact_workspace_bytes(self, B):
         return int(_cabi.lib().nb2_contact_workspace_bytes(self.handle, B))
 
