@@ -87,57 +87,38 @@ template <class R> NB2_HD V6<R> sv_ld6(const R* sv, size_t B, int k) {
   return v;
 }
 
-// Per-body constants (Xtree 12 + inertia 10 words).  `bt` is an optional copy of these tables in shared memory
-// ([body][NB2_BT_WORDS]): with several lanes per world the lanes of a warp sit on DIFFERENT bodies, and a constant-bank
-// load with a lane-varying index is replayed once per distinct address, while shared memory serves them in one pass.
-// bt == nullptr reads the kernel-parameter copy (one thread per world: the index is warp-uniform, constant bank is ideal).
-#define NB2_BT_WORDS 22
-template <class R> NB2_HD Xf<R> xtree(const Nb2ModelDev<R>& M, const R* bt, int i) {
+// Per-body constants (Xtree 12 + inertia 10 words), read from the model.  The contact-free kernels keep every warp on one body
+// at a time (nb2_coop.cuh), so the index is warp-uniform and a kernel-parameter model is read as constant-bank broadcasts.
+template <class R> NB2_HD Xf<R> xtree(const Nb2ModelDev<R>& M, int i) {
   Xf<R> T;
-  if (bt) {
-    const R* t = bt + NB2_BT_WORDS * i;
-    T.R_.m00 = t[0]; T.R_.m01 = t[1]; T.R_.m02 = t[2]; T.R_.m10 = t[3]; T.R_.m11 = t[4]; T.R_.m12 = t[5];
-    T.R_.m20 = t[6]; T.R_.m21 = t[7]; T.R_.m22 = t[8];
-    T.p = mk3<R>(t[9], t[10], t[11]);
-    return T;
-  }
   T.R_.m00 = M.Xtree[i][0]; T.R_.m01 = M.Xtree[i][1]; T.R_.m02 = M.Xtree[i][2];
   T.R_.m10 = M.Xtree[i][3]; T.R_.m11 = M.Xtree[i][4]; T.R_.m12 = M.Xtree[i][5];
   T.R_.m20 = M.Xtree[i][6]; T.R_.m21 = M.Xtree[i][7]; T.R_.m22 = M.Xtree[i][8];
   T.p = mk3<R>(M.Xtree[i][9], M.Xtree[i][10], M.Xtree[i][11]);
   return T;
 }
-template <class R> NB2_HD Xf<R> xtree(const Nb2ModelDev<R>& M, int i) { return xtree<R>(M, (const R*)nullptr, i); }
 // parent <- child transform of a revolute-z joint: Xtree * Rz(theta)
-template <class R> NB2_HD Xf<R> xf_rev(const Nb2ModelDev<R>& M, const R* bt, int i, R s, R c) {
-  Xf<R> X = xtree(M, bt, i), T;
+template <class R> NB2_HD Xf<R> xf_rev(const Nb2ModelDev<R>& M, int i, R s, R c) {
+  Xf<R> X = xtree(M, i), T;
   T.R_.m00 = c * X.R_.m00 + s * X.R_.m01; T.R_.m01 = c * X.R_.m01 - s * X.R_.m00; T.R_.m02 = X.R_.m02;
   T.R_.m10 = c * X.R_.m10 + s * X.R_.m11; T.R_.m11 = c * X.R_.m11 - s * X.R_.m10; T.R_.m12 = X.R_.m12;
   T.R_.m20 = c * X.R_.m20 + s * X.R_.m21; T.R_.m21 = c * X.R_.m21 - s * X.R_.m20; T.R_.m22 = X.R_.m22;
   T.p = X.p;
   return T;
 }
-template <class R> NB2_HD Xf<R> xf_rev(const Nb2ModelDev<R>& M, int i, R s, R c) { return xf_rev<R>(M, (const R*)nullptr, i, s, c); }
-template <class R> NB2_HD Xf<R> xf_pris(const Nb2ModelDev<R>& M, const R* bt, int i, R d) {
-  Xf<R> T = xtree(M, bt, i);
+template <class R> NB2_HD Xf<R> xf_pris(const Nb2ModelDev<R>& M, int i, R d) {
+  Xf<R> T = xtree(M, i);
   T.p.x += T.R_.m02 * d; T.p.y += T.R_.m12 * d; T.p.z += T.R_.m22 * d;
   return T;
 }
-template <class R> NB2_HD Xf<R> xf_pris(const Nb2ModelDev<R>& M, int i, R d) { return xf_pris<R>(M, (const R*)nullptr, i, d); }
 // wi: optional PER-WORLD inertia table (fp64, word-major [10*nb][wiB] like grad_inertia, already offset to the world) that replaces
-// the model's: the worlds of a warp are adjacent, so its loads coalesce.  nullptr = the model's table (kernel parameter or `bt`).
-template <class R> NB2_HD void inertia_of(const Nb2ModelDev<R>& M, const R* bt, const double* wi, size_t wiB, int i, R* m, V3<R>* h, S3<R>* Ib) {
+// the model's: the worlds of a warp are adjacent, so its loads coalesce.  nullptr = the model's table.
+template <class R> NB2_HD void inertia_of(const Nb2ModelDev<R>& M, const double* wi, size_t wiB, int i, R* m, V3<R>* h, S3<R>* Ib) {
   if (wi) {
     const double* t = wi + (size_t)(10 * i) * wiB;
     *m = (R)t[0]; *h = mk3<R>((R)t[wiB], (R)t[2 * wiB], (R)t[3 * wiB]);
     Ib->xx = (R)t[4 * wiB]; Ib->yy = (R)t[5 * wiB]; Ib->zz = (R)t[6 * wiB];
     Ib->xy = (R)t[7 * wiB]; Ib->xz = (R)t[8 * wiB]; Ib->yz = (R)t[9 * wiB];
-    return;
-  }
-  if (bt) {
-    const R* t = bt + NB2_BT_WORDS * i + 12;
-    *m = t[0]; *h = mk3<R>(t[1], t[2], t[3]);
-    Ib->xx = t[4]; Ib->yy = t[5]; Ib->zz = t[6]; Ib->xy = t[7]; Ib->xz = t[8]; Ib->yz = t[9];
     return;
   }
   *m = M.inertia[i][0];
@@ -157,10 +138,10 @@ template <class R, int ST> NB2_HD void stXf(R* p, const Xf<R>& T) {
   p[6 * ST] = T.R_.m20; p[7 * ST] = T.R_.m21; p[8 * ST] = T.R_.m22; p[9 * ST] = T.p.x; p[10 * ST] = T.p.y; p[11 * ST] = T.p.z;
 }
 // transform of body i during the sweeps that follow the kinematics pass (forward scratch layout)
-template <class R, int ST> NB2_HD Xf<R> body_xf_fwd(const Nb2ModelDev<R>& M, const R* bt, int i, const R* scr, const FwdLayout& L) {
+template <class R, int ST> NB2_HD Xf<R> body_xf_fwd(const Nb2ModelDev<R>& M, int i, const R* scr, const FwdLayout& L) {
   const int jt = M.jtype[i];
-  if (jt == NB2_JT_REV) { const R* b = scr + (size_t)(L.oBody + NB2_FWD_BODY_WORDS * i + 6) * ST; return xf_rev(M, bt, i, b[0], b[ST]); }
-  if (jt == NB2_JT_PRIS) return xf_pris(M, bt, i, scr[(size_t)(L.oQ + M.dof_off[i]) * ST]);
+  if (jt == NB2_JT_REV) { const R* b = scr + (size_t)(L.oBody + NB2_FWD_BODY_WORDS * i + 6) * ST; return xf_rev(M, i, b[0], b[ST]); }
+  if (jt == NB2_JT_PRIS) return xf_pris(M, i, scr[(size_t)(L.oQ + M.dof_off[i]) * ST]);
   return ldXf<R, ST>(scr + (size_t)(L.oFree + 18 * M.free_idx[i]) * ST);
 }
 // S * x for 1-dof joints / eta = ad(V, S v)
@@ -181,7 +162,7 @@ template <class R, int ST> NB2_HD R tau_of(const Nb2ModelDev<R>& M, const R* scr
 // forward: state=[q;v] (fp32 row), action (fp32 row) -> next state row; optionally streams intermediates to `sv`
 // =====================================================================================================
 template <class R, int ST>
-NB2_HD void fwd_pass1(const Nb2ModelDev<R>& M, R* scr, int lo, int hi, const R* bt = nullptr) {
+NB2_HD void fwd_pass1(const Nb2ModelDev<R>& M, R* scr, int lo, int hi) {
   const int nb = M.nb, n = M.ndof;
   const FwdLayout L = fwd_layout(nb, n, M.nslots, M.nfree);
   const R dt = M.dt;
@@ -195,15 +176,15 @@ NB2_HD void fwd_pass1(const Nb2ModelDev<R>& M, R* scr, int lo, int hi, const R* 
     if (jt == NB2_JT_REV) {
       R s, c; nb2_sincos(scr[(size_t)(L.oQ + o) * ST], &s, &c);
       bs[6 * ST] = s; bs[7 * ST] = c;
-      V = AdInvT(xf_rev(M, bt, i, s, c), Vp);
+      V = AdInvT(xf_rev(M, i, s, c), Vp);
       V.a.z += scr[(size_t)(L.oV + o) * ST];
     } else if (jt == NB2_JT_PRIS) {
-      V = AdInvT(xf_pris(M, bt, i, scr[(size_t)(L.oQ + o) * ST]), Vp);
+      V = AdInvT(xf_pris(M, i, scr[(size_t)(L.oQ + o) * ST]), Vp);
       V.l.z += scr[(size_t)(L.oV + o) * ST];
     } else {  // FREE (FreeJoint.cpp:74-81, 1027-1061)
       const R* q = scr + (size_t)(L.oQ + o) * ST;
       const R* v = scr + (size_t)(L.oV + o) * ST;
-      Xf<R> X = xtree(M, bt, i), T;
+      Xf<R> X = xtree(M, i), T;
       M3<R> Rq = expmap(mk3<R>(q[0], q[ST], q[2 * ST]));
       T.R_ = mul(X.R_, Rq);
       T.p = mul(X.R_, mk3<R>(q[3 * ST], q[4 * ST], q[5 * ST])) + X.p;
@@ -216,7 +197,7 @@ NB2_HD void fwd_pass1(const Nb2ModelDev<R>& M, R* scr, int lo, int hi, const R* 
 }
 
 template <class R, int ST>
-NB2_HD void fwd_pass2(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool save, int lo, int hi, const R* bt = nullptr, R* iinv_out = nullptr,
+NB2_HD void fwd_pass2(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool save, int lo, int hi, R* iinv_out = nullptr,
                       const double* wi = nullptr, size_t wiB = 0) {
   const int nb = M.nb, n = M.ndof;
   const FwdLayout L = fwd_layout(nb, n, M.nslots, M.nfree);
@@ -230,7 +211,7 @@ NB2_HD void fwd_pass2(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool sav
   for (int i = hi - 1; i >= lo; i--) {
     const int jt = M.jtype[i], p = M.parent[i], o = M.dof_off[i], fl = M.flags[i];
     R* bs = scr + (size_t)(L.oBody + NB2_FWD_BODY_WORDS * i) * ST;
-    R m; V3<R> h; S3<R> Ib; inertia_of(M, bt, wi, wiB, i, &m, &h, &Ib);
+    R m; V3<R> h; S3<R> Ib; inertia_of(M, wi, wiB, i, &m, &h, &Ib);
     const V6<R> V = ld6<R, ST>(bs);
     SI<R> IA = rigidSI(m, h, Ib);
     V6<R> pA = crf(V, mulG(m, h, Ib, V));
@@ -304,7 +285,7 @@ NB2_HD void fwd_pass2(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool sav
     }
     hvalid = false;
     if (p >= 0) {
-      const Xf<R> T = body_xf_fwd<R, ST>(M, bt, i, scr, L);
+      const Xf<R> T = body_xf_fwd<R, ST>(M, i, scr, L);
       const SI<R> Ic = xform_inertia(T, Pi);
       const V6<R> pc = dAdInvT(T, beta);
       if (fl & NB2_F_HANDOFF) { hI = Ic; hp = pc; hvalid = true; }
@@ -319,7 +300,7 @@ NB2_HD void fwd_pass2(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool sav
 
 // FD (forward dynamics, DESIGN.md §6k): no integration; qdd replaces the body's force words (oAct, spent after pass 2) for fd_store
 template <class R, int ST, bool FD = false>
-NB2_HD void fwd_pass3(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool save, int lo, int hi, const R* bt = nullptr) {
+NB2_HD void fwd_pass3(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool save, int lo, int hi) {
   const int nb = M.nb, n = M.ndof;
   const FwdLayout L = fwd_layout(nb, n, M.nslots, M.nfree);
   const R dt = M.dt;
@@ -330,7 +311,7 @@ NB2_HD void fwd_pass3(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool sav
   for (int i = lo; i < hi; i++) {
     const int jt = M.jtype[i], p = M.parent[i], o = M.dof_off[i];
     R* bs = scr + (size_t)(L.oBody + NB2_FWD_BODY_WORDS * i) * ST;
-    const Xf<R> T = body_xf_fwd<R, ST>(M, bt, i, scr, L);
+    const Xf<R> T = body_xf_fwd<R, ST>(M, i, scr, L);
     const V6<R> Ap = AdInvT(T, (p >= 0) ? ld6<R, ST>(scr + (size_t)(L.oBody + NB2_FWD_BODY_WORDS * p) * ST) : A0);  // the parent's V slot holds its A by now
     const V6<R> V = ld6<R, ST>(bs);
     V6<R> A;
@@ -388,12 +369,12 @@ NB2_HD void fwd_pass3(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool sav
   }
 }
 
-// ---- group I/O.  A GROUP is the set of worlds one warp works on (32/lanes of them on the device, one in the host
-// emulation and in the single-thread paths); its worlds are consecutive, so their state / action / output rows form
+// ---- group I/O.  A GROUP is the set of worlds a set of threads works on (32 on the device, or 32/lanes for the narrow groups of
+// nb2_coop.cuh; one in the host emulation and in the single-thread paths); its worlds are consecutive, so their state / action / output rows form
 // one contiguous block of global memory that the group's threads copy cooperatively (fully coalesced, every byte
 // touched once — the entry points may hand in mapped host memory).  scr0 = scratch of the group's first world.
 // Copy loops of the group I/O: 16-byte vector accesses when the block is aligned (it is whenever the batch pointers are,
-// since a group starts at a multiple of 4 worlds), several independent loads in flight per thread (the source may be
+// since a group starts at a multiple of 4 worlds: groups are 32 or 32/lanes >= 4 worlds wide), several independent loads in flight per thread (the source may be
 // host memory behind PCIe), index -> (world slot, dof) by multiply-high with the precomputed reciprocal.
 #define NB2_IO_UNROLL 4
 struct alignas(16) F4 { float x, y, z, w; };
@@ -456,8 +437,8 @@ template <class R, int ST> struct WordGather {
   }
 };
 
-// ---- group I/O.  A GROUP is the set of worlds one warp works on (32/lanes of them on the device, a few in the host
-// emulation, one in the single-thread paths); its worlds are consecutive, so their state / action / output rows form
+// ---- group I/O.  A GROUP is the set of worlds a set of threads works on (32 on the device, or 32/lanes for the narrow groups of
+// nb2_coop.cuh; a few in the host emulation, one in the single-thread paths); its worlds are consecutive, so their state / action / output rows form
 // one contiguous block of global memory that the group's threads copy cooperatively (fully coalesced, every byte
 // touched once — the entry points may hand in mapped host memory).  scr0 = scratch of the group's first world.
 // The copies are pure word moves (q, v and the raw action row are adjacent in the scratch); the action map and the
@@ -481,8 +462,8 @@ NB2_HD void fwd_store(const Nb2ModelDev<R>& M, const R* scr0, float* out0, int n
 }
 
 // The sweeps are cut into STAGES so that M.lanes threads can cooperate on one world: lane 0 owns the TRUNK (an
-// ancestor-closed set of bodies), every lane owns some LIMB subtrees (modelspec._partition_tree).  A warp barrier is
-// needed only where data crosses threads (NB2_FWD_SYNC_MASK bit = "barrier after this stage"):
+// ancestor-closed set of bodies), every lane owns some LIMB subtrees (modelspec._partition_tree).  A barrier over the
+// lanes is needed only where data crosses threads (NB2_FWD_SYNC_MASK bit = "barrier after this stage"):
 //   0 group load of q, v, tau (fwd_load)                     | barrier
 //   1 kinematics of the trunk           (lane 0, root->leaf) | barrier
 //   2 kinematics of the limbs           (every lane)
@@ -493,11 +474,13 @@ NB2_HD void fwd_store(const Nb2ModelDev<R>& M, const R* scr0, float* out0, int n
 //   7 group store of q+, v+ (fwd_store)
 // With lanes == 1 everything is trunk.  Each pass body is instantiated once (the stage index is a run-time value).
 // FD: the forward-dynamics variant of pass 3 (fwd_pass3), which the FD kernels use with their own group load / store.
+// The stage functions read the model from M only; their nullptr-typed argument after `stage` keeps the positional argument
+// lists of their callers (the host-emulation harnesses among them) unchanged.
 #define NB2_FWD_STAGES 8
 #define NB2_FWD_SYNC_MASK 0x6Bu       /* after stages 0, 1, 3, 5, 6 */
 #define NB2_FWD_SYNC_MASK_1LANE 0x41u /* lanes == 1: only the group load / store exchange data between threads */
 template <class R, int ST, bool FD = false>
-NB2_HD void world_forward_stage(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool save, int lane, int stage, const R* bt = nullptr, R* iinv_out = nullptr,
+NB2_HD void world_forward_stage(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool save, int lane, int stage, decltype(nullptr) = nullptr, R* iinv_out = nullptr,
                                 const double* wi = nullptr, size_t wiB = 0) {
   const int pass = (stage + 1) >> 1;                          // stages 1..6 -> passes 1, 2, 3
   const bool trunk = (stage == 1) | (stage == 4) | (stage == 5);
@@ -506,9 +489,9 @@ NB2_HD void world_forward_stage(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B
   for (int rr = 0; rr < nr; rr++) {
     const int r = (pass == 2) ? nr - 1 - rr : rr;
     const int lo = trunk ? M.trunk_lo[r] : M.limb_lo[lane][r], hi = trunk ? M.trunk_hi[r] : M.limb_hi[lane][r];
-    if (pass == 1) fwd_pass1<R, ST>(M, scr, lo, hi, bt);
-    else if (pass == 2) fwd_pass2<R, ST>(M, scr, sv, B, save, lo, hi, bt, iinv_out, wi, wiB);
-    else fwd_pass3<R, ST, FD>(M, scr, sv, B, save, lo, hi, bt);
+    if (pass == 1) fwd_pass1<R, ST>(M, scr, lo, hi);
+    else if (pass == 2) fwd_pass2<R, ST>(M, scr, sv, B, save, lo, hi, iinv_out, wi, wiB);
+    else fwd_pass3<R, ST, FD>(M, scr, sv, B, save, lo, hi);
   }
 }
 
@@ -560,7 +543,7 @@ template <class R> NB2_HD void inertia_param_form(const V6<R>& Y, const V6<R>& X
 // backward: g_next = dL/d[q+;v+]  ->  g_state = dL/d[q;v], g_action = dL/d action
 // =====================================================================================================
 template <class R, int ST, bool CONTACT>
-NB2_HD void bwd_B1(const Nb2ModelDev<R>& M, R* scr, const float* st, const R* sv, size_t B, int lo, int hi, const R* bt = nullptr) {
+NB2_HD void bwd_B1(const Nb2ModelDev<R>& M, R* scr, const float* st, const R* sv, size_t B, int lo, int hi) {
   const int nb = M.nb, n = M.ndof;
   constexpr int SLOTW = CONTACT ? 42 : 18;
   const BwdLayout L = bwd_layout(nb, n, M.nslots, M.nfree, SLOTW);
@@ -590,8 +573,8 @@ NB2_HD void bwd_B1(const Nb2ModelDev<R>& M, R* scr, const float* st, const R* sv
     hvalid = false;
     if (p >= 0) {
       Xf<R> T;
-      if (jt == NB2_JT_REV) T = xf_rev(M, bt, i, (R)s[19 * B], (R)s[20 * B]);
-      else if (jt == NB2_JT_PRIS) T = xf_pris(M, bt, i, scr[(size_t)(L.oSt + o) * ST]);
+      if (jt == NB2_JT_REV) T = xf_rev(M, i, (R)s[19 * B], (R)s[20 * B]);
+      else if (jt == NB2_JT_PRIS) T = xf_pris(M, i, scr[(size_t)(L.oSt + o) * ST]);
       else { R t12[12]; for (int k = 0; k < 12; k++) t12[k] = (R)sv[(size_t)(kFree + M.free_idx[i] * 33 + 21 + k) * B]; T = ldXf<R, 1>(t12); }
       const V6<R> pc = dAdInvT(T, beta);
       if (fl & NB2_F_HANDOFF) { hp = pc; hvalid = true; }
@@ -604,7 +587,7 @@ NB2_HD void bwd_B1(const Nb2ModelDev<R>& M, R* scr, const float* st, const R* sv
 }
 
 template <class R, int ST, bool CONTACT>
-NB2_HD void bwd_B2(const Nb2ModelDev<R>& M, R* scr, const float* st, const R* sv, size_t B, int lo, int hi, const R* bt = nullptr) {
+NB2_HD void bwd_B2(const Nb2ModelDev<R>& M, R* scr, const float* st, const R* sv, size_t B, int lo, int hi) {
   const int nb = M.nb, n = M.ndof;
   constexpr int SLOTW = CONTACT ? 42 : 18;
   const BwdLayout L = bwd_layout(nb, n, M.nslots, M.nfree, SLOTW);
@@ -619,7 +602,7 @@ NB2_HD void bwd_B2(const Nb2ModelDev<R>& M, R* scr, const float* st, const R* sv
     R* bs = scr + (size_t)(L.oBody + 7 * i) * ST;
     V6<R> W;
     if (jt != NB2_JT_FREE) {
-      Xf<R> T = (jt == NB2_JT_REV) ? xf_rev(M, bt, i, (R)s[19 * B], (R)s[20 * B]) : xf_pris(M, bt, i, scr[(size_t)(L.oSt + o) * ST]);
+      Xf<R> T = (jt == NB2_JT_REV) ? xf_rev(M, i, (R)s[19 * B], (R)s[20 * B]) : xf_pris(M, i, scr[(size_t)(L.oSt + o) * ST]);
       W = (p >= 0) ? AdInvT(T, ld6<R, ST>(scr + (size_t)(L.oBody + 7 * p + 1) * ST)) : zero6<R>();
       const R lam = (R)s[18 * B] * (bs[0] - dot(sv_ld6<R>(s, B, 12), W));
       scr[(size_t)(L.oLam + o) * ST] = lam;
@@ -640,7 +623,7 @@ NB2_HD void bwd_B2(const Nb2ModelDev<R>& M, R* scr, const float* st, const R* sv
 
 template <class R, int ST, bool CONTACT>
 NB2_HD void bwd_B3(const Nb2ModelDev<R>& M, R* scr, const float* st, const R* sv, size_t B, const BwdContactData<ST>& cd, int lo, int hi,
-                   float* gI = nullptr, const R* bt = nullptr, size_t gIB = 0, const double* wi = nullptr, size_t wiB = 0, double* gIa = nullptr) {
+                   float* gI = nullptr, size_t gIB = 0, const double* wi = nullptr, size_t wiB = 0, double* gIa = nullptr) {
   const int nb = M.nb, n = M.ndof;
   constexpr int SLOTW = CONTACT ? 42 : 18;
   const BwdLayout L = bwd_layout(nb, n, M.nslots, M.nfree, SLOTW);
@@ -660,7 +643,7 @@ NB2_HD void bwd_B3(const Nb2ModelDev<R>& M, R* scr, const float* st, const R* sv
   for (int i = hi - 1; i >= lo; i--) {
     const int jt = M.jtype[i], p = M.parent[i], o = M.dof_off[i], fl = M.flags[i];
     const R* s = sv + (size_t)(i * 21) * B;
-    R m; V3<R> h; S3<R> Ib; inertia_of(M, bt, wi, wiB, i, &m, &h, &Ib);
+    R m; V3<R> h; S3<R> Ib; inertia_of(M, wi, wiB, i, &m, &h, &Ib);
     const V6<R> V = sv_ld6<R>(s, B, 0);
     V6<R> A = sv_ld6<R>(s, B, 6);
     if (CONTACT && cd.active && !cd.pass2) { const auto a6 = cd.Aacc + 6 * i; A.a = mk3<R>((R)a6[0], (R)a6[1], (R)a6[2]); A.l = mk3<R>((R)a6[3], (R)a6[4], (R)a6[5]); }
@@ -716,7 +699,7 @@ NB2_HD void bwd_B3(const Nb2ModelDev<R>& M, R* scr, const float* st, const R* sv
       Sv = S_times<R>(jt, scr[(size_t)(L.oSt + n + o) * ST]);
       Sa = S_times<R>(jt, (CONTACT && cd.active && !cd.pass2) ? (R)cd.aeff[o] : (R)sv[(size_t)(kQdd + o) * B]);
       Sl = S_times<R>(jt, scr[(size_t)(L.oLam + o) * ST]);
-      T = (jt == NB2_JT_REV) ? xf_rev(M, bt, i, (R)s[19 * B], (R)s[20 * B]) : xf_pris(M, bt, i, scr[(size_t)(L.oSt + o) * ST]);
+      T = (jt == NB2_JT_REV) ? xf_rev(M, i, (R)s[19 * B], (R)s[20 * B]) : xf_pris(M, i, scr[(size_t)(L.oSt + o) * ST]);
     } else {
       Sv.a = mk3<R>(scr[(size_t)(L.oSt + n + o) * ST], scr[(size_t)(L.oSt + n + o + 1) * ST], scr[(size_t)(L.oSt + n + o + 2) * ST]); Sv.l = mk3<R>(scr[(size_t)(L.oSt + n + o + 3) * ST], scr[(size_t)(L.oSt + n + o + 4) * ST], scr[(size_t)(L.oSt + n + o + 5) * ST]);
       Sa = sv_ld6<R>(sv + (size_t)(kQdd + o) * B, B, 0);
@@ -901,7 +884,7 @@ NB2_HD constexpr CBwdIter cbwd_iter(int it) {
   return {(it < 4) ? it + 1 : (it == 4 || it == 6) ? 5 : (it == 5 || it == 7) ? 7 : (it == 8) ? 6 : 8, static_cast<bool>((it == 6) | (it == 7))};
 }
 template <class R, int ST, bool CONTACT = false>
-NB2_HD void world_backward_stage(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, int lane, int stage, float* gI = nullptr, const R* bt = nullptr,
+NB2_HD void world_backward_stage(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, int lane, int stage, float* gI = nullptr, decltype(nullptr) = nullptr,
                                  size_t gIB = 0, const BwdContactData<ST>* cdp = nullptr, const double* wi = nullptr, size_t wiB = 0,
                                  double* gIa = nullptr) {
   const float* st = nullptr;  // the passes read the state from the scratch (oSt)
@@ -915,9 +898,9 @@ NB2_HD void world_backward_stage(const Nb2ModelDev<R>& M, R* scr, const R* sv, s
   for (int rr = 0; rr < nr; rr++) {
     const int r = (pass == 1 || pass == 3) ? nr - 1 - rr : rr;
     const int lo = trunk ? M.trunk_lo[r] : M.limb_lo[lane][r], hi = trunk ? M.trunk_hi[r] : M.limb_hi[lane][r];
-    if (pass == 1) bwd_B1<R, ST, CONTACT>(M, scr, st, sv, B, lo, hi, bt);
-    else if (pass == 2) bwd_B2<R, ST, CONTACT>(M, scr, st, sv, B, lo, hi, bt);
-    else if (pass == 3) bwd_B3<R, ST, CONTACT>(M, scr, st, sv, B, cd, lo, hi, gI, bt, gIB ? gIB : B, wi, wiB, gIa);
+    if (pass == 1) bwd_B1<R, ST, CONTACT>(M, scr, st, sv, B, lo, hi);
+    else if (pass == 2) bwd_B2<R, ST, CONTACT>(M, scr, st, sv, B, lo, hi);
+    else if (pass == 3) bwd_B3<R, ST, CONTACT>(M, scr, st, sv, B, cd, lo, hi, gI, gIB ? gIB : B, wi, wiB, gIa);
     else bwd_assemble<R, ST, CONTACT>(M, scr, st, cd, lo, hi);
   }
 }
@@ -950,7 +933,7 @@ NB2_HD void id_rows_store(const R* scr0, R* dst, int width, unsigned magic, int 
 
 // root -> leaf: A_i = X^-1 A_p + S a + ad(V_i, S qdot), base acceleration -g (as fwd_pass3)
 template <class R, int ST>
-NB2_HD void id_pass_acc(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool save, int lo, int hi, const R* bt) {
+NB2_HD void id_pass_acc(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool save, int lo, int hi) {
   const FwdLayout L = fwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
   const R rdt = R(1) / M.dt;
   const int kFree = M.nb * 21, kQdd = M.nb * 21 + M.nfree * 33;
@@ -958,7 +941,7 @@ NB2_HD void id_pass_acc(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool s
   for (int i = lo; i < hi; i++) {
     const int jt = M.jtype[i], p = M.parent[i], o = M.dof_off[i];
     R* bs = scr + (size_t)(L.oBody + NB2_FWD_BODY_WORDS * i) * ST;
-    const Xf<R> T = body_xf_fwd<R, ST>(M, bt, i, scr, L);
+    const Xf<R> T = body_xf_fwd<R, ST>(M, i, scr, L);
     const V6<R> Ap = AdInvT(T, (p >= 0) ? ld6<R, ST>(scr + (size_t)(L.oBody + NB2_FWD_BODY_WORDS * p + 8) * ST) : A0);
     const V6<R> V = ld6<R, ST>(bs);
     V6<R> A = Ap;
@@ -990,7 +973,7 @@ NB2_HD void id_pass_acc(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool s
 
 // leaf -> root: f_i = G A_i + V_i x* G V_i + sum_c X*_c f_c ; tau = S^T f_i + K (q - q0 + qdot dt) + D qdot (into the action words)
 template <class R, int ST>
-NB2_HD void id_pass_force(const Nb2ModelDev<R>& M, R* scr, int lo, int hi, const R* bt, const double* wi, size_t wiB) {
+NB2_HD void id_pass_force(const Nb2ModelDev<R>& M, R* scr, int lo, int hi, const double* wi, size_t wiB) {
   const FwdLayout L = fwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
   const R dt = M.dt;
   V6<R> hf = zero6<R>();
@@ -998,7 +981,7 @@ NB2_HD void id_pass_force(const Nb2ModelDev<R>& M, R* scr, int lo, int hi, const
   for (int i = hi - 1; i >= lo; i--) {
     const int jt = M.jtype[i], p = M.parent[i], o = M.dof_off[i], fl = M.flags[i];
     const R* bs = scr + (size_t)(L.oBody + NB2_FWD_BODY_WORDS * i) * ST;
-    R m; V3<R> h; S3<R> Ib; inertia_of(M, bt, wi, wiB, i, &m, &h, &Ib);
+    R m; V3<R> h; S3<R> Ib; inertia_of(M, wi, wiB, i, &m, &h, &Ib);
     const V6<R> V = ld6<R, ST>(bs), A = ld6<R, ST>(bs + 8 * ST);
     V6<R> f = mulG(m, h, Ib, A) + crf(V, mulG(m, h, Ib, V));
     if (hvalid) f = f + hf;
@@ -1013,7 +996,7 @@ NB2_HD void id_pass_force(const Nb2ModelDev<R>& M, R* scr, int lo, int hi, const
     }
     hvalid = false;
     if (p >= 0) {
-      const V6<R> fc = dAdInvT(body_xf_fwd<R, ST>(M, bt, i, scr, L), f);
+      const V6<R> fc = dAdInvT(body_xf_fwd<R, ST>(M, i, scr, L), f);
       if (fl & NB2_F_HANDOFF) { hf = fc; hvalid = true; }
       else st6<R, ST>(scr + (size_t)(L.oSlot + 27 * M.slot_parent[i]) * ST, fc);
     }
@@ -1028,7 +1011,7 @@ NB2_HD void id_pass_force(const Nb2ModelDev<R>& M, R* scr, int lo, int hi, const
 #define NB2_ID_FWD_SYNC_MASK 0x1Bu        /* after stages 0, 1, 3, 4 */
 #define NB2_ID_FWD_SYNC_MASK_1LANE 0x11u  /* lanes == 1: after the group load and before the group store */
 template <class R, int ST>
-NB2_HD void id_forward_stage(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool save, int lane, int stage, const R* bt,
+NB2_HD void id_forward_stage(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, bool save, int lane, int stage, decltype(nullptr),
                              const double* wi, size_t wiB) {
   const bool trunk = (stage == 1) | (stage == 4);
   if (trunk && lane != 0) return;
@@ -1036,8 +1019,8 @@ NB2_HD void id_forward_stage(const Nb2ModelDev<R>& M, R* scr, R* sv, size_t B, b
   for (int rr = 0; rr < nr; rr++) {
     const int r = (stage >= 3) ? nr - 1 - rr : rr;
     const int lo = trunk ? M.trunk_lo[r] : M.limb_lo[lane][r], hi = trunk ? M.trunk_hi[r] : M.limb_hi[lane][r];
-    if (stage <= 2) { fwd_pass1<R, ST>(M, scr, lo, hi, bt); id_pass_acc<R, ST>(M, scr, sv, B, save, lo, hi, bt); }
-    else id_pass_force<R, ST>(M, scr, lo, hi, bt, wi, wiB);
+    if (stage <= 2) { fwd_pass1<R, ST>(M, scr, lo, hi); id_pass_acc<R, ST>(M, scr, sv, B, save, lo, hi); }
+    else id_pass_force<R, ST>(M, scr, lo, hi, wi, wiB);
   }
 }
 template <class R, int ST>
@@ -1058,22 +1041,22 @@ NB2_HD void id_store(const Nb2ModelDev<R>& M, const R* scr0, R* tau0, int nworld
 NB2_HD int id_bwd_words(int nb, int n, int nslots, int nfree) { return bwd_layout(nb, n, nslots, nfree).total + 6 * nslots; }
 // parent <- child transform of body i from the saved stream (as bwd_B3 forms it)
 template <class R, int ST>
-NB2_HD Xf<R> id_saved_xf(const Nb2ModelDev<R>& M, const R* bt, int i, const R* scr, const BwdLayout& L, const R* sv, size_t B) {
+NB2_HD Xf<R> id_saved_xf(const Nb2ModelDev<R>& M, int i, const R* scr, const BwdLayout& L, const R* sv, size_t B) {
   const int jt = M.jtype[i];
   const R* s = sv + (size_t)(i * 21) * B;
-  if (jt == NB2_JT_REV) return xf_rev(M, bt, i, s[19 * B], s[20 * B]);
-  if (jt == NB2_JT_PRIS) return xf_pris(M, bt, i, scr[(size_t)(L.oSt + M.dof_off[i]) * ST]);
+  if (jt == NB2_JT_REV) return xf_rev(M, i, s[19 * B], s[20 * B]);
+  if (jt == NB2_JT_PRIS) return xf_pris(M, i, scr[(size_t)(L.oSt + M.dof_off[i]) * ST]);
   R t12[12];
   for (int k = 0; k < 12; k++) t12[k] = sv[(size_t)(M.nb * 21 + M.free_idx[i] * 33 + 21 + k) * B];
   return ldXf<R, 1>(t12);
 }
 // root -> leaf: the field W_i = X^-1 W_p + S lambda_i that seeds bwd_B3 (it replaces B1 / B2 of the step)
 template <class R, int ST>
-NB2_HD void id_bwd_field(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, int lo, int hi, const R* bt) {
+NB2_HD void id_bwd_field(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, int lo, int hi) {
   const BwdLayout L = bwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
   for (int i = lo; i < hi; i++) {
     const int jt = M.jtype[i], p = M.parent[i], o = M.dof_off[i];
-    V6<R> W = (p >= 0) ? AdInvT(id_saved_xf<R, ST>(M, bt, i, scr, L, sv, B), ld6<R, ST>(scr + (size_t)(L.oBody + 7 * p + 1) * ST)) : zero6<R>();
+    V6<R> W = (p >= 0) ? AdInvT(id_saved_xf<R, ST>(M, i, scr, L, sv, B), ld6<R, ST>(scr + (size_t)(L.oBody + 7 * p + 1) * ST)) : zero6<R>();
     if (jt != NB2_JT_FREE) W = W + S_times<R>(jt, scr[(size_t)(L.oLam + o) * ST]);
     else W = W + ld6<R, ST>(scr + (size_t)(L.oLam + o) * ST);
     st6<R, ST>(scr + (size_t)(L.oBody + 7 * i + 1) * ST, W);
@@ -1082,7 +1065,7 @@ NB2_HD void id_bwd_field(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B,
 // leaf -> root, after bwd_B3 of the same bodies: M lambda = S^T sum_subtree X* G W, the assembly above, and (gI != nullptr)
 // dL/d(m, h, Ibar) of body i = d(W^T (G A + V x* G V))/d(theta) = t(W, A) - t(ad(V, W), V) in the arithmetic type (gI: fp64 [10*nb][gIB])
 template <class R, int ST>
-NB2_HD void id_bwd_mass(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, int lo, int hi, const R* bt, const double* wi, size_t wiB,
+NB2_HD void id_bwd_mass(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, int lo, int hi, const double* wi, size_t wiB,
                         double* gI, size_t gIB) {
   const BwdLayout L = bwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
   const int oS = L.total;
@@ -1091,7 +1074,7 @@ NB2_HD void id_bwd_mass(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, 
   bool hvalid = false;
   for (int i = hi - 1; i >= lo; i--) {
     const int jt = M.jtype[i], p = M.parent[i], o = M.dof_off[i], fl = M.flags[i];
-    R m; V3<R> h; S3<R> Ib; inertia_of(M, bt, wi, wiB, i, &m, &h, &Ib);
+    R m; V3<R> h; S3<R> Ib; inertia_of(M, wi, wiB, i, &m, &h, &Ib);
     const V6<R> W = ld6<R, ST>(scr + (size_t)(L.oBody + 7 * i + 1) * ST);
     V6<R> Ab = mulG(m, h, Ib, W);
     if (hvalid) Ab = Ab + hA;
@@ -1118,7 +1101,7 @@ NB2_HD void id_bwd_mass(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, 
     }
     hvalid = false;
     if (p >= 0) {
-      const V6<R> cA = dAdInvT(id_saved_xf<R, ST>(M, bt, i, scr, L, sv, B), Ab);
+      const V6<R> cA = dAdInvT(id_saved_xf<R, ST>(M, i, scr, L, sv, B), Ab);
       if (fl & NB2_F_HANDOFF) { hA = cA; hvalid = true; }
       else st6<R, ST>(scr + (size_t)(oS + 6 * M.slot_parent[i]) * ST, cA);
     }
@@ -1132,7 +1115,7 @@ NB2_HD void id_bwd_mass(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, 
 #define NB2_ID_BWD_SYNC_MASK 0x53u        /* after stages 0, 1, 4, 6 */
 #define NB2_ID_BWD_SYNC_MASK_1LANE 0x41u  /* lanes == 1: after the group load and before the group store */
 template <class R, int ST>
-NB2_HD void id_backward_stage(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, int lane, int stage, const R* bt,
+NB2_HD void id_backward_stage(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, int lane, int stage, decltype(nullptr),
                               const double* wi, size_t wiB, double* gI, size_t gIB) {
   const bool trunk = (stage == 1) | (stage == 5) | (stage == 6);
   if (trunk && lane != 0) return;
@@ -1141,9 +1124,9 @@ NB2_HD void id_backward_stage(const Nb2ModelDev<R>& M, R* scr, const R* sv, size
   for (int rr = 0; rr < nr; rr++) {
     const int r = (stage >= 3) ? nr - 1 - rr : rr;
     const int lo = trunk ? M.trunk_lo[r] : M.limb_lo[lane][r], hi = trunk ? M.trunk_hi[r] : M.limb_hi[lane][r];
-    if (stage <= 2) id_bwd_field<R, ST>(M, scr, sv, B, lo, hi, bt);
-    else if (stage == 3 || stage == 5) bwd_B3<R, ST, false>(M, scr, nullptr, sv, B, cd, lo, hi, nullptr, bt, B, wi, wiB, nullptr);
-    else id_bwd_mass<R, ST>(M, scr, sv, B, lo, hi, bt, wi, wiB, gI, gIB);
+    if (stage <= 2) id_bwd_field<R, ST>(M, scr, sv, B, lo, hi);
+    else if (stage == 3 || stage == 5) bwd_B3<R, ST, false>(M, scr, nullptr, sv, B, cd, lo, hi, nullptr, B, wi, wiB, nullptr);
+    else id_bwd_mass<R, ST>(M, scr, sv, B, lo, hi, wi, wiB, gI, gIB);
   }
 }
 template <class R, int ST>
@@ -1227,7 +1210,7 @@ NB2_HD void fd_bwd_assemble(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t
 // Stages and barriers of the step's backward (NB2_BWD_STAGES, NB2_BWD_SYNC_MASK): 0 group load | B1, B2, B3 as world_backward_stage |
 // fd_bwd_assemble in place of bwd_assemble | 9 group store
 template <class R, int ST>
-NB2_HD void fd_backward_stage(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, int lane, int stage, const R* bt, const double* wi, size_t wiB,
+NB2_HD void fd_backward_stage(const Nb2ModelDev<R>& M, R* scr, const R* sv, size_t B, int lane, int stage, decltype(nullptr), const double* wi, size_t wiB,
                               double* gI, size_t gIB) {
   const int pass = (stage == 1 || stage == 2) ? 1 : (stage == 3 || stage == 4) ? 2 : (stage == 5 || stage == 7) ? 3 : 4;
   const bool trunk = (stage == 2) | (stage == 3) | (stage == 7) | (stage == 8);
@@ -1237,9 +1220,9 @@ NB2_HD void fd_backward_stage(const Nb2ModelDev<R>& M, R* scr, const R* sv, size
   for (int rr = 0; rr < nr; rr++) {
     const int r = (pass == 1 || pass == 3) ? nr - 1 - rr : rr;
     const int lo = trunk ? M.trunk_lo[r] : M.limb_lo[lane][r], hi = trunk ? M.trunk_hi[r] : M.limb_hi[lane][r];
-    if (pass == 1) bwd_B1<R, ST, false>(M, scr, nullptr, sv, B, lo, hi, bt);
-    else if (pass == 2) bwd_B2<R, ST, false>(M, scr, nullptr, sv, B, lo, hi, bt);
-    else if (pass == 3) bwd_B3<R, ST, false>(M, scr, nullptr, sv, B, cd, lo, hi, nullptr, bt, B, wi, wiB, nullptr);
+    if (pass == 1) bwd_B1<R, ST, false>(M, scr, nullptr, sv, B, lo, hi);
+    else if (pass == 2) bwd_B2<R, ST, false>(M, scr, nullptr, sv, B, lo, hi);
+    else if (pass == 3) bwd_B3<R, ST, false>(M, scr, nullptr, sv, B, cd, lo, hi, nullptr, B, wi, wiB, nullptr);
     else fd_bwd_assemble<R, ST>(M, scr, sv, B, lo, hi, gI, gIB);
   }
 }

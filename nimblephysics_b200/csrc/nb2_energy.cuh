@@ -42,7 +42,7 @@ template <class R> NB2_HD void em_bodies(const Nb2ModelDev<R>& M, int root, cons
   for (int i = lane; i < M.nb; i += nl) {
     if (jac_root(M, i) != root) continue;
     const Xf<R> W = ldXf<R, 1>(ws + L.oW + 12 * i);
-    R m; V3<R> h; S3<R> Ib; inertia_of(M, (const R*)nullptr, wi, wiB, i, &m, &h, &Ib);
+    R m; V3<R> h; S3<R> Ib; inertia_of(M, wi, wiB, i, &m, &h, &Ib);
     const V6<R> Vb = AdInvT(W, ldv6(ws + L.oV + 6 * i)), Pb = mulG(m, h, Ib, Vb);
     put6(ws + L.oP + 6 * i, dAdInvT(W, Pb));
     ws[L.oX + i] = R(0.5) * dot(Vb, Pb);
@@ -106,7 +106,7 @@ NB2_HD void emb_bodies(const Nb2ModelDev<R>& M, const R* q, int root, const doub
       continue;
     }
     const Xf<R> W = ldXf<R, 1>(ws + L.oW + 12 * i);
-    R m; V3<R> h; S3<R> Ib; inertia_of(M, (const R*)nullptr, wi, wiB, i, &m, &h, &Ib);
+    R m; V3<R> h; S3<R> Ib; inertia_of(M, wi, wiB, i, &m, &h, &Ib);
     const V6<R> V = ldv6(ws + L.oV + 6 * i), Vb = AdInvT(W, V), Pbb = AdInvT(W, e.Pb);
     const V6<R> Y = dAdInvT(W, mulG(m, h, Ib, Vb * gT + Pbb)), P = dAdInvT(W, mulG(m, h, Ib, Vb));
     const V3<R> x = W.p * m + mul(W.R_, h);

@@ -14,10 +14,11 @@ struct FdArgs {
   const void* state; const void* gqdd; void* gstate; void* gtau; double* gI;
   const double* wi;
 };
-// the kernel of lane count K (1, 2, 4 or 8), forward (bwd = 0) or backward: for cudaFuncSetAttribute and the occupancy query
-template <class R> const void* nb2_fd_kernel(int K, int bwd);
+// the kernel of lane count K (1, 2, 4 or 8) and group width W (32, or NARROW_W<K> = 32/K with K > 1; nb2_coop.cuh), forward (bwd = 0) or
+// backward: for cudaFuncSetAttribute and the occupancy query
+template <class R> const void* nb2_fd_kernel(int K, int W, int bwd);
 template <class R>
-void nb2_fd_launch(int K, int bwd, unsigned blocks, unsigned threads, size_t smem, cudaStream_t st, const Nb2ModelDev<R>& M, int B, const FdArgs& a,
+void nb2_fd_launch(int K, int W, int bwd, unsigned blocks, unsigned threads, size_t smem, cudaStream_t st, const Nb2ModelDev<R>& M, int B, const FdArgs& a,
                    int words);
 // fp64 forward, one thread per world with its scratch in global memory (allocated stream-ordered for the call): the path of
 // nb2_forward_dynamics for a model that no schedule's shared-memory working set fits

@@ -199,7 +199,7 @@ template <class R> NB2_HD void jc_moments(const Nb2ModelDev<R>& M, int root, con
     const int p = M.parent[i];
     const Xf<R> W = p >= 0 ? jac_mul(ldXf<R, 1>(ws + L.oW + 12 * p), ldXf<R, 1>(ws + L.oW + 12 * i)) : ldXf<R, 1>(ws + L.oW + 12 * i);
     stXf<R, 1>(ws + L.oW + 12 * i, W);
-    R m; V3<R> h; S3<R> Ib; inertia_of(M, (const R*)nullptr, wi, wiB, i, &m, &h, &Ib);
+    R m; V3<R> h; S3<R> Ib; inertia_of(M, wi, wiB, i, &m, &h, &Ib);
     const V3<R> x = W.p * m + mul(W.R_, h);
     R* hm = ws + L.oHM + 4 * i;
     hm[0] = x.x; hm[1] = x.y; hm[2] = x.z; hm[3] = m;
@@ -517,7 +517,7 @@ template <class R> NB2_HD void jcd_vel(const Nb2ModelDev<R>& M, const R* qd, int
     V6<R> V = p >= 0 ? ldv6(ws + L.oV + 6 * p) : zero6<R>();
     for (int k = 0; k < mm_nd(jt); k++) V = V + AdT(W, mm_S<R>(jt, k)) * qd[o + k];
     put6(ws + L.oV + 6 * i, V);
-    R m; V3<R> h; S3<R> Ib; inertia_of(M, (const R*)nullptr, wi, wiB, i, &m, &h, &Ib);
+    R m; V3<R> h; S3<R> Ib; inertia_of(M, wi, wiB, i, &m, &h, &Ib);
     const V3<R> xd = V.l * m + cross(V.a, W.p * m + mul(W.R_, h));
     R* hd = ws + L.oHd + 4 * i;
     hd[0] = xd.x; hd[1] = xd.y; hd[2] = xd.z; hd[3] = R(0);
@@ -602,7 +602,7 @@ template <class R> NB2_HD void jcdb_bodies(const Nb2ModelDev<R>& M, int root, co
       continue;
     }
     const Xf<R> W = ldXf<R, 1>(ws + L.oW + 12 * i);
-    R m; V3<R> h; S3<R> Ib; inertia_of(M, (const R*)nullptr, wi, wiB, i, &m, &h, &Ib);
+    R m; V3<R> h; S3<R> Ib; inertia_of(M, wi, wiB, i, &m, &h, &Ib);
     const V3<R> x = W.p * m + mul(W.R_, h);
     const R* a = ws + L.oA + 8 * i;
     const V3<R> Y = mk3<R>(a[3], a[4], a[5]);

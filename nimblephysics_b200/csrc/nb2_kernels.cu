@@ -1,10 +1,11 @@
 // libnb2.so — kernels + C ABI (include/nb2.h).  sm_90a only.
 //
-// Kernel shape (contact-free step): ONE THREAD PER WORLD, 32 worlds per warp.  The model is a __grid_constant__
-// kernel parameter (constant-bank, warp-uniform loads); per-world working storage lives in dynamic shared memory,
-// interleaved [word][lane] so every access is bank-conflict free; the only HBM traffic is the fp32 state/action
-// rows, the outputs and the saved-for-backward stream ([word][B]: coalesced).  All branches depend on the model
-// only, so warps never diverge.  See DESIGN.md for the roofline discussion (the path is FP32-latency bound).
+// Kernel shape (contact-free step): groups of 32 worlds, one thread per world in each of the group's K warps, warp r
+// sweeping lane r of the schedule (nb2_coop.cuh).  The model is a __grid_constant__ kernel parameter (constant-bank,
+// warp-uniform loads); per-world working storage lives in dynamic shared memory, interleaved [word][slot] so every
+// access is bank-conflict free; the only HBM traffic is the fp32 state/action rows, the outputs and the saved-for-
+// backward stream ([word][B]: coalesced).  All branches depend on the model and the lane only, so warps never diverge.
+// See DESIGN.md for the roofline discussion (the path is FP32-latency bound).
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -43,9 +44,9 @@ static std::atomic<long long> g_launches{0};
 
 namespace {
 
-// ---- bulk (TMA) staging of a group's input rows.  The rows of the worlds of one warp are contiguous in global memory, so
+// ---- bulk (TMA) staging of a group's input rows.  The rows of the worlds of one group are contiguous in global memory, so
 // ONE thread hands each block of rows to the copy engine of the SM (cp.async.bulk, completion counted on an mbarrier) instead
-// of 32 threads looping over vector loads: the requests are as wide as they can be — which is what matters when `src` is
+// of the group's threads looping over vector loads: the requests are as wide as they can be — which is what matters when `src` is
 // mapped host memory behind PCIe — and cost two instructions.  The scatter into the [word][slot] scratch then reads shared
 // memory.  Needs 16-byte aligned sources and sizes; otherwise the vector-load path is used.
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
@@ -70,9 +71,9 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned pari
   __trap();
 }
 __device__ __forceinline__ bool bulk_ok(const void* p, size_t bytes) { return ((reinterpret_cast<size_t>(p) | bytes) & 15) == 0 && bytes > 0; }
-// bytes of staging per warp: rows of `nrows` floats per world, rounded to 16 + the mbarrier
-template <int K> __host__ __device__ constexpr size_t staging_bytes(int floats_per_world) {
-  return (((size_t)floats_per_world * CoopShape<K>::WPW * sizeof(float) + 15) & ~(size_t)15) + 16;
+// bytes of staging per group: rows of `floats_per_world` floats for its W worlds, rounded to 16 + the mbarrier
+template <int W> __host__ __device__ constexpr size_t staging_bytes(int floats_per_world) {
+  return (((size_t)floats_per_world * W * sizeof(float) + 15) & ~(size_t)15) + 16;
 }
 
 // ---- programmatic dependent launch (launch_dependent below): a step kernel's launch is processed, and its blocks are placed, while the
@@ -82,18 +83,18 @@ template <int K> __host__ __device__ constexpr size_t staging_bytes(int floats_p
 __device__ __forceinline__ void grid_dependency_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // ---- optional stage clocks of the contact-free step kernels (-DNB2_STEP_CLOCKS; dev builds only, scripts/dev/stage_clocks.py):
-// thread 0 of every NB2_CLK_EVERY-th warp of the grid (up to NB2_CLK_WARPS of them) records clock64() at kernel entry, after the
-// wait for the previous kernel, after the body-table and input staging, and after every stage including its barrier.  Default
-// builds compile none of it.
+// thread 0 of every NB2_CLK_EVERY-th group of the grid (up to NB2_CLK_GROUPS of them) — lane 0 of the schedule, the one that sweeps
+// the trunk — records clock64() at kernel entry, after the wait for the previous kernel, after the input staging, and after every
+// stage including its barrier.  Default builds compile none of it.
 #ifdef NB2_STEP_CLOCKS
-#define NB2_CLK_WARPS 8
-#define NB2_CLK_EVERY 64
+#define NB2_CLK_GROUPS 8
+#define NB2_CLK_EVERY 16
 #define NB2_CLK_SLOTS 16
-__device__ long long nb2_step_clk[2][NB2_CLK_WARPS][NB2_CLK_SLOTS];  // [forward, backward][sampled warp][entry, waited, staged, stage 0, 1, ...]
+__device__ long long nb2_step_clk[2][NB2_CLK_GROUPS][NB2_CLK_SLOTS];  // [forward, backward][sampled group][entry, waited, staged, stage 0, 1, ...]
 #define NB2_CLK(dir, k)                                                                                                   \
   do {                                                                                                                    \
-    const int w_ = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);                                                   \
-    if ((threadIdx.x & 31) == 0 && w_ % NB2_CLK_EVERY == 0 && w_ / NB2_CLK_EVERY < NB2_CLK_WARPS) nb2_step_clk[dir][w_ / NB2_CLK_EVERY][k] = clock64(); \
+    const int g_ = gp.gi;                                                                                                 \
+    if (gp.tid == 0 && g_ % NB2_CLK_EVERY == 0 && g_ / NB2_CLK_EVERY < NB2_CLK_GROUPS) nb2_step_clk[dir][g_ / NB2_CLK_EVERY][k] = clock64(); \
   } while (0)
 #else
 #define NB2_CLK(dir, k)
@@ -101,40 +102,36 @@ __device__ long long nb2_step_clk[2][NB2_CLK_WARPS][NB2_CLK_SLOTS];  // [forward
 
 // PW: the variant with a per-world inertia table (nb2_step_forward_pw).  A compile-time switch: as a run-time pointer test it cost the
 // shared-table kernels registers (fp32) and spills (fp64).
-template <class R, int K, bool PW>
-__global__ void __launch_bounds__(128)
+template <class R, int K, int W, bool PW>
+__global__ void __launch_bounds__(GroupShape<K, W>::MAX_THREADS)
 k_step_fwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, const float* __restrict__ state,
            const float* __restrict__ action, float* __restrict__ next, R* __restrict__ saved, int words,
            float* __restrict__ state_copy, float* __restrict__ action_copy, const double* __restrict__ winertia) {
   // worlds [w0, w0 + count) of a batch of B (B is the stride of the saved stream and of the per-world inertia; the host entry points launch chunks)
   extern __shared__ __align__(16) unsigned char nb2_smem[];
+  constexpr int ST = GroupShape<K, W>::ST, NT = GroupShape<K, W>::THREADS;
+  const GroupPos<K, W> gp(count);
   NB2_CLK(0, 0);
-  constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
-  const int li = threadIdx.x & 31, slot = li / K, lane = li % K;
-  const int g0 = (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * WPW;  // first world of this warp's group
-  const int nworlds = min(WPW, count - g0);                                      // <= 0: idle warp (grid tail)
-  const bool valid = slot < nworlds;
-  const size_t wg = (size_t)w0 + (nworlds > 0 ? g0 : 0);
-  R* scr0 = reinterpret_cast<R*>(nb2_smem) + body_table_words<K>(M.nb) + (size_t)(threadIdx.x >> 5) * words * ST;
-  R* scr = scr0 + slot;
-  R* sv = saved ? saved + wg + (valid ? slot : 0) : nullptr;
-  const double* wi = PW ? winertia + wg + (valid ? slot : 0) : nullptr;
+  const int nworlds = gp.nworlds;
+  const bool valid = gp.valid();
+  const size_t wg = (size_t)w0 + (nworlds > 0 ? gp.g0 : 0);
+  R* scr0 = reinterpret_cast<R*>(nb2_smem) + (size_t)gp.gb * words * ST;
+  R* scr = scr0 + gp.slot;
+  R* sv = saved ? saved + wg + (valid ? gp.slot : 0) : nullptr;
+  const double* wi = PW ? winertia + wg + (valid ? gp.slot : 0) : nullptr;
   constexpr unsigned sync_mask = (K > 1) ? NB2_FWD_SYNC_MASK : NB2_FWD_SYNC_MASK_1LANE;
   grid_dependency_wait();
   NB2_CLK(0, 1);
-  // input rows of the group: through the bulk-copy staging buffer when they qualify, else read in place.  The copy is in
-  // flight while the block stages the body table: the table's constant-bank loads (one replay per distinct address) and
-  // the DRAM round trip of the rows overlap instead of adding up.
+  // input rows of the group: through the bulk-copy staging buffer when they qualify, else read in place
   const float* st_src = state + wg * 2 * M.ndof;
   const float* act_src = action + wg * M.na;
-  unsigned long long* bar = nullptr;
   if (nworlds > 0) {
     const size_t sb = (size_t)nworlds * 2 * M.ndof * sizeof(float), ab = (size_t)nworlds * M.na * sizeof(float);
     if (bulk_ok(st_src, sb) && bulk_ok(act_src, ab)) {
-      unsigned char* stg = nb2_smem + (((size_t)body_table_words<K>(M.nb) + (size_t)(blockDim.x >> 5) * words * ST) * sizeof(R) + 15 & ~(size_t)15) +
-                           (size_t)(threadIdx.x >> 5) * staging_bytes<K>(2 * M.ndof + M.na);
-      bar = reinterpret_cast<unsigned long long*>(stg + staging_bytes<K>(2 * M.ndof + M.na) - 16);
-      if (li == 0) {
+      unsigned char* stg = nb2_smem + (((size_t)(blockDim.x / NT) * words * ST) * sizeof(R) + 15 & ~(size_t)15) +
+                           (size_t)gp.gb * staging_bytes<W>(2 * M.ndof + M.na);
+      unsigned long long* bar = reinterpret_cast<unsigned long long*>(stg + staging_bytes<W>(2 * M.ndof + M.na) - 16);
+      if (gp.tid == 0) {
         mbar_init(bar);
         mbar_expect_tx(bar, (unsigned)(sb + ab));
         bulk_g2s(stg, st_src, (unsigned)sb, bar);
@@ -142,48 +139,44 @@ k_step_fwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
       }
       st_src = reinterpret_cast<const float*>(stg);
       act_src = reinterpret_cast<const float*>(stg + sb);
+      group_sync<K>();  // the mbarrier is initialised before any thread of the group polls it
+      mbar_wait(bar, 0);
     }
-  }
-  const R* bt = stage_body_table<R, K>(M, reinterpret_cast<R*>(nb2_smem));
-  if (bar) {
-    __syncwarp();
-    mbar_wait(bar, 0);
   }
   NB2_CLK(0, 2);
 #pragma unroll 1
   for (int sg = 0; sg < NB2_FWD_STAGES; sg++) {
     if (sg == 0) {
-      if (nworlds > 0) nb2::fwd_load<R, ST>(M, scr0, st_src, act_src, nworlds, li, 32,
+      if (nworlds > 0) nb2::fwd_load<R, ST>(M, scr0, st_src, act_src, nworlds, gp.tid, NT,
                                             state_copy ? state_copy + wg * 2 * M.ndof : nullptr, action_copy ? action_copy + wg * M.na : nullptr);
     }
-    else if (sg == NB2_FWD_STAGES - 1) { if (nworlds > 0) nb2::fwd_store<R, ST>(M, scr0, next + wg * 2 * M.ndof, nworlds, li, 32); }
-    else if (valid) nb2::world_forward_stage<R, ST>(M, scr, sv, (size_t)B, saved != nullptr, lane, sg, bt, nullptr, wi, (size_t)B);
-    if ((sync_mask >> sg) & 1u) __syncwarp();
+    else if (sg == NB2_FWD_STAGES - 1) { if (nworlds > 0) nb2::fwd_store<R, ST>(M, scr0, next + wg * 2 * M.ndof, nworlds, gp.tid, NT); }
+    else if (valid) nb2::world_forward_stage<R, ST>(M, scr, sv, (size_t)B, saved != nullptr, gp.lane, sg, nullptr, nullptr, wi, (size_t)B);
+    if ((sync_mask >> sg) & 1u) group_sync<K>();
     NB2_CLK(0, 3 + sg);
   }
 }
 
-template <class R, int K, bool PW>
-__global__ void __launch_bounds__(128)
+template <class R, int K, int W, bool PW>
+__global__ void __launch_bounds__(GroupShape<K, W>::MAX_THREADS)
 k_step_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, const float* __restrict__ state,
            const float* __restrict__ action, const R* __restrict__ saved, const float* __restrict__ gnext,
            float* __restrict__ gstate, float* __restrict__ gaction, float* __restrict__ ginertia, int words,
            int stage_saved, int accumulate_state, unsigned in_stage_off, const double* __restrict__ winertia, double* __restrict__ ginertia_acc) {
   extern __shared__ __align__(16) unsigned char nb2_smem[];
+  constexpr int WPG = GroupShape<K, W>::WPG, ST = GroupShape<K, W>::ST, NT = GroupShape<K, W>::THREADS;
+  const GroupPos<K, W> gp(count);
   NB2_CLK(1, 0);
-  constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
-  const int li = threadIdx.x & 31, slot = li / K, lane = li % K;
-  const int g0 = (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * WPW;
-  const int nworlds = min(WPW, count - g0);
-  const bool valid = slot < nworlds;
-  const size_t wg = (size_t)w0 + (nworlds > 0 ? g0 : 0);
-  const size_t w = wg + (valid ? slot : 0);
-  R* scr0 = reinterpret_cast<R*>(nb2_smem) + body_table_words<K>(M.nb) + (size_t)(threadIdx.x >> 5) * words * ST;
-  R* scr = scr0 + slot;
+  const int nworlds = gp.nworlds;
+  const bool valid = gp.valid();
+  const size_t wg = (size_t)w0 + (nworlds > 0 ? gp.g0 : 0);
+  const size_t w = wg + (valid ? gp.slot : 0);
+  R* scr0 = reinterpret_cast<R*>(nb2_smem) + (size_t)gp.gb * words * ST;
+  R* scr = scr0 + gp.slot;
   grid_dependency_wait();  // no global access above this line (see k_step_fwd)
   NB2_CLK(1, 1);
-  // input rows (dL/dx', x, u) of the group through the bulk-copy staging buffer when they qualify; in flight, like the
-  // saved-stream burst below, while the block stages the body table (see k_step_fwd)
+  // input rows (dL/dx', x, u) of the group through the bulk-copy staging buffer when they qualify; in flight while the group
+  // issues the saved-stream burst below
   const float* g_src = gnext + wg * 2 * M.ndof;
   const float* st_src = state + wg * 2 * M.ndof;
   const float* act_src = action + wg * M.na;
@@ -191,9 +184,9 @@ k_step_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
   if (nworlds > 0 && in_stage_off) {
     const size_t sb = (size_t)nworlds * 2 * M.ndof * sizeof(float), ab = (size_t)nworlds * M.na * sizeof(float);
     if (bulk_ok(g_src, sb) && bulk_ok(st_src, sb) && bulk_ok(act_src, ab)) {
-      unsigned char* stg = nb2_smem + in_stage_off + (size_t)(threadIdx.x >> 5) * staging_bytes<K>(4 * M.ndof + M.na);
-      bar = reinterpret_cast<unsigned long long*>(stg + staging_bytes<K>(4 * M.ndof + M.na) - 16);
-      if (li == 0) {
+      unsigned char* stg = nb2_smem + in_stage_off + (size_t)gp.gb * staging_bytes<W>(4 * M.ndof + M.na);
+      bar = reinterpret_cast<unsigned long long*>(stg + staging_bytes<W>(4 * M.ndof + M.na) - 16);
+      if (gp.tid == 0) {
         mbar_init(bar);
         mbar_expect_tx(bar, (unsigned)(2 * sb + ab));
         bulk_g2s(stg, g_src, (unsigned)sb, bar);
@@ -206,100 +199,96 @@ k_step_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, int w0, int count, c
     }
   }
   // The sweeps walk the saved stream body by body, every access a dependent DRAM round trip.  When the launch leaves room
-  // (small batches: the regime where latency is all that matters) each warp first pulls its group's rows of the stream
-  // into shared memory with one burst of asynchronous 16-byte copies ([word][B] layout: the group's worlds are adjacent),
-  // and the sweeps then read `svp` with stride `svB` = WPW instead of the global stream with stride B.
-  const R* svp = saved + wg + (valid ? slot : 0);
+  // (small batches: the regime where latency is all that matters) each group first pulls its rows of the stream into shared
+  // memory with one burst of asynchronous 16-byte copies by all its threads ([word][B] layout: the group's 32 worlds are
+  // adjacent, a row of the group is 128 B in fp32), and the sweeps then read `svp` with stride `svB` = 32 instead of the global
+  // stream with stride B.
+  const R* svp = saved + wg + (valid ? gp.slot : 0);
   size_t svB = (size_t)B;
-  if (stage_saved && nworlds == WPW) {
+  if (stage_saved && nworlds == WPG) {
     const int sw = nb2_saved_words(M.nb, M.ndof, M.nfree);
-    R* svs = reinterpret_cast<R*>(nb2_smem) + ((body_table_words<K>(M.nb) + (size_t)(blockDim.x >> 5) * words * ST + 3) & ~(size_t)3)  // 16-byte aligned
-             + (size_t)(threadIdx.x >> 5) * sw * WPW;
-    constexpr int CH = (WPW * (int)sizeof(R)) / 16;  // 16-byte chunks per row of the group
+    R* svs = reinterpret_cast<R*>(nb2_smem + (((size_t)(blockDim.x / NT) * words * ST * sizeof(R) + 15) & ~(size_t)15))  // 16-byte aligned
+             + (size_t)gp.gb * sw * WPG;
+    constexpr int CH = (WPG * (int)sizeof(R)) / 16;  // 16-byte chunks per row of the group
     const unsigned dst0 = (unsigned)__cvta_generic_to_shared(svs);
     const char* src0 = reinterpret_cast<const char*>(saved + wg);
-    for (int idx = li; idx < sw * CH; idx += 32) {
+    for (int idx = gp.tid; idx < sw * CH; idx += NT) {
       const int k = idx / CH, c = idx - k * CH;
-      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst0 + (unsigned)(k * WPW * (int)sizeof(R) + c * 16)),
+      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst0 + (unsigned)(k * WPG * (int)sizeof(R) + c * 16)),
                    "l"(src0 + (size_t)k * B * sizeof(R) + c * 16));
     }
     asm volatile("cp.async.commit_group;");
-    svp = svs + slot;
-    svB = WPW;
+    svp = svs + gp.slot;
+    svB = WPG;
   }
   constexpr unsigned sync_mask = (K > 1) ? NB2_BWD_SYNC_MASK : NB2_BWD_SYNC_MASK_1LANE;
-  const R* bt = stage_body_table<R, K>(M, reinterpret_cast<R*>(nb2_smem));
   if (bar) {
-    __syncwarp();
+    group_sync<K>();  // the mbarrier is initialised before any thread of the group polls it
     mbar_wait(bar, 0);
   }
   NB2_CLK(1, 2);
 #pragma unroll 1
   for (int sg = 0; sg < NB2_BWD_STAGES; sg++) {
-    if (sg == 0) { if (nworlds > 0) nb2::bwd_load<R, ST, false>(M, scr0, st_src, act_src, g_src, nworlds, li, 32); }
+    if (sg == 0) { if (nworlds > 0) nb2::bwd_load<R, ST, false>(M, scr0, st_src, act_src, g_src, nworlds, gp.tid, NT); }
     else if (sg == NB2_BWD_STAGES - 1) {
-      if (nworlds > 0) nb2::bwd_store<R, ST, false>(M, scr0, gstate + wg * 2 * M.ndof, gaction + wg * M.na, false, nworlds, li, 32, accumulate_state != 0);
-    } else if (valid) nb2::world_backward_stage<R, ST>(M, scr, svp, svB, lane, sg, ginertia ? ginertia + w : nullptr, bt, (size_t)B, nullptr,
+      if (nworlds > 0) nb2::bwd_store<R, ST, false>(M, scr0, gstate + wg * 2 * M.ndof, gaction + wg * M.na, false, nworlds, gp.tid, NT, accumulate_state != 0);
+    } else if (valid) nb2::world_backward_stage<R, ST>(M, scr, svp, svB, gp.lane, sg, ginertia ? ginertia + w : nullptr, nullptr, (size_t)B, nullptr,
                                                        (PW && winertia) ? winertia + w : nullptr, (size_t)B, (PW && ginertia_acc) ? ginertia_acc + w : nullptr);
     if (sg == 0 && stage_saved) asm volatile("cp.async.wait_group 0;" ::: "memory");
-    if (((sync_mask >> sg) & 1u) || (sg == 0 && stage_saved)) __syncwarp();
+    if (((sync_mask >> sg) & 1u) || (sg == 0 && stage_saved)) group_sync<K>();
     NB2_CLK(1, 3 + sg);
   }
 }
 
-// ---- inverse dynamics (nb2_inverse_dynamics / _backward): the warp shape of the step kernels (K lanes per world, [word][slot]
-// scratch in shared memory), I/O rows in the arithmetic type R.  Per-world inertia is a run-time pointer test here: it costs these
-// kernels no spill (-Xptxas -v), unlike the step kernels (see k_step_fwd).
-template <class R, int K>
-__global__ void __launch_bounds__(128)
+// ---- inverse dynamics (nb2_inverse_dynamics / _backward): the group shape of the step kernels (nb2_coop.cuh), I/O rows in the
+// arithmetic type R.  Per-world inertia is a run-time pointer test here: it costs these kernels no spill (-Xptxas -v), unlike the
+// step kernels (see k_step_fwd).
+template <class R, int K, int W>
+__global__ void __launch_bounds__(GroupShape<K, W>::MAX_THREADS)
 k_id_fwd(const __grid_constant__ Nb2ModelDev<R> M, int B, const R* __restrict__ state, const R* __restrict__ next_vel, R* __restrict__ tau,
          R* __restrict__ saved, int words, const double* __restrict__ winertia) {
   extern __shared__ __align__(16) unsigned char nb2_smem[];
-  constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
-  const int li = threadIdx.x & 31, slot = li / K, lane = li % K;
-  const int g0 = (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * WPW;
-  const int nworlds = min(WPW, B - g0);  // <= 0: idle warp (grid tail)
-  const bool valid = slot < nworlds;
-  const size_t wg = nworlds > 0 ? g0 : 0, w = wg + (valid ? slot : 0);
-  const R* bt = stage_body_table<R, K>(M, reinterpret_cast<R*>(nb2_smem));
-  R* scr0 = reinterpret_cast<R*>(nb2_smem) + body_table_words<K>(M.nb) + (size_t)(threadIdx.x >> 5) * words * ST;
-  R* scr = scr0 + slot;
+  constexpr int ST = GroupShape<K, W>::ST, NT = GroupShape<K, W>::THREADS;
+  const GroupPos<K, W> gp(B);
+  const int nworlds = gp.nworlds;
+  const bool valid = gp.valid();
+  const size_t wg = nworlds > 0 ? gp.g0 : 0, w = wg + (valid ? gp.slot : 0);
+  R* scr0 = reinterpret_cast<R*>(nb2_smem) + (size_t)gp.gb * words * ST;
+  R* scr = scr0 + gp.slot;
   R* sv = saved ? saved + w : nullptr;
   const double* wi = winertia ? winertia + w : nullptr;
   constexpr unsigned sync_mask = (K > 1) ? NB2_ID_FWD_SYNC_MASK : NB2_ID_FWD_SYNC_MASK_1LANE;
 #pragma unroll 1
   for (int sg = 0; sg < NB2_ID_FWD_STAGES; sg++) {
-    if (sg == 0) { if (nworlds > 0) nb2::id_load<R, ST>(M, scr0, state + wg * 2 * M.ndof, next_vel + wg * M.ndof, nworlds, li, 32); }
-    else if (sg == NB2_ID_FWD_STAGES - 1) { if (nworlds > 0) nb2::id_store<R, ST>(M, scr0, tau + wg * M.ndof, nworlds, li, 32); }
-    else if (valid) nb2::id_forward_stage<R, ST>(M, scr, sv, (size_t)B, saved != nullptr, lane, sg, bt, wi, (size_t)B);
-    if ((sync_mask >> sg) & 1u) __syncwarp();
+    if (sg == 0) { if (nworlds > 0) nb2::id_load<R, ST>(M, scr0, state + wg * 2 * M.ndof, next_vel + wg * M.ndof, nworlds, gp.tid, NT); }
+    else if (sg == NB2_ID_FWD_STAGES - 1) { if (nworlds > 0) nb2::id_store<R, ST>(M, scr0, tau + wg * M.ndof, nworlds, gp.tid, NT); }
+    else if (valid) nb2::id_forward_stage<R, ST>(M, scr, sv, (size_t)B, saved != nullptr, gp.lane, sg, nullptr, wi, (size_t)B);
+    if ((sync_mask >> sg) & 1u) group_sync<K>();
   }
 }
 
-template <class R, int K>
-__global__ void __launch_bounds__(128)
+template <class R, int K, int W>
+__global__ void __launch_bounds__(GroupShape<K, W>::MAX_THREADS)
 k_id_bwd(const __grid_constant__ Nb2ModelDev<R> M, int B, const R* __restrict__ state, const R* __restrict__ saved, const R* __restrict__ gtau,
          R* __restrict__ gstate, R* __restrict__ gnext, double* __restrict__ ginertia, int words, const double* __restrict__ winertia) {
   extern __shared__ __align__(16) unsigned char nb2_smem[];
-  constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
-  const int li = threadIdx.x & 31, slot = li / K, lane = li % K;
-  const int g0 = (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * WPW;
-  const int nworlds = min(WPW, B - g0);
-  const bool valid = slot < nworlds;
-  const size_t wg = nworlds > 0 ? g0 : 0, w = wg + (valid ? slot : 0);
-  const R* bt = stage_body_table<R, K>(M, reinterpret_cast<R*>(nb2_smem));
-  R* scr0 = reinterpret_cast<R*>(nb2_smem) + body_table_words<K>(M.nb) + (size_t)(threadIdx.x >> 5) * words * ST;
-  R* scr = scr0 + slot;
+  constexpr int ST = GroupShape<K, W>::ST, NT = GroupShape<K, W>::THREADS;
+  const GroupPos<K, W> gp(B);
+  const int nworlds = gp.nworlds;
+  const bool valid = gp.valid();
+  const size_t wg = nworlds > 0 ? gp.g0 : 0, w = wg + (valid ? gp.slot : 0);
+  R* scr0 = reinterpret_cast<R*>(nb2_smem) + (size_t)gp.gb * words * ST;
+  R* scr = scr0 + gp.slot;
   const double* wi = winertia ? winertia + w : nullptr;
   double* gI = ginertia ? ginertia + w : nullptr;
   constexpr unsigned sync_mask = (K > 1) ? NB2_ID_BWD_SYNC_MASK : NB2_ID_BWD_SYNC_MASK_1LANE;
 #pragma unroll 1
   for (int sg = 0; sg < NB2_ID_BWD_STAGES; sg++) {
-    if (sg == 0) { if (nworlds > 0) nb2::id_bwd_load<R, ST>(M, scr0, state + wg * 2 * M.ndof, gtau + wg * M.ndof, nworlds, li, 32); }
+    if (sg == 0) { if (nworlds > 0) nb2::id_bwd_load<R, ST>(M, scr0, state + wg * 2 * M.ndof, gtau + wg * M.ndof, nworlds, gp.tid, NT); }
     else if (sg == NB2_ID_BWD_STAGES - 1) {
-      if (nworlds > 0) nb2::id_bwd_store<R, ST>(M, scr0, gstate + wg * 2 * M.ndof, gnext + wg * M.ndof, nworlds, li, 32);
-    } else if (valid) nb2::id_backward_stage<R, ST>(M, scr, saved + w, (size_t)B, lane, sg, bt, wi, (size_t)B, gI, (size_t)B);
-    if ((sync_mask >> sg) & 1u) __syncwarp();
+      if (nworlds > 0) nb2::id_bwd_store<R, ST>(M, scr0, gstate + wg * 2 * M.ndof, gnext + wg * M.ndof, nworlds, gp.tid, NT);
+    } else if (valid) nb2::id_backward_stage<R, ST>(M, scr, saved + w, (size_t)B, gp.lane, sg, nullptr, wi, (size_t)B, gI, (size_t)B);
+    if ((sync_mask >> sg) & 1u) group_sync<K>();
   }
 }
 
@@ -1072,18 +1061,20 @@ template <auto Kern> static int allow_max_smem() {
 }
 
 // the same for the forward-dynamics kernels of nb2_fd.cu, reached through their host stubs
-template <class R, int K> static int allow_max_smem_fd(int bwd) {
+template <class R, int K, int W> static int allow_max_smem_fd(int bwd) {
   static std::atomic<bool> done[2][64];
   int dev = 0; NB2_CUDA(cudaGetDevice(&dev));
   if (!done[bwd][dev & 63].load(std::memory_order_acquire)) {
-    NB2_CUDA(cudaFuncSetAttribute(nb2_fd_kernel<R>(K, bwd), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
+    NB2_CUDA(cudaFuncSetAttribute(nb2_fd_kernel<R>(K, W, bwd), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
     done[bwd][dev & 63].store(true, std::memory_order_release);
   }
   return NB2_OK;
 }
 
 // one sweep schedule of the model (same bodies, different lane count / slot assignment)
-struct LaunchShape { int warps_per_block = 0; int resident_warps = 0; };  // filled lazily from the occupancy API
+// groups of `wpg` worlds (nb2_coop.cuh): 32, or NARROW_W<K> for a K-lane schedule whose 32-world group does not fit (prepare_k);
+// filled lazily from the occupancy API
+struct LaunchShape { int groups_per_block = 0; int resident_groups = 0; int wpg = 32; };
 struct nb2_variant {
   Nb2ModelDev<float> mf;
   Nb2ModelDev<double> md;
@@ -1147,66 +1138,81 @@ static void init_variant(nb2_variant& v) {
 
 // ---- launch shape.  The kernels are latency bound (one dependent chain per world), so a launch costs about
 //   (sequential depth of the schedule) x (number of waves the batch needs at that schedule's occupancy).
-// Occupancy is limited by the per-warp scratch in shared memory; blocks of 1, 2 or 4 warps are tried and the shape
-// that keeps most warps resident wins.  Small batches use 1-warp blocks so that they spread over all SMs.
-template <class Kern>
-static LaunchShape occupancy_shape(Kern kern, size_t bytes_per_warp, size_t bytes_per_block) {
+// Occupancy is limited by the per-group scratch in shared memory; blocks of 1, 2 or 4 groups (of at most 128 threads, or one group
+// when a group is larger: GroupShape) are tried and the shape that keeps most groups resident wins.  Small batches use one-group
+// blocks so that they spread over all SMs.
+template <int K, int W, class Kern>
+static LaunchShape occupancy_shape(Kern kern, size_t bytes_per_group, size_t bytes_per_block) {
   LaunchShape best;
-  for (int w = 1; w <= 4; w *= 2) {
-    const size_t smem = bytes_per_warp * w + bytes_per_block;
+  best.wpg = W;
+  for (int g = 1; g <= GroupShape<K, W>::MAX_GROUPS; g *= 2) {
+    const size_t smem = bytes_per_group * g + bytes_per_block;
     if (smem > (size_t)kMaxSmem) break;
     int blocks = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kern, w * 32, smem) != cudaSuccess) { cudaGetLastError(); continue; }
-    if (blocks * w > best.resident_warps) { best.resident_warps = blocks * w; best.warps_per_block = w; }
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kern, g * GroupShape<K, W>::THREADS, smem) != cudaSuccess) { cudaGetLastError(); continue; }
+    if (blocks * g > best.resident_groups) { best.resident_groups = blocks * g; best.groups_per_block = g; }
   }
   return best;
 }
 
-// warps per block for one launch: a batch that fits in one wave is spread so that every SM gets about the same number of
-// warps in as few blocks as possible (measured: 4 warps in one block beat 4 one-warp blocks on the same SM); beyond one
+// groups per block for one launch: a batch that fits in one wave is spread so that every SM gets about the same number of
+// groups in as few blocks as possible (measured: 4 warps in one block beat 4 one-warp blocks on the same SM); beyond one
 // wave the occupancy-optimal shape is used.
-static int block_warps(int total_warps, int sm_count, const LaunchShape& sh, size_t per_warp) {
-  if ((long long)total_warps > (long long)sm_count * sh.resident_warps) return sh.warps_per_block;
-  int w = 1;
-  while (w < 4 && total_warps > sm_count * w && (size_t)(2 * w) * per_warp <= (size_t)kMaxSmem) w *= 2;
-  return w;
+template <int K>
+static int block_groups(int total_groups, int sm_count, const LaunchShape& sh, size_t per_group) {
+  if ((long long)total_groups > (long long)sm_count * sh.resident_groups) return sh.groups_per_block;
+  int g = 1;
+  while (g < GroupShape<K>::MAX_GROUPS && total_groups > sm_count * g && (size_t)(2 * g) * per_group <= (size_t)kMaxSmem) g *= 2;
+  return g;
 }
+static int groups_of(int B, int wpg) { return (B + wpg - 1) / wpg; }
 
-template <class R, int K>
-static int prepare_k(nb2_variant& v, int dir) {  // dir: LF_*
-  constexpr int ST = CoopShape<K>::ST;
+template <class R, int K, int W>
+static int prepare_kw(nb2_variant& v, int dir) {  // dir: LF_*
+  constexpr int ST = GroupShape<K, W>::ST;
   LaunchShape& sh = v.shape[dir][sizeof(R) == 8];
-  // the occupancy query sizes a step warp with its scratch AND its input-staging buffer, in both directions (the inverse- and
+  // the occupancy query sizes a step group with its scratch AND its input-staging buffer, in both directions (the inverse- and
   // forward-dynamics kernels stage nothing)
   const size_t scratch_and_staging =
       dir == LF_ID_FWD || dir == LF_FD_FWD ? (size_t)v.fwd_words * ST * sizeof(R) : dir == LF_ID_BWD ? (size_t)v.id_bwd_words * ST * sizeof(R) :
       dir == LF_FD_BWD ? (size_t)v.bwd_words * ST * sizeof(R) :
       (size_t)(dir ? v.bwd_words : v.fwd_words) * ST * sizeof(R) +
-          (dir ? staging_bytes<K>(4 * v.mf.ndof + v.mf.na) : staging_bytes<K>(2 * v.mf.ndof + v.mf.na));
-  const size_t per_block = (size_t)body_table_words<K>(v.mf.nb) * sizeof(R) + 16;
+          (dir ? staging_bytes<W>(4 * v.mf.ndof + v.mf.na) : staging_bytes<W>(2 * v.mf.ndof + v.mf.na));
+  const size_t per_block = 16;
   if (scratch_and_staging + per_block > (size_t)kMaxSmem) {
-    g_err = "model needs " + std::to_string(scratch_and_staging) + " B of shared memory per warp (> 227 KB)"; return NB2_ERR_UNSUPPORTED;
+    g_err = "model needs " + std::to_string(scratch_and_staging) + " B of shared memory per group of " + std::to_string(W) + " worlds (> 227 KB)"; return NB2_ERR_UNSUPPORTED;
   }
   int rc;
   if (dir == 0) {  // the per-world-inertia variant launches with the shape of the shared-table kernel
-    if ((rc = allow_max_smem<k_step_fwd<R, K, false>>()) || (rc = allow_max_smem<k_step_fwd<R, K, true>>())) return rc;
-    if (!sh.warps_per_block) sh = occupancy_shape(k_step_fwd<R, K, false>, scratch_and_staging, per_block);
+    if ((rc = allow_max_smem<k_step_fwd<R, K, W, false>>()) || (rc = allow_max_smem<k_step_fwd<R, K, W, true>>())) return rc;
+    if (!sh.groups_per_block) sh = occupancy_shape<K, W>(k_step_fwd<R, K, W, false>, scratch_and_staging, per_block);
   } else if (dir == LF_STEP_BWD) {
-    if ((rc = allow_max_smem<k_step_bwd<R, K, false>>()) || (rc = allow_max_smem<k_step_bwd<R, K, true>>())) return rc;
-    if (!sh.warps_per_block) sh = occupancy_shape(k_step_bwd<R, K, false>, scratch_and_staging, per_block);
+    if ((rc = allow_max_smem<k_step_bwd<R, K, W, false>>()) || (rc = allow_max_smem<k_step_bwd<R, K, W, true>>())) return rc;
+    if (!sh.groups_per_block) sh = occupancy_shape<K, W>(k_step_bwd<R, K, W, false>, scratch_and_staging, per_block);
   } else if (dir == LF_ID_FWD) {
-    if ((rc = allow_max_smem<k_id_fwd<R, K>>())) return rc;
-    if (!sh.warps_per_block) sh = occupancy_shape(k_id_fwd<R, K>, scratch_and_staging, per_block);
+    if ((rc = allow_max_smem<k_id_fwd<R, K, W>>())) return rc;
+    if (!sh.groups_per_block) sh = occupancy_shape<K, W>(k_id_fwd<R, K, W>, scratch_and_staging, per_block);
   } else if (dir == LF_ID_BWD) {
-    if ((rc = allow_max_smem<k_id_bwd<R, K>>())) return rc;
-    if (!sh.warps_per_block) sh = occupancy_shape(k_id_bwd<R, K>, scratch_and_staging, per_block);
+    if ((rc = allow_max_smem<k_id_bwd<R, K, W>>())) return rc;
+    if (!sh.groups_per_block) sh = occupancy_shape<K, W>(k_id_bwd<R, K, W>, scratch_and_staging, per_block);
   } else {  // the forward-dynamics kernels live in nb2_fd.cu
     const int bwd = dir == LF_FD_BWD;
-    if ((rc = allow_max_smem_fd<R, K>(bwd))) return rc;
-    if (!sh.warps_per_block) sh = occupancy_shape(nb2_fd_kernel<R>(K, bwd), scratch_and_staging, per_block);
+    if ((rc = allow_max_smem_fd<R, K, W>(bwd))) return rc;
+    if (!sh.groups_per_block) sh = occupancy_shape<K, W>(nb2_fd_kernel<R>(K, W, bwd), scratch_and_staging, per_block);
   }
-  if (!sh.warps_per_block) { g_err = "no launch shape fits this model"; return NB2_ERR_UNSUPPORTED; }
+  if (!sh.groups_per_block) { g_err = "no launch shape fits this model"; return NB2_ERR_UNSUPPORTED; }
   return NB2_OK;
+}
+// The 32-world group, or for a multi-lane schedule a narrow group of 32/K worlds when the 32-world group's working set does not fit
+// shared memory (the largest models; in fp64 also smaller ones): a narrow group needs what one warp of the earlier in-warp shape
+// (32/K worlds per warp) needed, so every model that fitted a schedule then fits one now.
+template <class R, int K>
+static int prepare_k(nb2_variant& v, int dir) {
+  const int rc = prepare_kw<R, K, 32>(v, dir);
+  if constexpr (K > 1) {
+    if (rc == NB2_ERR_UNSUPPORTED) return prepare_kw<R, K, NARROW_W<K>>(v, dir);
+  }
+  return rc;
 }
 template <class R>
 static int prepare_variant(nb2_variant& v, int dir) {
@@ -1222,8 +1228,7 @@ static int pick_variant(nb2_model* m, int B, int dir, nb2_variant** out) {
     int rc = prepare_variant<R>(v, dir);
     if (rc) { if (m->variants.size() == 1 || m->forced_lanes) return rc; continue; }
     const LaunchShape& sh = v.shape[dir][sizeof(R) == 8];
-    const double warps = ((double)B * v.mf.lanes + 31) / 32;
-    double waves = warps / ((double)m->sm_count * sh.resident_warps);
+    double waves = (double)groups_of(B, sh.wpg) / ((double)m->sm_count * sh.resident_groups);
     if (waves < 1) waves = 1;
     const double cost = (v.depth + 3) * waves;   // +3: per-sweep fixed part (loads, stores, barriers)
     if (!best || cost < best_cost - 1e-9) { best = &v; best_cost = cost; }
@@ -1252,19 +1257,27 @@ static void launch_dependent(void (*kern)(P...), int blocks, int threads, size_t
   cudaLaunchKernelEx(&cfg, kern, std::forward<A>(args)...);
 }
 
-template <class R, int K>
-static int launch_fwd_k(const nb2_variant& v, int sm_count, int Btot, int w0, int B, const float* state, const float* action,
-                        float* next, R* saved, cudaStream_t st, float* state_copy, float* action_copy, const double* wi) {
-  constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
+// Calls f with the group width of launch shape `sh` as a compile-time std::integral_constant (narrow groups exist for K > 1 only).
+template <int K, class F> static int with_width(const LaunchShape& sh, F&& f) {
+  if constexpr (K > 1) {
+    if (sh.wpg == NARROW_W<K>) return f(std::integral_constant<int, NARROW_W<K>>());
+  }
+  return f(std::integral_constant<int, 32>());
+}
+
+template <class R, int K, int W>
+static int launch_fwd_kw(const nb2_variant& v, int sm_count, int Btot, int w0, int B, const float* state, const float* action,
+                         float* next, R* saved, cudaStream_t st, float* state_copy, float* action_copy, const double* wi) {
+  constexpr int ST = GroupShape<K, W>::ST, NT = GroupShape<K, W>::THREADS;
   const LaunchShape& sh = v.shape[0][sizeof(R) == 8];
-  const size_t per_warp = (size_t)v.fwd_words * ST * sizeof(R) + staging_bytes<K>(2 * v.mf.ndof + v.mf.na);  // scratch + input staging
-  const int total_warps = (B + WPW - 1) / WPW;
-  const int warps = block_warps(total_warps, sm_count, sh, per_warp);
-  const int blocks = (total_warps + warps - 1) / warps;
-  const size_t smem = per_warp * warps + (size_t)body_table_words<K>(v.mf.nb) * sizeof(R) + 16;
-  if (wi) launch_dependent(k_step_fwd<R, K, true>, blocks, warps * 32, smem, st, model_of<R>(v), Btot, w0, B, state, action, next, saved, v.fwd_words,
+  const size_t per_group = (size_t)v.fwd_words * ST * sizeof(R) + staging_bytes<W>(2 * v.mf.ndof + v.mf.na);  // scratch + input staging
+  const int total_groups = groups_of(B, W);
+  const int groups = block_groups<K>(total_groups, sm_count, sh, per_group);
+  const int blocks = (total_groups + groups - 1) / groups;
+  const size_t smem = per_group * groups + 16;
+  if (wi) launch_dependent(k_step_fwd<R, K, W, true>, blocks, groups * NT, smem, st, model_of<R>(v), Btot, w0, B, state, action, next, saved, v.fwd_words,
                            state_copy, action_copy, wi);
-  else launch_dependent(k_step_fwd<R, K, false>, blocks, warps * 32, smem, st, model_of<R>(v), Btot, w0, B, state, action, next, saved, v.fwd_words,
+  else launch_dependent(k_step_fwd<R, K, W, false>, blocks, groups * NT, smem, st, model_of<R>(v), Btot, w0, B, state, action, next, saved, v.fwd_words,
                         state_copy, action_copy, nullptr);
   g_launches++;
   NB2_CUDA(cudaGetLastError());
@@ -1278,39 +1291,41 @@ static int launch_fwd(nb2_model* m, int B, const float* state, const float* acti
   int rc = pick_variant<R>(m, B, 0, &pv);
   if (rc) return rc;
   return with_lanes(pv->mf.lanes, [&](auto k) {
-    return launch_fwd_k<R, decltype(k)::value>(*pv, m->sm_count, Btot, w0, B, state, action, next, saved, st, state_copy, action_copy, wi);
+    constexpr int K = decltype(k)::value;
+    return with_width<K>(pv->shape[0][sizeof(R) == 8], [&](auto w) {
+      return launch_fwd_kw<R, K, decltype(w)::value>(*pv, m->sm_count, Btot, w0, B, state, action, next, saved, st, state_copy, action_copy, wi);
+    });
   });
 }
 static bool no_stage_saved() {
   static const bool off = [] { const char* e = getenv("NB2_NO_STAGE_SAVED"); return e && atoi(e); }();
   return off;
 }
-template <class R, int K>
-static int launch_bwd_k(const nb2_variant& v, int sm_count, int Btot, int w0, int B, const float* state, const float* action,
+template <class R, int K, int W>
+static int launch_bwd_kw(const nb2_variant& v, int sm_count, int Btot, int w0, int B, const float* state, const float* action,
                         const R* saved, const float* gnext, float* gstate, float* gaction, float* ginertia, cudaStream_t st, int accumulate,
                         const double* wi, double* gIa) {
-  constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
+  constexpr int ST = GroupShape<K, W>::ST, NT = GroupShape<K, W>::THREADS;
   const LaunchShape& sh = v.shape[1][sizeof(R) == 8];
-  // the warps per block are sized with the scratch only, while prepare_k's occupancy query (scratch_and_staging) also counts the input staging
-  const size_t scratch_per_warp = (size_t)v.bwd_words * ST * sizeof(R);
-  const int total_warps = (B + WPW - 1) / WPW;
-  const int warps = block_warps(total_warps, sm_count, sh, scratch_per_warp);
-  const int blocks = (total_warps + warps - 1) / warps;
-  const size_t tab = (size_t)body_table_words<K>(v.mf.nb) * sizeof(R);
-  // stage the saved stream in shared memory when the whole batch is resident at once anyway (see the kernel)
-  const size_t stage_per_warp = (size_t)nb2_saved_words(v.mf.nb, v.mf.ndof, v.mf.nfree) * WPW * sizeof(R);
-  const bool aligned = (((size_t)Btot * sizeof(R)) % 16 == 0) && (((size_t)w0 * sizeof(R)) % 16 == 0) && ((reinterpret_cast<size_t>(saved) & 15) == 0) &&
-                       ((WPW * sizeof(R)) % 16 == 0);
-  const size_t in_per_warp = staging_bytes<K>(4 * v.mf.ndof + v.mf.na);  // bulk-copy staging of dL/dx', x, u rows
-  const size_t smem_staged = (scratch_per_warp + stage_per_warp) * warps + tab + 16;
+  // the groups per block are sized with the scratch only, while prepare_k's occupancy query (scratch_and_staging) also counts the input staging
+  const size_t scratch_per_group = (size_t)v.bwd_words * ST * sizeof(R);
+  const int total_groups = groups_of(B, W);
+  const int groups = block_groups<K>(total_groups, sm_count, sh, scratch_per_group);
+  const int blocks = (total_groups + groups - 1) / groups;
+  // stage the saved stream in shared memory when the whole batch is resident at once anyway (see the kernel); the rows of a group
+  // are W worlds, a multiple of 16 bytes
+  const size_t stage_per_group = (size_t)nb2_saved_words(v.mf.nb, v.mf.ndof, v.mf.nfree) * W * sizeof(R);
+  const bool aligned = (((size_t)Btot * sizeof(R)) % 16 == 0) && (((size_t)w0 * sizeof(R)) % 16 == 0) && ((reinterpret_cast<size_t>(saved) & 15) == 0);
+  const size_t in_per_group = staging_bytes<W>(4 * v.mf.ndof + v.mf.na);  // bulk-copy staging of dL/dx', x, u rows
+  const size_t smem_staged = (scratch_per_group + stage_per_group) * groups + 16;
   const int blocks_per_sm = (blocks + sm_count - 1) / sm_count;
-  const bool stage = aligned && (smem_staged + in_per_warp * warps) * blocks_per_sm + 1024 * blocks_per_sm <= (size_t)kMaxSmem && !no_stage_saved();
-  const size_t base = ((stage ? smem_staged : scratch_per_warp * warps + tab) + 15) & ~(size_t)15;
-  const bool in_stage = base + in_per_warp * warps <= (size_t)kMaxSmem;
-  const size_t smem = in_stage ? base + in_per_warp * warps : base;
-  if (wi || gIa) launch_dependent(k_step_bwd<R, K, true>, blocks, warps * 32, smem, st, model_of<R>(v), Btot, w0, B, state, action, saved, gnext, gstate,
+  const bool stage = aligned && (smem_staged + in_per_group * groups) * blocks_per_sm + 1024 * blocks_per_sm <= (size_t)kMaxSmem && !no_stage_saved();
+  const size_t base = ((stage ? smem_staged : scratch_per_group * groups) + 15) & ~(size_t)15;
+  const bool in_stage = base + in_per_group * groups <= (size_t)kMaxSmem;
+  const size_t smem = in_stage ? base + in_per_group * groups : base;
+  if (wi || gIa) launch_dependent(k_step_bwd<R, K, W, true>, blocks, groups * NT, smem, st, model_of<R>(v), Btot, w0, B, state, action, saved, gnext, gstate,
                                   gaction, ginertia, v.bwd_words, stage ? 1 : 0, accumulate, in_stage ? (unsigned)base : 0u, wi, gIa);
-  else launch_dependent(k_step_bwd<R, K, false>, blocks, warps * 32, smem, st, model_of<R>(v), Btot, w0, B, state, action, saved, gnext, gstate,
+  else launch_dependent(k_step_bwd<R, K, W, false>, blocks, groups * NT, smem, st, model_of<R>(v), Btot, w0, B, state, action, saved, gnext, gstate,
                         gaction, ginertia, v.bwd_words, stage ? 1 : 0, accumulate, in_stage ? (unsigned)base : 0u, nullptr, nullptr);
   g_launches++;
   NB2_CUDA(cudaGetLastError());
@@ -1325,23 +1340,27 @@ static int launch_bwd(nb2_model* m, int B, const float* state, const float* acti
   int rc = pick_variant<R>(m, B, 1, &pv);
   if (rc) return rc;
   return with_lanes(pv->mf.lanes, [&](auto k) {
-    return launch_bwd_k<R, decltype(k)::value>(*pv, m->sm_count, Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia, st, accumulate, wi, gIa);
+    constexpr int K = decltype(k)::value;
+    return with_width<K>(pv->shape[1][sizeof(R) == 8], [&](auto w) {
+      return launch_bwd_kw<R, K, decltype(w)::value>(*pv, m->sm_count, Btot, w0, B, state, action, saved, gnext, gstate, gaction, ginertia, st,
+                                                     accumulate, wi, gIa);
+    });
   });
 }
 
 // ---- inverse dynamics: the launch family of the step kernels (variant pick, lane schedules, block shape), dir LF_ID_FWD or LF_ID_BWD
-template <class R, int K>
-static int launch_id_k(const nb2_variant& v, int sm_count, int B, int dir, const R* state, const R* next_vel, R* tau, R* saved, const R* gtau,
+template <class R, int K, int W>
+static int launch_id_kw(const nb2_variant& v, int sm_count, int B, int dir, const R* state, const R* next_vel, R* tau, R* saved, const R* gtau,
                        R* gstate, R* gnext, double* gI, const double* wi, cudaStream_t st) {
-  constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
+  constexpr int ST = GroupShape<K, W>::ST, NT = GroupShape<K, W>::THREADS;
   const int words = dir == LF_ID_FWD ? v.fwd_words : v.id_bwd_words;
-  const size_t per_warp = (size_t)words * ST * sizeof(R);
-  const int total_warps = (B + WPW - 1) / WPW;
-  const int warps = block_warps(total_warps, sm_count, v.shape[dir][sizeof(R) == 8], per_warp);
-  const int blocks = (total_warps + warps - 1) / warps;
-  const size_t smem = per_warp * warps + (size_t)body_table_words<K>(v.mf.nb) * sizeof(R);
-  if (dir == LF_ID_FWD) k_id_fwd<R, K><<<blocks, warps * 32, smem, st>>>(model_of<R>(v), B, state, next_vel, tau, saved, words, wi);
-  else k_id_bwd<R, K><<<blocks, warps * 32, smem, st>>>(model_of<R>(v), B, state, saved, gtau, gstate, gnext, gI, words, wi);
+  const size_t per_group = (size_t)words * ST * sizeof(R);
+  const int total_groups = groups_of(B, W);
+  const int groups = block_groups<K>(total_groups, sm_count, v.shape[dir][sizeof(R) == 8], per_group);
+  const int blocks = (total_groups + groups - 1) / groups;
+  const size_t smem = per_group * groups;
+  if (dir == LF_ID_FWD) k_id_fwd<R, K, W><<<blocks, groups * NT, smem, st>>>(model_of<R>(v), B, state, next_vel, tau, saved, words, wi);
+  else k_id_bwd<R, K, W><<<blocks, groups * NT, smem, st>>>(model_of<R>(v), B, state, saved, gtau, gstate, gnext, gI, words, wi);
   g_launches++;
   NB2_CUDA(cudaGetLastError());
   return NB2_OK;
@@ -1353,21 +1372,24 @@ static int launch_id(nb2_model* m, int B, int dir, const R* state, const R* next
   int rc = pick_variant<R>(m, B, dir, &pv);
   if (rc) return rc;
   return with_lanes(pv->mf.lanes, [&](auto k) {
-    return launch_id_k<R, decltype(k)::value>(*pv, m->sm_count, B, dir, state, next_vel, tau, saved, gtau, gstate, gnext, gI, wi, st);
+    constexpr int K = decltype(k)::value;
+    return with_width<K>(pv->shape[dir][sizeof(R) == 8], [&](auto w) {
+      return launch_id_kw<R, K, decltype(w)::value>(*pv, m->sm_count, B, dir, state, next_vel, tau, saved, gtau, gstate, gnext, gI, wi, st);
+    });
   });
 }
 
 // ---- forward dynamics: the same launch family, dir LF_FD_FWD (q, qdot rows qs / vs words apart) or LF_FD_BWD
-template <class R, int K>
-static int launch_fd_k(const nb2_variant& v, int sm_count, int B, int dir, const FdArgs& a, cudaStream_t st) {
-  constexpr int WPW = CoopShape<K>::WPW, ST = CoopShape<K>::ST;
+template <class R, int K, int W>
+static int launch_fd_kw(const nb2_variant& v, int sm_count, int B, int dir, const FdArgs& a, cudaStream_t st) {
+  constexpr int ST = GroupShape<K, W>::ST, NT = GroupShape<K, W>::THREADS;
   const int words = dir == LF_FD_FWD ? v.fwd_words : v.bwd_words;
-  const size_t per_warp = (size_t)words * ST * sizeof(R);
-  const int total_warps = (B + WPW - 1) / WPW;
-  const int warps = block_warps(total_warps, sm_count, v.shape[dir][sizeof(R) == 8], per_warp);
-  const int blocks = (total_warps + warps - 1) / warps;
-  const size_t smem = per_warp * warps + (size_t)body_table_words<K>(v.mf.nb) * sizeof(R);
-  nb2_fd_launch<R>(K, dir == LF_FD_BWD, blocks, warps * 32, smem, st, fd_model_of<R>(v), B, a, words);
+  const size_t per_group = (size_t)words * ST * sizeof(R);
+  const int total_groups = groups_of(B, W);
+  const int groups = block_groups<K>(total_groups, sm_count, v.shape[dir][sizeof(R) == 8], per_group);
+  const int blocks = (total_groups + groups - 1) / groups;
+  const size_t smem = per_group * groups;
+  nb2_fd_launch<R>(K, W, dir == LF_FD_BWD, blocks, groups * NT, smem, st, fd_model_of<R>(v), B, a, words);
   g_launches++;
   NB2_CUDA(cudaGetLastError());
   return NB2_OK;
@@ -1377,7 +1399,10 @@ static int launch_fd(nb2_model* m, int B, int dir, const FdArgs& a, cudaStream_t
   nb2_variant* pv = nullptr;
   int rc = pick_variant<R>(m, B, dir, &pv);
   if (rc) return rc;
-  return with_lanes(pv->mf.lanes, [&](auto k) { return launch_fd_k<R, decltype(k)::value>(*pv, m->sm_count, B, dir, a, st); });
+  return with_lanes(pv->mf.lanes, [&](auto k) {
+    constexpr int K = decltype(k)::value;
+    return with_width<K>(pv->shape[dir][sizeof(R) == 8], [&](auto w) { return launch_fd_kw<R, K, decltype(w)::value>(*pv, m->sm_count, B, dir, a, st); });
+  });
 }
 
 // ---- contact inverse dynamics: the chain of the contact body, checked (in range, under a free root), and the chain kernels' launch
@@ -1852,7 +1877,7 @@ int nb2_model_contact_capacity(const nb2_model* m) { return (m && m->has_contact
 int nb2_step_clocks_read(long long* out64, int reset) {
 #ifdef NB2_STEP_CLOCKS
   if (out64 && cudaMemcpyFromSymbol(out64, nb2_step_clk, sizeof(nb2_step_clk)) != cudaSuccess) return 0;
-  if (reset) { static const long long z[2 * NB2_CLK_WARPS * NB2_CLK_SLOTS] = {}; cudaMemcpyToSymbol(nb2_step_clk, z, sizeof(z)); }
+  if (reset) { static const long long z[2 * NB2_CLK_GROUPS * NB2_CLK_SLOTS] = {}; cudaMemcpyToSymbol(nb2_step_clk, z, sizeof(z)); }
   return 1;
 #else
   (void)out64; (void)reset; return 0;

@@ -33,7 +33,7 @@ template <class R> NB2_HD void crba_init(const Nb2ModelDev<R>& M, const R* q, co
   const MmLayout L = mm_layout(M.nb, M.ndof);
   for (int i = lane; i < M.nb; i += nl) {
     if (M.parent[i] >= 0) stXf<R, 1>(ws + L.oX + 12 * i, cid_xf(M, i, q));
-    R m; V3<R> h; S3<R> Ib; inertia_of(M, (const R*)nullptr, wi, wiB, i, &m, &h, &Ib);
+    R m; V3<R> h; S3<R> Ib; inertia_of(M, wi, wiB, i, &m, &h, &Ib);
     stSI<R, 1, false>(ws + L.oI + 21 * i, rigidSI(m, h, Ib));
   }
   mm_zero(ws + L.oMat, M.ndof * M.ndof, lane, nl);
@@ -99,7 +99,7 @@ template <class R> NB2_HD void minv_articulated(const Nb2ModelDev<R>& M, R* ws, 
   if (lane != 0) return;
   const MinvLayout L = minv_layout(M.nb, M.ndof, M.nslots, M.nfree, nl);
   fwd_pass1<R, 1>(M, ws + L.oScr, 0, M.nb);
-  fwd_pass2<R, 1>(M, ws + L.oScr, nullptr, 0, false, 0, M.nb, nullptr, ws + L.oIinv, wi, wiB);
+  fwd_pass2<R, 1>(M, ws + L.oScr, nullptr, 0, false, 0, M.nb, ws + L.oIinv, wi, wiB);
 }
 // stage 2, lanes over columns: column d of M^-1 (rows >= d written, mirrored)
 template <class R> NB2_HD void minv_columns(const Nb2ModelDev<R>& M, R* ws, int lane, int nl) {
@@ -124,7 +124,7 @@ template <class R> NB2_HD void minv_columns(const Nb2ModelDev<R>& M, R* ws, int 
     }
     int r = b;
     for (int i = b; M.parent[i] >= 0;) {
-      const V6<R> pA = dAdInvT(body_xf_fwd<R, 1>(M, nullptr, i, scr, F), beta);
+      const V6<R> pA = dAdInvT(body_xf_fwd<R, 1>(M, i, scr, F), beta);
       i = M.parent[i]; r = i;
       const int jt = M.jtype[i], o = M.dof_off[i];
       if (jt == NB2_JT_FREE) {
@@ -140,7 +140,7 @@ template <class R> NB2_HD void minv_columns(const Nb2ModelDev<R>& M, R* ws, int 
     // root -> leaf over the tree: qdd and the accelerations
     for (int i = r; i < M.nb && (i == r || M.parent[i] >= 0); i++) {
       const int jt = M.jtype[i], o = M.dof_off[i], p = M.parent[i];
-      const V6<R> Ap = (p >= 0) ? AdInvT(body_xf_fwd<R, 1>(M, nullptr, i, scr, F), ldv6(A + 6 * p)) : zero6<R>();
+      const V6<R> Ap = (p >= 0) ? AdInvT(body_xf_fwd<R, 1>(M, i, scr, F), ldv6(A + 6 * p)) : zero6<R>();
       V6<R> Ai;
       if (jt == NB2_JT_FREE) {
         const V6<R> y = mul(ldSI<R, 1>(ws + L.oIinv + 21 * M.free_idx[i]), ldv6(u + o));
@@ -225,7 +225,7 @@ template <class R> NB2_HD void mmb_body_forces(const Nb2ModelDev<R>& M, R* ws, i
   const MmbLayout L = mmb_layout(M.nb, M.ndof, nl);
   const int n = M.ndof;
   const int16_t* ch; const int D = mmb_chain(M, ws, b, nl, &ch);
-  R m; V3<R> h; S3<R> Ib; inertia_of(M, (const R*)nullptr, wi, wiB, b, &m, &h, &Ib);
+  R m; V3<R> h; S3<R> Ib; inertia_of(M, wi, wiB, b, &m, &h, &Ib);
   R acc[10];
   for (int k = 0; k < 10; k++) acc[k] = R(0);
   for (int t = lane; t < D; t += nl) {

@@ -45,7 +45,7 @@ template <class R> NB2_HD void reg_poses(const Nb2ModelDev<R>& M, R* ws, int lan
   const FwdLayout F = fwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
   for (int i = 0; i < M.nb; i++) {
     const int p = M.parent[i];
-    const Xf<R> T = body_xf_fwd<R, 1>(M, nullptr, i, ws, F);
+    const Xf<R> T = body_xf_fwd<R, 1>(M, i, ws, F);
     stXf<R, 1>(ws + L.oX + 12 * i, p >= 0 ? jac_mul(ldXf<R, 1>(ws + L.oX + 12 * p), T) : T);
   }
 }

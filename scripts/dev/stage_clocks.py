@@ -3,10 +3,10 @@
     nvcc <the flags of __graft_entry__.NVCC_FLAGS> -DNB2_STEP_CLOCKS -o build/clk/libnb2.so nimblephysics_b200/csrc/nb2_kernels.cu nimblephysics_b200/csrc/nb2_fd.cu
     NB2_LIB=build/clk/libnb2.so python scripts/dev/stage_clocks.py [--batch 4096] [--lanes 4 1] [--reps 20]
 
-Thread 0 of a few warps spread over the grid records clock64() at kernel entry, after the wait for the previous kernel
-(griddepcontrol.wait), after the body-table / input staging and after every stage with its barrier (nb2_kernels.cu, NB2_CLK).
-The backward of a rep is launched right behind its forward, so its wait covers the forward's tail.  Thread 0 is lane 0 of the
-group's first world: the lane that sweeps the trunk.  For every stage the table gives the median over the sampled warps and
+Thread 0 of a few groups spread over the grid records clock64() at kernel entry, after the wait for the previous kernel
+(griddepcontrol.wait), after the input staging and after every stage with its barrier (nb2_kernels.cu, NB2_CLK).
+The backward of a rep is launched right behind its forward, so its wait covers the forward's tail.  Thread 0 of a group is in
+its warp 0, lane 0 of the schedule: the lane that sweeps the trunk.  For every stage the table gives the median over the sampled groups and
 launches, and for the body sweeps the number of bodies lane 0 walks in it and the cycles per body.  Cycles are SM clocks; the
 instrumented build adds a few instructions per stage, so compare stages with each other, not with the default build's kernel
 times.
@@ -26,7 +26,7 @@ from nimblephysics_b200 import _cabi
 from nimblephysics_b200.engine import FP32
 from bench import make_inputs
 
-WARPS, SLOTS = 8, 16
+GROUPS, SLOTS = 8, 16
 # stage names and which body set lane 0 sweeps in it ("trunk", "limb" or None): world_forward_stage / world_backward_stage
 FWD = [("load q, v, tau", None), ("kinematics trunk", "trunk"), ("kinematics limbs", "limb"), ("inertias limbs", "limb"),
        ("inertias trunk", "trunk"), ("accelerations trunk", "trunk"), ("accelerations limbs", "limb"), ("store q+, v+", None)]
@@ -46,7 +46,7 @@ def main():
     args = ap.parse_args()
     assert torch.cuda.is_available(), "stage_clocks.py needs a GPU"
     L = _cabi.lib()
-    buf = (ctypes.c_longlong * (2 * WARPS * SLOTS))()
+    buf = (ctypes.c_longlong * (2 * GROUPS * SLOTS))()
     if not hasattr(L, "nb2_step_clocks_read") or not L.nb2_step_clocks_read(buf, 1):
         sys.exit("stage_clocks.py needs a library built with -DNB2_STEP_CLOCKS (set NB2_LIB to it)")
     raw = nb.RawModel.load(os.path.join(ROOT, "tests", "golden", "models", "atlas.json"))
@@ -56,7 +56,7 @@ def main():
     nxt, gs, ga = torch.empty((B, 2 * n), device="cuda"), torch.empty((B, 2 * n), device="cuda"), torch.empty((B, na), device="cuda")
     saved = torch.empty((dm.saved_words, B), device="cuda")
     stream = torch.cuda.current_stream().cuda_stream
-    print(f"{torch.cuda.get_device_name()}  Atlas fp32, B = {B}; cycles = median over {args.reps} launches x up to {WARPS} sampled warps")
+    print(f"{torch.cuda.get_device_name()}  Atlas fp32, B = {B}; cycles = median over {args.reps} launches x up to {GROUPS} sampled groups")
     for K in args.lanes:
         dm.set_lanes(K)
         assert dm.lanes_for(B, False, FP32) == K and dm.lanes_for(B, True, FP32) == K, f"no {K}-lane schedule"
@@ -71,9 +71,9 @@ def main():
             L.nb2_step_clocks_read(buf, 0)
             if rep < 3:  # warm-up launches
                 continue
-            c = np.frombuffer(buf, dtype=np.int64).reshape(2, WARPS, SLOTS)
+            c = np.frombuffer(buf, dtype=np.int64).reshape(2, GROUPS, SLOTS)
             for d, stages in ((0, FWD), (1, BWD)):
-                for w in range(WARPS):
+                for w in range(GROUPS):
                     t = c[d, w, :len(stages) + 3]
                     if t[0] and np.all(t[1:] >= t[:-1]):
                         runs[d].append(np.diff(t))
@@ -85,7 +85,7 @@ def main():
             med = np.median(np.stack(runs[d]), axis=0)
             print(f"{kname} ({len(runs[d])} samples)   {'stage':<22}{'cycles':>9}{'bodies':>8}{'per body':>10}")
             print(f"{'':<24}{'entry: wait for previous kernel':<33}{med[0]:>9.0f}")
-            print(f"{'':<24}{'entry: body table + input staging':<33}{med[1]:>9.0f}")
+            print(f"{'':<24}{'entry: input staging':<33}{med[1]:>9.0f}")
             groups = {"fixed": med[1], "trunk": 0.0, "limb": 0.0}
             for k, (name, part) in enumerate(stages):
                 cyc = med[2 + k]
