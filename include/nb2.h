@@ -418,6 +418,25 @@ int nb2_constrained_forward_dynamics_jacobians(const nb2_model* m, int B, const 
                                                 double damping, const double* world_inertia, void* accel, void* wrenches, void* J_q, void* J_qdot,
                                                 void* J_tau, void* W_q, void* W_qdot, void* W_tau, int precision, void* stream);
 
+/* Impulse dynamics (DESIGN.md §6q): the impact map of worlds whose k contact points strike and are held from then on.  Contacts, offsets,
+ * point_contacts, damping and world_inertia as nb2_constrained_forward_dynamics, with J [m, ndof] the stack of the points' rows.  With
+ * state [B, 2 ndof] = [q ; qdot-], e = restitution in [0, 1] and rho = damping,
+ *     M (qdot+ - qdot-) = J^T Lam ,    J qdot+ = -e J qdot- - rho Lam ,
+ * vel_after [B, ndof] = qdot+ (the step's velocity coordinates); impulses [B, k, 6] = [Lam_a + p_i x Lam_l ; Lam_l] (Lam_i = [angular
+ * impulse about p_i ; linear impulse], world axes, N s: about the world origin) or, with point_contacts, [B, k, 3] = Lam_l.  Gravity, joint
+ * springs and damping, limits, contacts of the model and the LCP cache play no part.  A world whose J M^-1 J^T + rho I has a Cholesky
+ * pivot at or below 64 eps max(diagonal) gets NaN rows.  The backward recomputes the forward and writes grad_state [B, 2 ndof],
+ * grad_offsets [B, k, 3] (or NULL) and grad_inertia ([10 nb, B] fp64, or NULL).  One warp per world; stateless, nothing allocated, B = 0
+ * only validates.  NB2_ERR_INVALID as nb2_constrained_forward_dynamics and for a restitution outside [0, 1]; NB2_ERR_UNSUPPORTED when the
+ * working set does not fit shared memory. */
+int nb2_impulse_dynamics(const nb2_model* m, int B, const void* state, int k, const int32_t* body, const double* T_owner_from_node,
+                         const void* offsets, int offsets_per_world, int point_contacts, double restitution, double damping,
+                         const double* world_inertia, void* vel_after, void* impulses, int precision, void* stream);
+int nb2_impulse_dynamics_backward(const nb2_model* m, int B, const void* state, int k, const int32_t* body, const double* T_owner_from_node,
+                                  const void* offsets, int offsets_per_world, int point_contacts, double restitution, double damping,
+                                  const double* world_inertia, const void* grad_vel, const void* grad_impulses, void* grad_state,
+                                  void* grad_offsets, double* grad_inertia, int precision, void* stream);
+
 /* Batched boxed-LCP solves on the device: B independent problems, one warp each — the reference's pointer-style lower boundary
  * BoxedLcpSolver::solve(n, A, x, b, nub, lo, hi, findex, earlyTermination) (dart/constraint/BoxedLcpSolver.hpp:125-135) and the
  * solve chain of BoxedLcpConstraintSolver::solveLcp (BoxedLcpConstraintSolver.cpp:352-789).  Device pointers; problem w has dimension

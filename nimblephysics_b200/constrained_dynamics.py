@@ -26,8 +26,14 @@ problem regular: it picks the solution with the least wrench norm in the limit.
 ``constrained_forward_dynamics_jacobians`` returns qdd, the wrenches and their dense Jacobians in state and tau in one launch, for iLQR /
 DDP, linearised MPC and contact-force constraints that need the matrices rather than products with one gradient.
 
-The reference simulator has no counterpart: it resolves contact only through its LCP step.  The work is done by libnb2.so (include/nb2.h
-``nb2_constrained_forward_dynamics``, its backward and ``nb2_constrained_forward_dynamics_jacobians``), one warp per world.
+``impulse_dynamics`` is the impact map at a phase switch of the same contact description: when the points strike, the pre-impact velocity
+qdot- jumps to a qdot+ that satisfies the new constraints, with restitution e in [0, 1]:
+
+    M (qdot+ - qdot-) = J^T Lam ,     J qdot+ = -e J qdot- - rho Lam .
+
+The reference simulator has no counterpart: it resolves contact and impacts only through its LCP step.  The work is done by libnb2.so
+(include/nb2.h ``nb2_constrained_forward_dynamics``, its backward, ``nb2_constrained_forward_dynamics_jacobians`` and
+``nb2_impulse_dynamics`` with its backward), one warp per world.
 """
 from __future__ import annotations
 
@@ -38,18 +44,27 @@ import torch
 
 from .engine import FP32, FP64, device_model_for
 from .inverse_dynamics import MAX_CONTACT_BODIES, _backward_buffers, _check_fd, _input_grads, _prepare, _ptr
-from .timestep import _word_major_inertia, per_world_inertia, set_shared_masses
+from .timestep import _inertia_grad, _word_major_inertia, per_world_inertia, set_shared_masses, shared_mass_jacobian
 from .world_jacobian import _body_index, resolve_nodes
 
 _WHO = "constrained_forward_dynamics()"
 _WHO_J = "constrained_forward_dynamics_jacobians()"
+_WHO_I = "impulse_dynamics()"
 
 
 def _check_contacts(world, state, tau, nodes, offsets, damping, who=_WHO):
-    """ValueError before any device work for a bad contact set, offsets, damping or dtype; returns the nodes as a list."""
-    _check_fd(world, state, tau, who, "tau")
+    """ValueError before any device work for a bad contact set, offsets, damping or dtype; returns the nodes as a list.  tau None: the
+    checks of impulse_dynamics, which takes no force."""
+    if tau is None:  # impulse dynamics: the state alone
+        if world.getNumDofs() == 0:
+            raise ValueError(f"{who}: the world has no degrees of freedom")
+        n = world.getNumDofs()
+        if state.dim() not in (1, 2) or state.shape[-1] != 2 * n:
+            raise ValueError(f"{who}: state has shape {tuple(state.shape)}, expected [..., {2 * n}] (= getStateSize())")
+    else:
+        _check_fd(world, state, tau, who, "tau")
     for name, t in (("state", state), ("tau", tau)):
-        if not t.dtype.is_floating_point:
+        if t is not None and not t.dtype.is_floating_point:
             raise ValueError(f"{who}: {name} has dtype {t.dtype}, expected a floating-point tensor")
     nodes = list(nodes)
     if not 1 <= len(nodes) <= MAX_CONTACT_BODIES:
@@ -190,3 +205,100 @@ def constrained_forward_dynamics_jacobians(world, state: torch.Tensor, tau: torc
     if single:
         res = [x[0] for x in res]
     return tuple(x.to(device=state.device, dtype=state.dtype) for x in res)
+
+
+class ImpulseDynamicsLayer(torch.autograd.Function):
+    """(qdot_after, impulses) of the canonical contact bodies `bodies` with placements T12 (world_jacobian.resolve_nodes); world_inertia
+    as for InverseDynamicsLayer (exclusive with the 1-D `mass`); offsets None, [k, 3] or [B, k, 3]; point, restitution and damping as
+    impulse_dynamics.  No gradient reaches restitution or damping."""
+
+    @staticmethod
+    def forward(ctx, world, state, mass, world_inertia, offsets, bodies, T12, point, restitution, damping):
+        if mass is not None and world_inertia is not None:
+            raise ValueError(f"{_WHO_I}: give either a mass vector or a per-world inertia table, not both")
+        dm = set_shared_masses(world, mass, _WHO_I) if mass is not None else device_model_for(world)
+        if not torch.cuda.is_available():
+            raise RuntimeError(f"nimblephysics_b200.{_WHO_I[:-2]} needs a CUDA device; there is no CPU fallback")
+        ctx.single = state.dim() == 1
+        s2 = state.detach().reshape(1, -1) if ctx.single else state.detach()
+        dev = s2.device if s2.is_cuda else torch.device("cuda", torch.cuda.current_device())
+        rdt = torch.float64 if state.dtype == torch.float64 else torch.float32
+        sd = s2.to(device=dev, dtype=rdt).contiguous()
+        B, k = sd.shape[0], len(bodies)
+        if world_inertia is not None and (ctx.single or tuple(world_inertia.shape) != (B, dm.cm.nb, 10)):
+            raise ValueError(f"{_WHO_I}: per-world inertia has shape {tuple(world_inertia.shape)}, expected [{B}, {dm.cm.nb}, 10] with a 2-D state")
+        wi = _word_major_inertia(dm, world_inertia, B, dev)
+        od = None if offsets is None else offsets.detach().to(device=dev, dtype=rdt).contiguous()
+        ctx.dm, ctx.B, ctx.prec = dm, B, FP64 if rdt == torch.float64 else FP32
+        ctx.bodies, ctx.T12, ctx.point, ctx.e, ctx.damping, ctx.off_like = bodies, T12, bool(point), float(restitution), float(damping), offsets
+        ctx.state_meta = (state.device, state.dtype)
+        ctx.mass_grad = mass is not None and ctx.needs_input_grad[2]
+        if ctx.mass_grad:
+            ctx.mass_P, ctx.mass_like = shared_mass_jacobian(world, dm, dev), mass
+        ctx.wi_grad, ctx.wi_like = world_inertia is not None and ctx.needs_input_grad[3], world_inertia
+        with torch.cuda.device(dev):
+            vel = torch.empty((B, dm.ndof), dtype=rdt, device=dev)
+            imp = torch.empty((B, k, 3 if point else 6), dtype=rdt, device=dev)
+            if B > 0:  # an empty batch has no rows to hand over (its data pointers may be NULL)
+                dm.impulse_dynamics_device(B, sd.data_ptr(), bodies, T12, _ptr(od), od is not None and od.dim() == 3, ctx.point, ctx.e, ctx.damping,
+                                           vel.data_ptr(), imp.data_ptr(), torch.cuda.current_stream().cuda_stream, ctx.prec, wi_ptr=_ptr(wi))
+        if any(ctx.needs_input_grad[1:5]):
+            ctx.save_for_backward(sd, od, wi)
+        if ctx.single:
+            vel, imp = vel[0], imp[0]
+        return vel.to(device=state.device, dtype=state.dtype), imp.to(device=state.device, dtype=state.dtype)
+
+    @staticmethod
+    def backward(ctx, grad_vel, grad_impulses):
+        dm, B = ctx.dm, ctx.B
+        sd, od, wi = ctx.saved_tensors
+        dev, k = sd.device, len(ctx.bodies)
+        g = grad_vel.detach().reshape(B, dm.ndof).to(device=dev, dtype=sd.dtype).contiguous()
+        gw = grad_impulses.detach().reshape(B, k, 3 if ctx.point else 6).to(device=dev, dtype=sd.dtype).contiguous()
+        want_off = ctx.off_like is not None and ctx.needs_input_grad[4]
+        with torch.cuda.device(dev):
+            gs = torch.empty((B, 2 * dm.ndof), dtype=sd.dtype, device=dev)
+            gi = torch.empty((10 * dm.cm.nb, B), dtype=torch.float64, device=dev) if (ctx.mass_grad or ctx.wi_grad) else None
+            go = torch.empty((B, k, 3), dtype=sd.dtype, device=dev) if want_off else None
+            if B > 0:
+                dm.impulse_dynamics_backward_device(B, sd.data_ptr(), ctx.bodies, ctx.T12, _ptr(od), od is not None and od.dim() == 3, ctx.point,
+                                                    ctx.e, ctx.damping, g.data_ptr(), gw.data_ptr(), gs.data_ptr(), _ptr(go),
+                                                    torch.cuda.current_stream().cuda_stream, ctx.prec, ginertia_ptr=_ptr(gi), wi_ptr=_ptr(wi))
+            elif gi is not None:
+                gi.zero_()
+        gm = (ctx.mass_P @ gi.sum(dim=1)).to(device=ctx.mass_like.device, dtype=ctx.mass_like.dtype) if ctx.mass_grad else None
+        gwi = _inertia_grad(gi, ctx.wi_like) if ctx.wi_grad else None
+        if want_off:
+            if ctx.off_like.dim() == 2:  # offsets shared by the batch: the worlds' gradients add up
+                go = go.sum(dim=0)
+            go = go.to(device=ctx.off_like.device, dtype=ctx.off_like.dtype)
+        gs = gs[0] if ctx.single else gs
+        return None, gs.to(device=ctx.state_meta[0], dtype=ctx.state_meta[1]), gm, gwi, go, None, None, None, None, None
+
+
+def impulse_dynamics(world, state: torch.Tensor, contact_nodes: Sequence, offsets: Optional[torch.Tensor] = None, point_contacts: bool = False,
+                     restitution: float = 0.0, damping: float = 0.0, mass: Optional[torch.Tensor] = None):
+    """(qdot_after, impulses): the post-impact velocities [B, n] and contact impulses [B, k, 6] ([B, k, 3] with point_contacts; [n] and
+    [k, 6] / [k, 3] for a 1-D state) of every world at `state` [B, 2n] = [q ; qdot-] when the k `contact_nodes` strike and are held, with
+    restitution e = `restitution` and damping rho = `damping`:
+
+        Lam = -(J M^-1 J^T + rho I)^-1 (1 + e) J qdot- ,   qdot_after = qdot- + M^-1 J^T Lam .
+
+    Lam_i is [angular impulse about p_i ; linear impulse] in world axes, in N s; a 6-D contact returns it about the world origin,
+    [Lam_a + p_i x Lam_l ; Lam_l], a point contact Lam_l (the wrench convention of constrained_forward_dynamics).  The impact is
+    instantaneous: gravity, joint springs and damping, limits, the world's own contacts and the LCP cache play no part.  With rho = 0,
+    e = 1 keeps the kinetic energy and e < 1 loses (1 - e^2) / 2 (J qdot-)^T (J M^-1 J^T)^-1 (J qdot-); at e = 0 a second impact changes
+    nothing.  Velocities are in the step's coordinates (free joints use the body twist).
+
+    contact_nodes, offsets, point_contacts, damping and mass as constrained_forward_dynamics; restitution: a Python number in [0, 1].
+    Precision follows state.dtype.  Gradients of both outputs reach state (both halves), offsets and mass; none reach restitution or
+    damping.  A singular contact set gives NaN rows in that world only, as in constrained_forward_dynamics.  ValueError before any device
+    work for a bad contact set, shape, dtype, damping or restitution."""
+    nodes = _check_contacts(world, state, None, contact_nodes, offsets, damping, _WHO_I)
+    if isinstance(restitution, (torch.Tensor, bool)) or not isinstance(restitution, (int, float)) or not math.isfinite(restitution) \
+            or not 0.0 <= restitution <= 1.0:
+        raise ValueError(f"{_WHO_I}: restitution must be a finite float in [0, 1], got {restitution!r}")
+    wi = per_world_inertia(world, state, mass, _WHO_I) if mass is not None and mass.dim() == 2 else None
+    bodies, T12 = _resolve(world, nodes, _WHO_I)
+    return ImpulseDynamicsLayer.apply(world, state, None if wi is not None else mass, wi, offsets, bodies, T12, point_contacts,
+                                      float(restitution), float(damping))

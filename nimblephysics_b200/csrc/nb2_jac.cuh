@@ -138,8 +138,11 @@ template <class R> NB2_HD void jpb_terms(const Nb2ModelDev<R>& M, int b, const R
     put6(ws + L.oRU + 6 * t, ru);
   }
 }
-// node stage c, lane 0: leaf -> root over the chain's joints, the joints' position gradients; the offset gradient (go: [3] or nullptr)
-template <class R> NB2_HD void jpb_reduce(const Nb2ModelDev<R>& M, const R* q, int b, R* ws, R* go, int lane) {
+// node stage c, lane 0: leaf -> root over the chain's joints, the joints' position gradients; the offset gradient (go: [3] or nullptr).
+// PE: the loss also depends on the point itself, with adjoint pe [3]; the point moves with every joint of the chain, so pe joins the
+// column term P of every joint and the offset gradient.
+template <class R, bool PE = false>
+NB2_HD void jpb_reduce(const Nb2ModelDev<R>& M, const R* q, int b, R* ws, R* go, int lane, const R* pe = nullptr) {
   if (lane != 0) return;
   const JpbLayout L = jpb_layout(M.nb, M.ndof);
   const int D = jpb_chain_len(M, b);
@@ -147,6 +150,7 @@ template <class R> NB2_HD void jpb_reduce(const Nb2ModelDev<R>& M, const R* q, i
   R* gq = ws + L.oGq;
   V3<R> Ptot = zero3<R>();
   for (int t = 0; t < D; t++) Ptot = Ptot + ldv6(ws + L.oRU + 6 * t).l;
+  if (PE) Ptot = Ptot + mk3<R>(pe[0], pe[1], pe[2]);
   if (go) {
     const V3<R> v = b >= 0 ? mulT(ldXf<R, 1>(ws + L.oRe).R_, Ptot) : zero3<R>();
     go[0] = v.x; go[1] = v.y; go[2] = v.z;

@@ -29,6 +29,7 @@
 #include "nb2_fd.h"
 #include "nb2_reg.h"
 #include "nb2_cfd.h"
+#include "nb2_imp.h"
 
 static thread_local std::string g_err;
 static std::atomic<long long> g_launches{0};
@@ -2483,9 +2484,8 @@ int nb2_energy_regressor(const nb2_model* m, int B, const void* state, void* Y_k
 // ---- constrained forward dynamics (nb2_cfd.cu; its dense Jacobians nb2_cfdj.cu): one warp per world, one world per block, the create-time
 // schedule's FD model, as many row slots as shared memory leaves room for.  The contacts are checked here: 1..NB2_MAX_CONTACT_BODIES
 // distinct movable canonical bodies.
-static int launch_cfd(const nb2_model* m, int B, int k, const int32_t* body, const double* T, int point, double damping, CfdArgs a, int precision,
-                      void* stream, const char* who) {
-  if (!m || B < 0 || (B > 0 && (!a.state || !a.tau))) { g_err = std::string(who) + ": bad argument"; return NB2_ERR_INVALID; }
+// NB2_OK, or NB2_ERR_INVALID for a model without dofs, a bad contact set or a bad damping
+static int contacts_ok(const nb2_model* m, int k, const int32_t* body, const double* T, double damping, const char* who) {
   if (m->mf.ndof == 0) { g_err = std::string(who) + ": the model has no dofs"; return NB2_ERR_INVALID; }
   if (k < 1 || k > NB2_MAX_CONTACT_BODIES || !body || !T) {
     g_err = std::string(who) + ": " + std::to_string(k) + " contacts, expected 1.." + std::to_string(NB2_MAX_CONTACT_BODIES);
@@ -2497,6 +2497,12 @@ static int launch_cfd(const nb2_model* m, int B, int k, const int32_t* body, con
       if (body[f] == body[e]) { g_err = std::string(who) + ": body " + std::to_string(body[e]) + " is held twice"; return NB2_ERR_INVALID; }
   }
   if (!(damping >= 0.0) || damping > 1.7976931348623157e308) { g_err = std::string(who) + ": damping must be finite and >= 0"; return NB2_ERR_INVALID; }
+  return NB2_OK;
+}
+static int launch_cfd(const nb2_model* m, int B, int k, const int32_t* body, const double* T, int point, double damping, CfdArgs a, int precision,
+                      void* stream, const char* who) {
+  if (!m || B < 0 || (B > 0 && (!a.state || !a.tau))) { g_err = std::string(who) + ": bad argument"; return NB2_ERR_INVALID; }
+  if (int rc = contacts_ok(m, k, body, T, damping, who)) return rc;
   if (B == 0) return NB2_OK;
   a.k = k; a.body = body; a.T = T; a.point = point ? 1 : 0; a.rho = damping;
   return with_precision(precision, [&](auto r) {
@@ -2555,6 +2561,49 @@ int nb2_constrained_forward_dynamics_jacobians(const nb2_model* m, int B, const 
   a.state = state; a.tau = tau; a.off = offsets; a.off_pw = offsets_per_world; a.wi = world_inertia; a.qdd = accel; a.wrench = wrenches;
   a.J[0] = J_q; a.J[1] = J_qdot; a.J[2] = J_tau; a.J[3] = W_q; a.J[4] = W_qdot; a.J[5] = W_tau;
   return launch_cfd(m, B, k, body, T_owner_from_node, point_contacts, damping, a, precision, stream, who);
+}
+}  // extern "C"
+
+// ---- impulse dynamics (nb2_imp.cu): the launch shape and working set of constrained forward dynamics, on the passive-free copy of the
+// create-time schedule's FD model
+static int launch_imp(const nb2_model* m, int B, int k, const int32_t* body, const double* T, int point, double restitution, double damping,
+                      ImpArgs a, int precision, void* stream, const char* who) {
+  if (!m || B < 0 || (B > 0 && !a.state)) { g_err = std::string(who) + ": bad argument"; return NB2_ERR_INVALID; }
+  if (int rc = contacts_ok(m, k, body, T, damping, who)) return rc;
+  if (!(restitution >= 0.0 && restitution <= 1.0)) { g_err = std::string(who) + ": restitution must be in [0, 1]"; return NB2_ERR_INVALID; }
+  if (B == 0) return NB2_OK;
+  a.k = k; a.body = body; a.T = T; a.point = point ? 1 : 0; a.e = restitution; a.rho = damping;
+  return with_precision(precision, [&](auto r) {
+    using R = decltype(r);
+    const Nb2ModelDev<R>& M = fd_model_of<R>(m->variants[0]);
+    size_t smem = 0;
+    const int slots = nb2_cfd_slots(M.nb, M.ndof, M.nslots, M.nfree, k * (a.point ? 3 : 6), 0, sizeof(R), kMaxSmem, &smem);
+    if (!slots) { g_err = std::string(who) + ": the model's working set does not fit in shared memory"; return NB2_ERR_UNSUPPORTED; }
+    NB2_CUDA(nb2_imp_launch<R>(a.gvel != nullptr, slots, smem, (cudaStream_t)stream, M, B, a));
+    g_launches++;
+    return NB2_OK;
+  });
+}
+extern "C" {
+int nb2_impulse_dynamics(const nb2_model* m, int B, const void* state, int k, const int32_t* body, const double* T_owner_from_node,
+                         const void* offsets, int offsets_per_world, int point_contacts, double restitution, double damping,
+                         const double* world_inertia, void* vel_after, void* impulses, int precision, void* stream) {
+  static const char* who = "nb2_impulse_dynamics";
+  if (B > 0 && (!vel_after || !impulses)) { g_err = std::string(who) + ": bad argument"; return NB2_ERR_INVALID; }
+  ImpArgs a{};
+  a.state = state; a.off = offsets; a.off_pw = offsets_per_world; a.wi = world_inertia; a.vel = vel_after; a.imp = impulses;
+  return launch_imp(m, B, k, body, T_owner_from_node, point_contacts, restitution, damping, a, precision, stream, who);
+}
+int nb2_impulse_dynamics_backward(const nb2_model* m, int B, const void* state, int k, const int32_t* body, const double* T_owner_from_node,
+                                  const void* offsets, int offsets_per_world, int point_contacts, double restitution, double damping,
+                                  const double* world_inertia, const void* grad_vel, const void* grad_impulses, void* grad_state,
+                                  void* grad_offsets, double* grad_inertia, int precision, void* stream) {
+  static const char* who = "nb2_impulse_dynamics_backward";
+  if (B > 0 && (!grad_vel || !grad_impulses || !grad_state)) { g_err = std::string(who) + ": bad argument"; return NB2_ERR_INVALID; }
+  ImpArgs a{};
+  a.state = state; a.off = offsets; a.off_pw = offsets_per_world; a.wi = world_inertia;
+  a.gvel = grad_vel; a.gimp = grad_impulses; a.gstate = grad_state; a.goff = grad_offsets; a.gI = grad_inertia;
+  return launch_imp(m, B, k, body, T_owner_from_node, point_contacts, restitution, damping, a, precision, stream, who);
 }
 int nb2_model_ndof(const nb2_model* m) { return m ? m->mf.ndof : -1; }
 int nb2_model_na(const nb2_model* m) { return m ? m->mf.na : -1; }

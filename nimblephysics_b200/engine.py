@@ -332,6 +332,24 @@ class DeviceModel:
                                                                            off_ptr, int(off_per_world), int(point), float(damping), wi_ptr, qdd_ptr,
                                                                            wrench_ptr, *jac_ptrs, precision, stream))
 
+    def impulse_dynamics_device(self, B, state_ptr, bodies, T12, off_ptr, off_per_world, point, restitution, damping, vel_ptr, imp_ptr, stream,
+                                precision=FP32, wi_ptr=None):
+        """Post-impact velocities [B, n] and contact impulses [B, k, 6 or 3] with the bodies held (include/nb2.h nb2_impulse_dynamics);
+        bodies [k] int32 and T12 [k, 12] fp64 are host arrays."""
+        b = np.ascontiguousarray(bodies, np.int32)
+        T = np.ascontiguousarray(T12, np.float64)
+        _cabi.check(_cabi.lib().nb2_impulse_dynamics(self.handle, B, state_ptr, len(b), b.ctypes.data, T.ctypes.data, off_ptr, int(off_per_world),
+                                                     int(point), float(restitution), float(damping), wi_ptr, vel_ptr, imp_ptr, precision, stream))
+
+    def impulse_dynamics_backward_device(self, B, state_ptr, bodies, T12, off_ptr, off_per_world, point, restitution, damping, gvel_ptr,
+                                         gimp_ptr, gstate_ptr, goff_ptr, stream, precision=FP32, ginertia_ptr=None, wi_ptr=None):
+        """VJP of impulse_dynamics_device; goff_ptr: optional [B, k, 3], ginertia_ptr: optional [10*nb, B] float64."""
+        b = np.ascontiguousarray(bodies, np.int32)
+        T = np.ascontiguousarray(T12, np.float64)
+        _cabi.check(_cabi.lib().nb2_impulse_dynamics_backward(self.handle, B, state_ptr, len(b), b.ctypes.data, T.ctypes.data, off_ptr,
+                                                              int(off_per_world), int(point), float(restitution), float(damping), wi_ptr,
+                                                              gvel_ptr, gimp_ptr, gstate_ptr, goff_ptr, ginertia_ptr, precision, stream))
+
     def contact_workspace_bytes(self, B):
         return int(_cabi.lib().nb2_contact_workspace_bytes(self.handle, B))
 

@@ -1,7 +1,7 @@
 """Small end-to-end run for compute-sanitizer (memcheck): contact-free fwd+bwd (device + pinned-host paths, partial groups),
 contact fwd+bwd, fused rollout, inverse dynamics, contact and multiple-contact inverse dynamics fwd+bwd, the mass matrix and its inverse fwd+bwd, the world and COM Jacobians
 and their time derivatives fwd+bwd, forward dynamics fwd+bwd, the pointer-style forward dynamics and the dense Jacobians of inverse and
-forward dynamics, the inverse-dynamics and energy regressors, constrained forward dynamics fwd+bwd and its dense Jacobians (both precisions, per-world masses and offsets, partial groups and partial blocks)."""
+forward dynamics, the inverse-dynamics and energy regressors, constrained forward dynamics fwd+bwd and its dense Jacobians, impulse dynamics fwd+bwd (both precisions, per-world masses and offsets, partial groups and partial blocks)."""
 import sys
 import numpy as np, torch
 sys.path.insert(0, ".")
@@ -62,6 +62,10 @@ for B in (7, 203):
         (q2.sum() + w2.sum()).backward()
         nb.constrained_forward_dynamics_jacobians(mw, st, tau, bodies, off, mass=mass.detach() * torch.tensor(mw.getMasses(), device="cuda"))
         nb.constrained_forward_dynamics_jacobians(mw, st, tau, bodies[:2], point_contacts=True, damping=1e-3)
+        v2, i2 = nb.impulse_dynamics(mw, st, bodies, off, restitution=0.5, mass=mass * torch.tensor(mw.getMasses(), device="cuda"))
+        (v2.sum() + i2.sum()).backward()
+        v2, i2 = nb.impulse_dynamics(mw, st, bodies, point_contacts=True, restitution=1.0, damping=1e-3)
+        (v2.sum() + i2.sum()).backward()
     sd = torch.tensor(s, device="cuda", dtype=torch.float64)
     nb.device_model_for(w).forward_dynamics(sd[:, :raw.ndof], sd[:, raw.ndof:], sd[:, raw.ndof:] * 10)
 torch.cuda.synchronize()
