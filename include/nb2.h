@@ -436,6 +436,21 @@ int nb2_impulse_dynamics_backward(const nb2_model* m, int B, const void* state, 
                                   const void* offsets, int offsets_per_world, int point_contacts, double restitution, double damping,
                                   const double* world_inertia, const void* grad_vel, const void* grad_impulses, void* grad_state,
                                   void* grad_offsets, double* grad_inertia, int precision, void* stream);
+/* Dense Jacobians of impulse dynamics (DESIGN.md §6r), in one launch.  Arguments as nb2_impulse_dynamics, whose vel_after [B, ndof] and
+ * impulses [B, k, r] (r = 6, or 3 with point_contacts) it also writes, with m = k r and
+ *     V_q, V_qdot [B, ndof, ndof] :  V_x[w, i, j] = d vel_after[w, i] / d x[w, j] ,
+ *     I_q, I_qdot [B, m, ndof]    :  I_x[w, i r + c, j] = d impulses[w, i, c] / d x[w, j] ,
+ * x = the positions or the pre-impact velocities (the two halves of state).  Row i of each block is nb2_impulse_dynamics_backward with
+ * the seed e_i on that output, so free joints follow its conventions (position columns for the six stored coordinates, body-twist
+ * velocity columns) and the blocks equal the VJP's rows up to rounding.  vel_after and the impulses are written by the forward of
+ * nb2_impulse_dynamics itself (a second launch on the stream), so they equal its outputs bit for bit.  Offsets, masses, restitution and
+ * damping are held fixed.  A singular world gets NaN in its outputs and every block.  Stateless, stream-ordered, nothing allocated, B = 0
+ * only validates.  NB2_ERR_INVALID as nb2_impulse_dynamics; NB2_ERR_UNSUPPORTED when the working set does not fit shared memory even at
+ * one row slot. */
+int nb2_impulse_dynamics_jacobians(const nb2_model* m, int B, const void* state, int k, const int32_t* body, const double* T_owner_from_node,
+                                   const void* offsets, int offsets_per_world, int point_contacts, double restitution, double damping,
+                                   const double* world_inertia, void* vel_after, void* impulses, void* V_q, void* V_qdot, void* I_q,
+                                   void* I_qdot, int precision, void* stream);
 
 /* Batched boxed-LCP solves on the device: B independent problems, one warp each — the reference's pointer-style lower boundary
  * BoxedLcpSolver::solve(n, A, x, b, nub, lo, hi, findex, earlyTermination) (dart/constraint/BoxedLcpSolver.hpp:125-135) and the

@@ -218,6 +218,8 @@ def lib() -> ctypes.CDLL:
                                             ctypes.c_double] + [vp] * 3 + [ctypes.c_int, vp])
         L.nb2_impulse_dynamics_backward.argtypes = ([vp, ctypes.c_int, vp, ctypes.c_int, vp, vp, vp, ctypes.c_int, ctypes.c_int,
                                                      ctypes.c_double, ctypes.c_double] + [vp] * 6 + [ctypes.c_int, vp])
+        L.nb2_impulse_dynamics_jacobians.argtypes = ([vp, ctypes.c_int, vp, ctypes.c_int, vp, vp, vp, ctypes.c_int, ctypes.c_int,
+                                                      ctypes.c_double, ctypes.c_double] + [vp] * 7 + [ctypes.c_int, vp])
         L.nb2_lcp_solve_batch.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double] + [vp] * 11
         L.nb2_model_set_contact_capacity.argtypes = [vp, ctypes.c_int]
         L.nb2_model_contact_capacity.argtypes = [vp]

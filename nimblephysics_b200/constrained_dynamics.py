@@ -31,9 +31,12 @@ qdot- jumps to a qdot+ that satisfies the new constraints, with restitution e in
 
     M (qdot+ - qdot-) = J^T Lam ,     J qdot+ = -e J qdot- - rho Lam .
 
+``impulse_dynamics_jacobians`` returns qdot+, the impulses and their dense Jacobians in q and qdot- in one launch: the linearisation of the
+reset map at a touchdown, for hybrid iLQR / DDP and trajectory optimisers.
+
 The reference simulator has no counterpart: it resolves contact and impacts only through its LCP step.  The work is done by libnb2.so
 (include/nb2.h ``nb2_constrained_forward_dynamics``, its backward, ``nb2_constrained_forward_dynamics_jacobians`` and
-``nb2_impulse_dynamics`` with its backward), one warp per world.
+``nb2_impulse_dynamics`` with its backward and ``nb2_impulse_dynamics_jacobians``), one warp per world.
 """
 from __future__ import annotations
 
@@ -50,6 +53,7 @@ from .world_jacobian import _body_index, resolve_nodes
 _WHO = "constrained_forward_dynamics()"
 _WHO_J = "constrained_forward_dynamics_jacobians()"
 _WHO_I = "impulse_dynamics()"
+_WHO_IJ = "impulse_dynamics_jacobians()"
 
 
 def _check_contacts(world, state, tau, nodes, offsets, damping, who=_WHO):
@@ -88,6 +92,12 @@ def _check_contacts(world, state, tau, nodes, offsets, damping, who=_WHO):
     if isinstance(damping, torch.Tensor) or not isinstance(damping, (int, float)) or not math.isfinite(damping) or damping < 0:
         raise ValueError(f"{who}: damping must be a finite float >= 0, got {damping!r}")
     return nodes
+
+
+def _check_restitution(restitution, who):
+    if isinstance(restitution, (torch.Tensor, bool)) or not isinstance(restitution, (int, float)) or not math.isfinite(restitution) \
+            or not 0.0 <= restitution <= 1.0:
+        raise ValueError(f"{who}: restitution must be a finite float in [0, 1], got {restitution!r}")
 
 
 def _resolve(world, nodes, who=_WHO):
@@ -295,10 +305,60 @@ def impulse_dynamics(world, state: torch.Tensor, contact_nodes: Sequence, offset
     damping.  A singular contact set gives NaN rows in that world only, as in constrained_forward_dynamics.  ValueError before any device
     work for a bad contact set, shape, dtype, damping or restitution."""
     nodes = _check_contacts(world, state, None, contact_nodes, offsets, damping, _WHO_I)
-    if isinstance(restitution, (torch.Tensor, bool)) or not isinstance(restitution, (int, float)) or not math.isfinite(restitution) \
-            or not 0.0 <= restitution <= 1.0:
-        raise ValueError(f"{_WHO_I}: restitution must be a finite float in [0, 1], got {restitution!r}")
+    _check_restitution(restitution, _WHO_I)
     wi = per_world_inertia(world, state, mass, _WHO_I) if mass is not None and mass.dim() == 2 else None
     bodies, T12 = _resolve(world, nodes, _WHO_I)
     return ImpulseDynamicsLayer.apply(world, state, None if wi is not None else mass, wi, offsets, bodies, T12, point_contacts,
                                       float(restitution), float(damping))
+
+
+def impulse_dynamics_jacobians(world, state: torch.Tensor, contact_nodes: Sequence, offsets: Optional[torch.Tensor] = None,
+                               point_contacts: bool = False, restitution: float = 0.0, damping: float = 0.0, mass: Optional[torch.Tensor] = None):
+    """(qdot_after, impulses, dv_dq, dv_dqdot, dimp_dq, dimp_dqdot): the outputs of impulse_dynamics for the same arguments (equal to them
+    bit for bit) and their dense Jacobians in the layout of torch.autograd.functional.jacobian, dv_dx [B, n, n] and dimp_dx [B, k, r, n]
+    (r = 6, or 3 with point_contacts), entry [w, ..., j] = d out / d x_j, x = the positions q or the pre-impact velocities qdot-.  Row i of
+    each block is impulse_dynamics's vector-Jacobian product with the seed e_i on that output, so the blocks equal autograd's Jacobian up
+    to rounding; free joints follow its conventions (position columns for the six stored coordinates, body-twist velocity columns) and
+    the impulses of 6-D contacts are about the world origin.  With A = J M^-1 J^T + rho I, e the restitution and Lam in point form (the
+    returned 6-D impulse is [Lam_a + p x Lam_l ; Lam_l]):
+
+        dv_dqdot = I - (1 + e) M^-1 J^T A^-1 J ,   dLam_dqdot = -(1 + e) A^-1 J ,
+
+    and qdot_after and Lam are linear in qdot- at fixed q (qdot_after = dv_dqdot qdot-, Lam = dLam_dqdot qdot-).  With rho = 0,
+    J dv_dqdot = -e J, and at e = 0 dv_dqdot is a projector whose product with M is symmetric.  Differentiating the constraint in q:
+    J dv_dq + d(J(q) v)/dq |_(v = qdot_after + e qdot-) = -rho dLam_dq.  For the hybrid state x = [q ; qdot], the reset map at the
+    touchdown has the Jacobian
+
+        dDelta/dx = [[I, 0], [dv_dq, dv_dqdot]] .
+
+    Arguments, shapes, masses and precision as impulse_dynamics; a 1-D state gives the same blocks without B.  The outputs carry no
+    autograd history: there are no second derivatives and no offset, mass, restitution or damping Jacobian.  A singular world gets NaN in
+    every output and block; the other worlds are unaffected.  ValueError before any device work for the argument errors of
+    impulse_dynamics."""
+    nodes = _check_contacts(world, state, None, contact_nodes, offsets, damping, _WHO_IJ)
+    _check_restitution(restitution, _WHO_IJ)
+    wi = per_world_inertia(world, state, mass, _WHO_IJ) if mass is not None and mass.dim() == 2 else None
+    bodies, T12 = _resolve(world, nodes, _WHO_IJ)
+    dm = set_shared_masses(world, mass, _WHO_IJ) if mass is not None and wi is None else device_model_for(world)
+    if not torch.cuda.is_available():
+        raise RuntimeError(f"nimblephysics_b200.{_WHO_IJ[:-2]} needs a CUDA device; there is no CPU fallback")
+    single = state.dim() == 1
+    s2 = state.detach().reshape(1, -1) if single else state.detach()
+    dev = s2.device if s2.is_cuda else torch.device("cuda", torch.cuda.current_device())
+    rdt = torch.float64 if state.dtype == torch.float64 else torch.float32
+    sd = s2.to(device=dev, dtype=rdt).contiguous()
+    od = None if offsets is None else offsets.detach().to(device=dev, dtype=rdt).contiguous()
+    B, n, k, r = sd.shape[0], dm.ndof, len(nodes), 3 if point_contacts else 6
+    with torch.cuda.device(dev):
+        vel = torch.empty((B, n), dtype=rdt, device=dev)
+        imp = torch.empty((B, k, r), dtype=rdt, device=dev)
+        J = [torch.empty((B, n, n), dtype=rdt, device=dev) for _ in range(2)] + [torch.empty((B, k, r, n), dtype=rdt, device=dev) for _ in range(2)]
+        if B > 0:  # an empty batch has no rows to hand over (its data pointers may be NULL)
+            dm.impulse_dynamics_jacobians_device(B, sd.data_ptr(), bodies, T12, _ptr(od), od is not None and od.dim() == 3, bool(point_contacts),
+                                                 float(restitution), float(damping), vel.data_ptr(), imp.data_ptr(), [x.data_ptr() for x in J],
+                                                 torch.cuda.current_stream().cuda_stream, FP64 if rdt == torch.float64 else FP32,
+                                                 wi_ptr=_ptr(_word_major_inertia(dm, wi, B, dev)))
+    res = [vel, imp] + J
+    if single:
+        res = [x[0] for x in res]
+    return tuple(x.to(device=state.device, dtype=state.dtype) for x in res)

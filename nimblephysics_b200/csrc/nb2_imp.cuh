@@ -208,4 +208,141 @@ NB2_HD void imp_world(const Nb2ModelDev<R>& M, const CfdNodes<R>& N, const ImpRo
   });
 }
 
+// ---- dense Jacobians (DESIGN.md §6r).  Row i of each block is the backward above with the seed e_i on one output: n seeds on qdot+, then
+// m on the impulses.  The forward is imp_world's own, run once; the seed-free words it leaves (J, the points, Y, the factor, Lam in the c
+// words) serve every row, and so do the saved stream of FD([q ; 0], J^T Lam) and qdot+ + e qdot-, built once after it.  Rounds of ST seeds
+// in cfdj_layout's per-slot words: mu, lambar, pbar, the seed vbar (its qddbar words), [dL/dq ; dL/dqdot-] and u.  Seed t's FD backward
+// runs in row slot t, swept by thread t over every lane of the schedule; the dL/dqdot- row needs no sweep; the point-Jacobian VJPs take
+// the seeds one after the other on the warp.  The world's blocks: dqdot+/dq, dqdot+/dqdot- [n][n] and dimp/dq, dimp/dqdot- [m][n],
+// row-major.
+template <class R> struct ImpJacRows { R* Vq; R* Vqd; R* Iq; R* Iqd; };
+
+template <class R, int ST, class Stage>
+NB2_HD void impj_world(const Nb2ModelDev<R>& M, const CfdNodes<R>& N, const ImpRows<R>& io, const ImpJacRows<R>& out, R* ws, Stage&& stage) {
+  const int n = M.ndof, k = N.k, rpc = N.point ? 3 : 6, r0c = N.point ? 3 : 0, m = k * rpc, rows = n + m;
+  const CfdjLayout X = cfdj_layout(M.nb, M.ndof, M.nslots, M.nfree, m, ST);
+  const CfdLayout& L = X.C;
+  const BwdLayout BL = bwd_layout(M.nb, M.ndof, M.nslots, M.nfree);
+  const R* s = io.state;
+  const R* qd = s + n;
+  const R ep1 = R(1) + io.e;
+  R* K = ws + L.oK;
+  R* gb = ws + L.oGb;  // the row [q ; 0] until the first seed's point-Jacobian VJP
+  imp_world<R, ST, false>(M, N, io, ws, stage);  // qdot+ and the impulses written
+  // ---- seed-free: the saved stream of FD([q ; 0], J^T Lam) (read before the seed block overwrites the row), then qdot+ + e qdot- in the
+  // tau words
+  stage([&](int lane, int nl) {
+    for (int d = lane; d < n; d += nl) {
+      R t = R(0);
+      for (int r = 0; r < m; r++) t += ws[L.oJ + r * n + d] * ws[L.oC + r];
+      ws[L.oTau + d] = t;
+    }
+  });
+  stage([&](int lane, int nl) { dj_load<R>(M, ws, gb, ws + L.oTau, lane, nl); });
+  cfd_fd_forward<R>(M, ws, io.wi, io.wiB, stage);
+  stage([&](int lane, int nl) {
+    for (int d = lane; d < n; d += nl) {
+      R v = qd[d];
+      for (int r = 0; r < m; r++) v += ws[L.oY + r * n + d] * ws[L.oC + r];
+      ws[L.oTau + d] = v + io.e * qd[d];
+    }
+  });
+  for (int s0 = 0; s0 < rows; s0 += ST) {
+    const int ns = (rows - s0 < ST) ? rows - s0 : ST;
+    // the seeds: e_row on qdot+ (row < n) or on the impulse entry row - n; then in point form, in place
+    stage([&](int lane, int nl) {
+      for (int idx = lane; idx < ns * rows; idx += nl) {
+        const int t = idx / rows, e = idx - t * rows;
+        if (e < n) ws[X.oQb + t * n + e] = (s0 + t == e) ? R(1) : R(0);
+        else ws[X.oLb + t * m + e - n] = (s0 + t == e) ? R(1) : R(0);
+      }
+    });
+    stage([&](int lane, int nl) {
+      for (int idx = lane; idx < ns * k; idx += nl) {
+        const int t = idx / k, i = idx - t * k;
+        R* lb = ws + X.oLb + t * m + i * rpc;
+        cfd_point_form<R>(N, L, ws, i, lb, lb, ws + X.oPb + 12 * t + 3 * i);
+      }
+    });
+    // mu = (J M^-1 J^T + rho I)^-1 (lambar + Y vbar), slot t on lane t
+    stage([&](int lane, int nl) {
+      for (int idx = lane; idx < ns * m; idx += nl) {
+        const int t = idx / m, r = idx - t * m;
+        R v = ws[X.oLb + t * m + r];
+        for (int d = 0; d < n; d++) v += ws[L.oY + r * n + d] * ws[X.oQb + t * n + d];
+        ws[X.oMu + t * m + r] = v;
+      }
+    });
+    stage([&](int lane, int) { if (lane < ns && ws[L.oFlag] == R(0)) cfd_solve<R>(ws + L.oA, m, ws + X.oMu + lane * m); });
+    // g = vbar - J^T mu into row slot t at [q ; 0] (the state words from s and 0: the row may be overwritten), and the dL/dqdot- row
+    stage([&](int lane, int nl) {
+      for (int idx = lane; idx < ns * n; idx += nl) {
+        const int t = idx / n, d = idx - t * n;
+        R* rb = ws + L.D.oB + t;
+        R jm = R(0);
+        for (int r = 0; r < m; r++) jm += ws[L.oJ + r * n + d] * ws[X.oMu + t * m + r];
+        const R vb = ws[X.oQb + t * n + d];
+        rb[(size_t)(BL.oGV + d) * ST] = vb - jm;
+        rb[(size_t)(BL.oSt + d) * ST] = s[d];
+        rb[(size_t)(BL.oSt + n + d) * ST] = R(0);
+        ws[X.oG + 2 * n * t + n + d] = vb - ep1 * jm;
+      }
+    });
+    stage([&](int lane, int) {
+      if (lane >= ns) return;
+      R* rb = ws + L.D.oB + lane;
+      for (int sg = 1; sg < NB2_BWD_STAGES - 1; sg++)
+        for (int l = 0; l < M.lanes; l++) fd_backward_stage<R, ST>(M, rb, ws + L.D.oS, 1, l, sg, nullptr, io.wi, io.wiB, nullptr, 0);
+    });
+    stage([&](int lane, int nl) {
+      for (int idx = lane; idx < ns * n; idx += nl) {
+        const int t = idx / n, d = idx - t * n;
+        const R* rb = ws + L.D.oB + t;
+        ws[X.oG + 2 * n * t + d] = rb[(size_t)(BL.oQb + d) * ST];
+        ws[X.oU + n * t + d] = rb[(size_t)(BL.oLam + d) * ST];
+      }
+    });
+    // seed by seed, the point-Jacobian VJP: J with Lam u^T - mu (qdot+ + e qdot-)^T, the points with pbar
+    for (int t = 0; t < ns; t++) {
+      const R* mu = ws + X.oMu + t * m;
+      const R* u = ws + X.oU + n * t;
+      stage([&](int lane, int nl) { jpb_init<R>(M, K, lane, nl); });
+      for (int i = 0; i < k; i++) {
+        const int b = N.body[i];
+        const R* o = io.off ? io.off + 3 * i : nullptr;
+        stage([&](int lane, int nl) {
+          for (int idx = lane; idx < 6 * n; idx += nl) {
+            const int rw = idx / n, d = idx - rw * n, j = rw - r0c;
+            R g = R(0);
+            if (j >= 0) {
+              const int r = i * rpc + j;
+              g = ws[L.oC + r] * u[d] - mu[r] * ws[L.oTau + d];
+            }
+            gb[idx] = g;
+          }
+        });
+        stage([&](int lane, int) { jpb_walk<R>(M, s, b, N.T[i], o, K, lane); });
+        stage([&](int lane, int nl) { jpb_terms<R>(M, b, gb, K, lane, nl); });
+        stage([&](int lane, int) { jpb_reduce<R, true>(M, s, b, K, ws + L.oGo + 3 * i, lane, ws + X.oPb + 12 * t + 3 * i); });
+      }
+      stage([&](int lane, int nl) {
+        R* G = ws + X.oG + 2 * n * t;
+        for (int d = lane; d < n; d += nl) G[d] = G[d] + K[jpb_layout(M.nb, n).oGq + d];
+      });
+    }
+    // the round's rows, in address order within each block
+    stage([&](int lane, int nl) {
+      const bool bad = ws[L.oFlag] != R(0);
+      for (int idx = lane; idx < ns * n; idx += nl) {
+        const int t = idx / n, j = idx - t * n, row = s0 + t;
+        const bool vel = row < n;
+        const size_t e = (size_t)(vel ? row : row - n) * n + j;
+        const R gq = ws[X.oG + 2 * n * t + j], gv = ws[X.oG + 2 * n * t + n + j];
+        (vel ? out.Vq : out.Iq)[e] = bad ? cfd_nan<R>() : gq;
+        (vel ? out.Vqd : out.Iqd)[e] = bad ? cfd_nan<R>() : gv;
+      }
+    });
+  }
+}
+
 }  // namespace nb2

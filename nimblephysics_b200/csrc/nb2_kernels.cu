@@ -2564,8 +2564,8 @@ int nb2_constrained_forward_dynamics_jacobians(const nb2_model* m, int B, const 
 }
 }  // extern "C"
 
-// ---- impulse dynamics (nb2_imp.cu): the launch shape and working set of constrained forward dynamics, on the passive-free copy of the
-// create-time schedule's FD model
+// ---- impulse dynamics (nb2_imp.cu; its dense Jacobians nb2_impj.cu): the launch shape and working set of constrained forward dynamics,
+// on the passive-free copy of the create-time schedule's FD model
 static int launch_imp(const nb2_model* m, int B, int k, const int32_t* body, const double* T, int point, double restitution, double damping,
                       ImpArgs a, int precision, void* stream, const char* who) {
   if (!m || B < 0 || (B > 0 && !a.state)) { g_err = std::string(who) + ": bad argument"; return NB2_ERR_INVALID; }
@@ -2577,9 +2577,19 @@ static int launch_imp(const nb2_model* m, int B, int k, const int32_t* body, con
     using R = decltype(r);
     const Nb2ModelDev<R>& M = fd_model_of<R>(m->variants[0]);
     size_t smem = 0;
-    const int slots = nb2_cfd_slots(M.nb, M.ndof, M.nslots, M.nfree, k * (a.point ? 3 : 6), 0, sizeof(R), kMaxSmem, &smem);
+    const int slots = nb2_cfd_slots(M.nb, M.ndof, M.nslots, M.nfree, k * (a.point ? 3 : 6), a.J[0] != nullptr, sizeof(R), kMaxSmem, &smem);
     if (!slots) { g_err = std::string(who) + ": the model's working set does not fit in shared memory"; return NB2_ERR_UNSUPPORTED; }
-    NB2_CUDA(nb2_imp_launch<R>(a.gvel != nullptr, slots, smem, (cudaStream_t)stream, M, B, a));
+    if (a.J[0]) {
+      NB2_CUDA(nb2_impj_launch<R>(slots, smem, (cudaStream_t)stream, M, B, a));
+      g_launches++;
+      // then k_imp's own forward rewrites vel_after and the impulses, so that they are nb2_impulse_dynamics's bit for bit (as for
+      // constrained forward dynamics: compiled into another kernel the same forward is not rounded identically)
+      size_t fsmem = 0;
+      const int fslots = nb2_cfd_slots(M.nb, M.ndof, M.nslots, M.nfree, k * (a.point ? 3 : 6), 0, sizeof(R), kMaxSmem, &fsmem);
+      NB2_CUDA(nb2_imp_launch<R>(0, fslots, fsmem, (cudaStream_t)stream, M, B, a));
+    } else {
+      NB2_CUDA(nb2_imp_launch<R>(a.gvel != nullptr, slots, smem, (cudaStream_t)stream, M, B, a));
+    }
     g_launches++;
     return NB2_OK;
   });
@@ -2603,6 +2613,20 @@ int nb2_impulse_dynamics_backward(const nb2_model* m, int B, const void* state, 
   ImpArgs a{};
   a.state = state; a.off = offsets; a.off_pw = offsets_per_world; a.wi = world_inertia;
   a.gvel = grad_vel; a.gimp = grad_impulses; a.gstate = grad_state; a.goff = grad_offsets; a.gI = grad_inertia;
+  return launch_imp(m, B, k, body, T_owner_from_node, point_contacts, restitution, damping, a, precision, stream, who);
+}
+int nb2_impulse_dynamics_jacobians(const nb2_model* m, int B, const void* state, int k, const int32_t* body, const double* T_owner_from_node,
+                                   const void* offsets, int offsets_per_world, int point_contacts, double restitution, double damping,
+                                   const double* world_inertia, void* vel_after, void* impulses, void* V_q, void* V_qdot, void* I_q,
+                                   void* I_qdot, int precision, void* stream) {
+  static const char* who = "nb2_impulse_dynamics_jacobians";
+  if (B > 0 && (!vel_after || !impulses || !V_q || !V_qdot || !I_q || !I_qdot)) {
+    g_err = std::string(who) + ": bad argument";
+    return NB2_ERR_INVALID;
+  }
+  ImpArgs a{};
+  a.state = state; a.off = offsets; a.off_pw = offsets_per_world; a.wi = world_inertia; a.vel = vel_after; a.imp = impulses;
+  a.J[0] = V_q; a.J[1] = V_qdot; a.J[2] = I_q; a.J[3] = I_qdot;
   return launch_imp(m, B, k, body, T_owner_from_node, point_contacts, restitution, damping, a, precision, stream, who);
 }
 int nb2_model_ndof(const nb2_model* m) { return m ? m->mf.ndof : -1; }

@@ -350,6 +350,16 @@ class DeviceModel:
                                                               int(off_per_world), int(point), float(restitution), float(damping), wi_ptr,
                                                               gvel_ptr, gimp_ptr, gstate_ptr, goff_ptr, ginertia_ptr, precision, stream))
 
+    def impulse_dynamics_jacobians_device(self, B, state_ptr, bodies, T12, off_ptr, off_per_world, point, restitution, damping, vel_ptr, imp_ptr,
+                                          jac_ptrs, stream, precision=FP32, wi_ptr=None):
+        """qdot_after, impulses and the dense Jacobians of impulse_dynamics_device (include/nb2.h nb2_impulse_dynamics_jacobians); jac_ptrs:
+        (V_q, V_qdot [B, n, n], I_q, I_qdot [B, m, n])."""
+        b = np.ascontiguousarray(bodies, np.int32)
+        T = np.ascontiguousarray(T12, np.float64)
+        _cabi.check(_cabi.lib().nb2_impulse_dynamics_jacobians(self.handle, B, state_ptr, len(b), b.ctypes.data, T.ctypes.data, off_ptr,
+                                                               int(off_per_world), int(point), float(restitution), float(damping), wi_ptr,
+                                                               vel_ptr, imp_ptr, *jac_ptrs, precision, stream))
+
     def contact_workspace_bytes(self, B):
         return int(_cabi.lib().nb2_contact_workspace_bytes(self.handle, B))
 

@@ -66,6 +66,8 @@ for B in (7, 203):
         (v2.sum() + i2.sum()).backward()
         v2, i2 = nb.impulse_dynamics(mw, st, bodies, point_contacts=True, restitution=1.0, damping=1e-3)
         (v2.sum() + i2.sum()).backward()
+        nb.impulse_dynamics_jacobians(mw, st, bodies, off, restitution=0.5, mass=mass.detach() * torch.tensor(mw.getMasses(), device="cuda"))
+        nb.impulse_dynamics_jacobians(mw, st, bodies[:2], point_contacts=True, restitution=1.0, damping=1e-3)
     sd = torch.tensor(s, device="cuda", dtype=torch.float64)
     nb.device_model_for(w).forward_dynamics(sd[:, :raw.ndof], sd[:, raw.ndof:], sd[:, raw.ndof:] * 10)
 torch.cuda.synchronize()
