@@ -284,6 +284,22 @@ int nb2_multiple_contact_inverse_dynamics_backward(const nb2_model* m, int B, in
                                                    const void* wrenches, const void* guess, const void* grad_tau, const void* grad_wrenches,
                                                    void* seed, void* grad_state, void* grad_next_vel, double* grad_inertia, void* grad_guess,
                                                    int precision, void* stream);
+/* Dense Jacobians of nb2_multiple_contact_inverse_dynamics (DESIGN.md §6s), in one launch.  Arguments as that call (no saved stream), whose
+ * tau [B, ndof] and wrenches [B, k, 6] it also writes, with m = 6k and row-major blocks in the arithmetic type, device memory:
+ *     T_q, T_qdot, T_next_vel [B, ndof, ndof],  T_guess [B, ndof, m] :  T_x[w, i, j] = d tau[w, i] / d x[w, j] ,
+ *     W_q, W_qdot, W_next_vel [B, m, ndof],     W_guess [B, m, m]    :  W_x[w, 6 i + c, j] = d wrenches[w, i, c] / d x[w, j] ,
+ * next_vel held fixed in the q and qdot blocks.  Row i of each block is nb2_multiple_contact_inverse_dynamics_backward with the seed e_i on
+ * that output (with k = 1 nb2_contact_inverse_dynamics_backward's), so free joints follow its conventions (position columns for the six
+ * stored coordinates, body-twist velocity columns) and the blocks equal the VJP's rows up to rounding; the free root's six rows of every
+ * T block are 0.  T_guess and W_guess may be NULL; with k = 1 they are 0 (the guess is not read).  tau and the wrenches are written by the
+ * forward of nb2_multiple_contact_inverse_dynamics itself (further launches on the stream), so they equal its outputs bit for bit.  Masses
+ * are held fixed.  Stateless, stream-ordered, nothing allocated, B = 0 only validates.  NB2_ERR_INVALID as
+ * nb2_multiple_contact_inverse_dynamics; NB2_ERR_UNSUPPORTED when the working set does not fit shared memory even at 4 row slots. */
+int nb2_multiple_contact_inverse_dynamics_jacobians(const nb2_model* m, int B, int ncontact, const int32_t* contact_body,
+                                                    const double* contact_point, const void* state, const void* next_vel,
+                                                    const double* world_inertia, const void* guess, void* tau, void* wrenches, void* T_q,
+                                                    void* T_qdot, void* T_next_vel, void* T_guess, void* W_q, void* W_qdot, void* W_next_vel,
+                                                    void* W_guess, int precision, void* stream);
 
 /* Joint-space mass matrix M(q) [B, ndof, ndof] (row-major) of B worlds at the positions pos [B, ndof]: the matrix the step inverts, in its
  * velocity coordinates (free joints: body twist, S = I6), block-diagonal over trees; contacts, limits, springs and damping are not part of

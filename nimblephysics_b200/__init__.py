@@ -7,7 +7,8 @@ from .modelspec import RawModel, CanonModel, flatten_world, compile_model, mass_
 from .timestep import timestep, TimestepLayer, contact_cache, reset_contact_cache, check_contact_status
 from .inverse_dynamics import (inverse_dynamics, InverseDynamicsLayer, contact_inverse_dynamics, ContactInverseDynamicsLayer,
                                multiple_contact_inverse_dynamics, MultipleContactInverseDynamicsLayer, forward_dynamics,
-                               ForwardDynamicsLayer, inverse_dynamics_jacobians, forward_dynamics_jacobians)
+                               ForwardDynamicsLayer, inverse_dynamics_jacobians, forward_dynamics_jacobians,
+                               contact_inverse_dynamics_jacobians, multiple_contact_inverse_dynamics_jacobians)
 from .mass_matrix import mass_matrix, inverse_mass_matrix, MassMatrixLayer, InverseMassMatrixLayer
 from .world_jacobian import world_jacobian, com_jacobian, WorldJacobianLayer, ComJacobianLayer
 from .world_jacobian import world_jacobian_deriv, com_jacobian_deriv, WorldJacobianDerivLayer, ComJacobianDerivLayer
@@ -21,7 +22,8 @@ from .rollout import rollout, rollout_fused, rollout_tape_bytes, multishot_rollo
 __all__ = ["World", "Skeleton", "BodyNode", "Joint", "Isometry3", "BoxShape", "SphereShape", "CapsuleShape",
            "loadWorld", "load_skeleton", "timestep", "TimestepLayer", "inverse_dynamics", "InverseDynamicsLayer", "contact_inverse_dynamics", "ContactInverseDynamicsLayer",
            "multiple_contact_inverse_dynamics", "MultipleContactInverseDynamicsLayer", "forward_dynamics", "ForwardDynamicsLayer",
-           "inverse_dynamics_jacobians", "forward_dynamics_jacobians", "mass_matrix", "inverse_mass_matrix", "MassMatrixLayer", "InverseMassMatrixLayer",
+           "inverse_dynamics_jacobians", "forward_dynamics_jacobians", "contact_inverse_dynamics_jacobians",
+           "multiple_contact_inverse_dynamics_jacobians", "mass_matrix", "inverse_mass_matrix", "MassMatrixLayer", "InverseMassMatrixLayer",
            "world_jacobian", "com_jacobian", "WorldJacobianLayer", "ComJacobianLayer",
            "world_jacobian_deriv", "com_jacobian_deriv", "WorldJacobianDerivLayer", "ComJacobianDerivLayer", "energy_and_momentum", "EnergyMomentumLayer", "inverse_dynamics_regressor", "energy_regressor", "constrained_forward_dynamics", "constrained_forward_dynamics_jacobians", "ConstrainedForwardDynamicsLayer", "impulse_dynamics", "impulse_dynamics_jacobians", "ImpulseDynamicsLayer", "rollout", "rollout_fused", "DeviceModel", "device_model_for", "RawModel", "CanonModel", "flatten_world", "compile_model", "mass_to_inertia"]
 from .lcp import solve_boxed_lcp_batch

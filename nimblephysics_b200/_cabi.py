@@ -192,6 +192,7 @@ def lib() -> ctypes.CDLL:
         L.nb2_contact_inverse_dynamics_backward.argtypes = [vp, ctypes.c_int, ctypes.c_int] + [vp] * 11 + [ctypes.c_int, vp]
         L.nb2_multiple_contact_inverse_dynamics.argtypes = [vp, ctypes.c_int, ctypes.c_int] + [vp] * 9 + [ctypes.c_int, vp]
         L.nb2_multiple_contact_inverse_dynamics_backward.argtypes = [vp, ctypes.c_int, ctypes.c_int] + [vp] * 15 + [ctypes.c_int, vp]
+        L.nb2_multiple_contact_inverse_dynamics_jacobians.argtypes = [vp, ctypes.c_int, ctypes.c_int] + [vp] * 16 + [ctypes.c_int, vp]
         L.nb2_mass_matrix.argtypes = [vp, ctypes.c_int, vp, vp, vp, ctypes.c_int, vp]
         L.nb2_inverse_mass_matrix.argtypes = [vp, ctypes.c_int, vp, vp, vp, ctypes.c_int, vp]
         L.nb2_mass_matrix_backward.argtypes = [vp, ctypes.c_int] + [vp] * 5 + [ctypes.c_int, vp]

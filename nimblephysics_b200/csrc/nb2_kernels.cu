@@ -30,6 +30,7 @@
 #include "nb2_reg.h"
 #include "nb2_cfd.h"
 #include "nb2_imp.h"
+#include "nb2_mcidj.h"
 
 static thread_local std::string g_err;
 static std::atomic<long long> g_launches{0};
@@ -2111,6 +2112,43 @@ int nb2_multiple_contact_inverse_dynamics_backward(const nb2_model* cm, int B, i
     if (rc) return rc;
     if (b.k == 1) return launch_cid<R>(m, b.c[0], B, false, S, nullptr, Wr, nullptr, Gt, Gw, nullptr, (R*)grad_state, st);
     return launch_mcid<R>(m, b, B, false, S, G, nullptr, Wr, nullptr, Gt, Gw, nullptr, nullptr, (R*)grad_state, st);
+  });
+}
+// Dense Jacobians (nb2_mcidj.cu): one warp per world on the create-time schedule, as many row slots as shared memory leaves room for.  Then
+// the forward of nb2_multiple_contact_inverse_dynamics rewrites tau and the wrenches, so that they are its outputs bit for bit (compiled
+// into another kernel the same forward is not rounded identically).
+int nb2_multiple_contact_inverse_dynamics_jacobians(const nb2_model* cm, int B, int ncontact, const int32_t* contact_body,
+                                                    const double* contact_point, const void* state, const void* next_vel,
+                                                    const double* world_inertia, const void* guess, void* tau, void* wrenches, void* T_q,
+                                                    void* T_qdot, void* T_next_vel, void* T_guess, void* W_q, void* W_qdot, void* W_next_vel,
+                                                    void* W_guess, int precision, void* stream) {
+  static const char* who = "nb2_multiple_contact_inverse_dynamics_jacobians";
+  nb2_model* m = const_cast<nb2_model*>(cm);
+  if (!m || B < 0 || !contact_body || !contact_point ||
+      (B > 0 && (!state || !next_vel || !tau || !wrenches || !T_q || !T_qdot || !T_next_vel || !W_q || !W_qdot || !W_next_vel))) {
+    g_err = std::string(who) + ": bad argument"; return NB2_ERR_INVALID;
+  }
+  return with_precision(precision, [&](auto r) -> int {
+    using R = decltype(r);
+    nb2::McidBodies<R> b;
+    if (int rc = mcid_bodies_of(m, ncontact, contact_body, contact_point, &b, who)) return rc;
+    const Nb2ModelDev<R>& M = model_of<R>(m->variants[0]);
+    size_t smem = 0;
+    const int slots = nb2_mcidj_slots(M.nb, M.ndof, M.nslots, M.nfree, b.k, sizeof(R), kMaxSmem, &smem);
+    if (!slots) { g_err = std::string(who) + ": the model's working set does not fit in shared memory"; return NB2_ERR_UNSUPPORTED; }
+    if (B == 0) return NB2_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    McidjArgs a{};
+    a.k = b.k; a.body = contact_body; a.point = contact_point;
+    a.state = state; a.next_vel = next_vel; a.guess = guess; a.wi = world_inertia; a.tau = tau; a.wrench = wrenches;
+    void* J[8] = {T_q, T_qdot, T_next_vel, T_guess, W_q, W_qdot, W_next_vel, W_guess};
+    for (int i = 0; i < 8; i++) a.J[i] = J[i];
+    NB2_CUDA(nb2_mcidj_launch<R>(slots, smem, st, M, B, a));
+    g_launches++;
+    int rc = launch_id<R>(m, B, LF_ID_FWD, (const R*)state, (const R*)next_vel, (R*)tau, nullptr, nullptr, nullptr, nullptr, nullptr, world_inertia, st);
+    if (rc) return rc;
+    if (b.k == 1) return launch_cid<R>(m, b.c[0], B, true, (const R*)state, (R*)tau, nullptr, (R*)wrenches, nullptr, nullptr, nullptr, nullptr, st);
+    return launch_mcid<R>(m, b, B, true, (const R*)state, (const R*)guess, (R*)tau, nullptr, (R*)wrenches, nullptr, nullptr, nullptr, nullptr, nullptr, st);
   });
 }
 }  // extern "C"

@@ -216,6 +216,16 @@ class DeviceModel:
                                                                                seed_ptr, gstate_ptr, gnext_ptr, ginertia_ptr, gguess_ptr,
                                                                                precision, stream))
 
+    def multiple_contact_inverse_dynamics_jacobians_device(self, B, bodies, points, state_ptr, next_vel_ptr, guess_ptr, tau_ptr, wrench_ptr,
+                                                           jac_ptrs, stream, precision=FP32, wi_ptr=None):
+        """tau, the wrenches and the dense Jacobians of multiple_contact_inverse_dynamics_device (include/nb2.h
+        nb2_multiple_contact_inverse_dynamics_jacobians); jac_ptrs: (T_q, T_qdot, T_next_vel [B, n, n], T_guess [B, n, 6k] or None,
+        W_q, W_qdot, W_next_vel [B, 6k, n], W_guess [B, 6k, 6k] or None)."""
+        k, b, p = self._contact_set(bodies, points)
+        _cabi.check(_cabi.lib().nb2_multiple_contact_inverse_dynamics_jacobians(self.handle, B, k, b.ctypes.data, p.ctypes.data, state_ptr,
+                                                                                next_vel_ptr, wi_ptr, guess_ptr, tau_ptr, wrench_ptr, *jac_ptrs,
+                                                                                precision, stream))
+
     def mass_matrix_device(self, B, pos_ptr, out_ptr, stream, precision=FP32, wi_ptr=None):
         """M(q) [B, n, n] (include/nb2.h nb2_mass_matrix): rows in the arithmetic type of `precision`."""
         _cabi.check(_cabi.lib().nb2_mass_matrix(self.handle, B, pos_ptr, wi_ptr, out_ptr, precision, stream))

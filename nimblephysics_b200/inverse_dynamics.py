@@ -50,6 +50,8 @@ per world, the World is left untouched).  The work is done by libnb2.so (include
 ``inverse_dynamics_jacobians`` and ``forward_dynamics_jacobians`` return the dense Jacobians of ``inverse_dynamics`` and
 ``forward_dynamics`` (with their outputs) in one launch (``nb2_inverse_dynamics_jacobians`` / ``nb2_forward_dynamics_jacobians``), for
 iLQR / DDP, Gauss-Newton or linearised-MPC users who need the matrices rather than products with one gradient.
+``contact_inverse_dynamics_jacobians`` and ``multiple_contact_inverse_dynamics_jacobians`` do the same for the two contact splits
+(``nb2_multiple_contact_inverse_dynamics_jacobians``).
 """
 from __future__ import annotations
 
@@ -67,6 +69,8 @@ _WHO_MULTI = "multiple_contact_inverse_dynamics()"
 _WHO_FD = "forward_dynamics()"
 _WHO_IDJ = "inverse_dynamics_jacobians()"
 _WHO_FDJ = "forward_dynamics_jacobians()"
+_WHO_CIDJ = "contact_inverse_dynamics_jacobians()"
+_WHO_MCIDJ = "multiple_contact_inverse_dynamics_jacobians()"
 MAX_CONTACT_BODIES = 4  # include/nb2.h NB2_MAX_CONTACT_BODIES
 
 
@@ -342,6 +346,14 @@ def contact_body_indices(world, bodies, who: str = _WHO_MULTI) -> list:
     return raw
 
 
+def _check_guesses(state, k, guesses, who):
+    """ValueError unless guesses is None or [B, k, 6] ([k, 6] for a 1-D state); nothing touches the device."""
+    if guesses is not None:
+        want = tuple(state.shape[:-1]) + (k, 6)
+        if tuple(guesses.shape) != want:
+            raise ValueError(f"{who}: wrench_guesses has shape {tuple(guesses.shape)}, expected {list(want)}")
+
+
 class MultipleContactInverseDynamicsLayer(torch.autograd.Function):
     """Multiple-contact inverse dynamics of the raw bodies `raw_bodies` (see contact_body_indices); guesses: [B, k, 6] / [k, 6] or None;
     world_inertia as for InverseDynamicsLayer.  Returns (tau, wrenches)."""
@@ -426,11 +438,86 @@ def multiple_contact_inverse_dynamics(world, state: torch.Tensor, next_vel: torc
     mass and the guesses."""
     raw_bodies = contact_body_indices(world, contact_bodies)
     _check_rows(world, state, next_vel, _WHO_MULTI)
-    if wrench_guesses is not None:
-        want = tuple(state.shape[:-1]) + (len(raw_bodies), 6)
-        if tuple(wrench_guesses.shape) != want:
-            raise ValueError(f"{_WHO_MULTI}: wrench_guesses has shape {tuple(wrench_guesses.shape)}, expected {list(want)}")
+    _check_guesses(state, len(raw_bodies), wrench_guesses, _WHO_MULTI)
     if mass is not None and mass.dim() == 2:
         return MultipleContactInverseDynamicsLayer.apply(world, state, next_vel, None, per_world_inertia(world, state, mass, _WHO_MULTI),
                                                          wrench_guesses, raw_bodies)
     return MultipleContactInverseDynamicsLayer.apply(world, state, next_vel, mass, None, wrench_guesses, raw_bodies)
+
+
+def _contact_jacobians(world, state, next_vel, raw_bodies, mass, guesses, who, guess_blocks):
+    """The body of the two contact Jacobian calls: (tau [B, n], wrenches [B, k, 6], T_q, T_qdot, T_next_vel [B, n, n], T_guess [B, n, k, 6],
+    W_q, W_qdot, W_next_vel [B, k, 6, n], W_guess [B, k, 6, k, 6]) in the state's dtype and device, the guess blocks None unless
+    guess_blocks.  Every argument is checked before any device work."""
+    _check_rows(world, state, next_vel, who)
+    _check_guesses(state, len(raw_bodies), guesses, who)
+    wi = per_world_inertia(world, state, mass, who) if mass is not None and mass.dim() == 2 else None
+    dm = set_shared_masses(world, mass, who) if mass is not None and wi is None else device_model_for(world)
+    if not torch.cuda.is_available():
+        raise RuntimeError(f"nimblephysics_b200.{who[:-2]} needs a CUDA device; there is no CPU fallback")
+    single = state.dim() == 1
+    s2 = state.detach().reshape(1, -1) if single else state.detach()
+    v2 = next_vel.detach().reshape(1, -1) if single else next_vel.detach()
+    dev = s2.device if s2.is_cuda else torch.device("cuda", torch.cuda.current_device())
+    rdt = torch.float64 if state.dtype == torch.float64 else torch.float32
+    sd = s2.to(device=dev, dtype=rdt).contiguous()
+    vd = v2.to(device=dev, dtype=rdt).contiguous()
+    B, n, k, cm = sd.shape[0], dm.ndof, len(raw_bodies), dm.cm
+    gd = guesses.detach().reshape(B, k, 6).to(device=dev, dtype=rdt).contiguous() if guesses is not None else None
+    bodies = [int(cm.body_owner[r]) for r in raw_bodies]
+    points = [cm.body_T[r][:3, 3].astype(float) for r in raw_bodies]  # each body's own origin in its owner's canonical frame
+    with torch.cuda.device(dev):
+        tau = torch.empty((B, n), dtype=rdt, device=dev)
+        w = torch.empty((B, k, 6), dtype=rdt, device=dev)
+        T = [torch.empty((B, n, n), dtype=rdt, device=dev) for _ in range(3)]
+        W = [torch.empty((B, k, 6, n), dtype=rdt, device=dev) for _ in range(3)]
+        Tg = torch.empty((B, n, k, 6), dtype=rdt, device=dev) if guess_blocks else None
+        Wg = torch.empty((B, k, 6, k, 6), dtype=rdt, device=dev) if guess_blocks else None
+        if B > 0:  # an empty batch has no rows to hand over (its data pointers may be NULL)
+            dm.multiple_contact_inverse_dynamics_jacobians_device(B, bodies, points, sd.data_ptr(), vd.data_ptr(), _ptr(gd), tau.data_ptr(),
+                                                                  w.data_ptr(), [_ptr(x) for x in T + [Tg] + W + [Wg]],
+                                                                  torch.cuda.current_stream().cuda_stream, FP64 if rdt == torch.float64 else FP32,
+                                                                  wi_ptr=_ptr(_word_major_inertia(dm, wi, B, dev)))
+    res = [tau, w] + T + [Tg] + W + [Wg]
+    if single:
+        res = [r[0] if r is not None else None for r in res]
+    return tuple(r.to(device=state.device, dtype=state.dtype) if r is not None else None for r in res)
+
+
+def contact_inverse_dynamics_jacobians(world, state: torch.Tensor, next_vel: torch.Tensor, contact_body, mass: Optional[torch.Tensor] = None):
+    """(tau, wrench, dtau_dq, dtau_dqdot, dtau_dnext_vel, dw_dq, dw_dqdot, dw_dnext_vel): (tau [B, n], wrench [B, 6]) =
+    contact_inverse_dynamics(world, state, next_vel, contact_body, mass), bit for bit, and their dense Jacobians, dtau_* [B, n, n] and
+    dw_* [B, 6, n], J[w, i, j] = d out_i / d x_j (the layout of torch.autograd.functional.jacobian), next_vel held fixed in the q and qdot
+    blocks.  From tau + J_c^T wrench = tau_ID and wrench = X*(root -> world) F_r (F_r: tau_ID's six free-root entries):
+
+        dtau_dx + J_c^T dw_dx = dtau_ID/dx   for x = qdot, next_vel  (J_c does not depend on them),   dtau_dnext_vel + J_c^T dw_dnext_vel = M / dt,
+
+    the root's six rows of every dtau block are 0, and the rows of dofs off the chain from the root to contact_body are
+    inverse_dynamics_jacobians's.  Row i is contact_inverse_dynamics's vector-Jacobian product with the seed e_i, so the blocks equal
+    autograd's Jacobian of that layer up to rounding; free joints follow its conventions (position columns for the six stored coordinates,
+    body-twist velocity columns).  Arguments, precision and masses as contact_inverse_dynamics (a 1-D state gives unbatched shapes); the
+    outputs carry no autograd history and there is no mass Jacobian.  ValueError before any device work as contact_inverse_dynamics."""
+    raw_body = contact_body_index(world, contact_body, _WHO_CIDJ)
+    out = _contact_jacobians(world, state, next_vel, [raw_body], mass, None, _WHO_CIDJ, False)
+    tau, w, Tq, Tqd, Tn, _, Wq, Wqd, Wn, _ = out
+    return (tau, w[..., 0, :], Tq, Tqd, Tn, Wq[..., 0, :, :], Wqd[..., 0, :, :], Wn[..., 0, :, :])
+
+
+def multiple_contact_inverse_dynamics_jacobians(world, state: torch.Tensor, next_vel: torch.Tensor, contact_bodies: Sequence,
+                                                mass: Optional[torch.Tensor] = None, wrench_guesses: Optional[torch.Tensor] = None):
+    """(tau, wrenches, dtau_dq, dtau_dqdot, dtau_dnext_vel, dtau_dguess, dw_dq, dw_dqdot, dw_dnext_vel, dw_dguess): (tau [B, n],
+    wrenches [B, k, 6]) = multiple_contact_inverse_dynamics(world, state, next_vel, contact_bodies, mass, wrench_guesses), bit for bit,
+    and their dense Jacobians in the layout of torch.autograd.functional.jacobian: dtau_dq, dtau_dqdot, dtau_dnext_vel [B, n, n],
+    dtau_dguess [B, n, k, 6], dw_dq, dw_dqdot, dw_dnext_vel [B, k, 6, n], dw_dguess [B, k, 6, k, 6]; next_vel held fixed in the q and qdot
+    blocks.  With J_i the contact Jacobians:
+
+        dtau_dx + sum_i J_i^T dw_i_dx = dtau_ID/dx   for x = qdot, next_vel ,     sum_i dw_i_dx = the one-body wrench block (x = q, qdot, next_vel),
+        sum_i dw_i_dg = 0 ,   dtau_dg = -sum_i J_i^T dw_i_dg ,
+
+    the root's six rows of every dtau block are 0, and rows of dofs off the union of the chains are inverse_dynamics_jacobians's.  With
+    one body the guess is not read and both guess blocks are 0.  Row i is the layer's vector-Jacobian product with the seed e_i, so the
+    blocks equal autograd's Jacobian of multiple_contact_inverse_dynamics up to rounding; free joints follow its conventions.  Arguments,
+    precision and masses as multiple_contact_inverse_dynamics (a 1-D state gives unbatched shapes); the outputs carry no autograd history
+    and there is no mass Jacobian.  ValueError before any device work as multiple_contact_inverse_dynamics."""
+    raw_bodies = contact_body_indices(world, contact_bodies, _WHO_MCIDJ)
+    return _contact_jacobians(world, state, next_vel, raw_bodies, mass, wrench_guesses, _WHO_MCIDJ, True)

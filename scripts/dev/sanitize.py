@@ -53,6 +53,8 @@ for B in (7, 203):
         nb.forward_dynamics(mw, st, tau, mass * torch.tensor(mw.getMasses(), device="cuda")).sum().backward()
         nb.inverse_dynamics_jacobians(mw, st, vn, mass.detach() * torch.tensor(mw.getMasses(), device="cuda"))
         nb.forward_dynamics_jacobians(mw, st, tau, mass.detach() * torch.tensor(mw.getMasses(), device="cuda"))
+        nb.multiple_contact_inverse_dynamics_jacobians(mw, st, vn, bodies, mass.detach() * torch.tensor(mw.getMasses(), device="cuda"), guess.detach())
+        nb.contact_inverse_dynamics_jacobians(mw, st, vn, bodies[0])
         sum(x.sum() for x in nb.energy_and_momentum(mw, st, mw.skeletons[0], mass * torch.tensor(mw.getMasses(), device="cuda"))).backward()
         nb.inverse_dynamics_regressor(mw, st, vn)
         nb.energy_regressor(mw, st)
